@@ -1,12 +1,13 @@
 #!/usr/bin/env python3
-"""bench.py -- H.x throughput of the B200-native hot path (driver contract; DESIGN.md section 6).
+"""bench.py -- H.x throughput of the CUDA hot path on H100 (DESIGN.md section 6).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload NAME] [--dtype c128|f64] [--secondary a,b|none]
+                    [--dump-outputs DIR]
     python bench.py --impl reference ...      # the reference's algorithm on the host cores (oracle port)
 
 A "step" is one matrix-vector product y <- H x over the whole basis of the workload.  The workload is
 ``heisenberg_square_6x6`` (BASELINE.json configs[4], the configuration the 1/2/4/8-GPU sweep of the metric is quoted
-on; it fits one B200) for EVERY N, so the driver's 1 -> 8 curve measures a problem that can scale; the other BASELINE
+on; it fits one H100) for EVERY N, so the 1 -> 8 curve measures a problem that can scale; the other BASELINE
 configs run as ``secondary`` entries of the same JSON line (a few products each, with their own parity figure).
 
   value        basis states / s with x, y resident in HBM: CUDA events on the launching stream around each product,
@@ -20,11 +21,15 @@ configs run as ``secondary`` entries of the same JSON line (a few products each,
                computeOffDiag on source i), using the reference's criterion |a-b| <= max(1e-14, 1e-12 max(|a|,|b|))
                (test/TestMatrixVectorProduct.chpl:15-20).  x follows the reference's recipe (input_for_matvec.py:8,31:
                RandomState(42), rand(N) - 0.5 in global sorted order; the imaginary part continues the stream).
-  roofline     algorithmic bytes of SURVEY.md 8(d) / duration of the dominant kernel against MEASURED_PEAKS.json, plus
-               what actually limits that kernel (measured DRAM traffic, issue-slot share) from the committed ncu
-               capture (profiles/ncu_constants.json).
+  roofline     algorithmic bytes of SURVEY.md 8(d) / duration of the dominant kernel against MEASURED_PEAKS.json when
+               present, else the H100 SXM data-sheet HBM3 bandwidth (3.35 TB/s; peak_kind says which).
   cpu_baseline the reference's algorithm restated in C (oracle/oracle.c, OpenMP, group elements as Benes networks) on
                a bounded slab of source rows, on this box's host cores.
+
+--dump-outputs DIR writes what the timed product computed in its last timed step: y at a fixed, seeded sample of rows
+(all rows when there are few), as DIR/rows.npy (global row indices), DIR/y_re.npy and DIR/y_im.npy (float64, 48 MB at
+most; a ".rank<r>" suffix per rank under torchrun).  x is fixed by the recipe, so two builds can be compared output for
+output.
 """
 from __future__ import annotations
 
@@ -52,6 +57,7 @@ DEFAULT_WORKLOAD = "heisenberg_square_6x6"   # BASELINE.json configs[4]: the sca
 SECONDARY = ["heisenberg_chain_24", "heisenberg_kagome_16", "heisenberg_chain_32_symm", "heisenberg_chain_36_symm"]
 X_RECIPE = "numpy RandomState(42): rand(N) - 0.5 in global sorted order (+ 1j (rand(N) - 0.5) for c128)"
 L2_NOTE = "GPU arm: 256 MB written between timed products (L2 flush); CPU arm: not applicable"
+DUMP_ROWS = 1 << 21      # rows of y written by --dump-outputs: 3 float64 arrays of 16 MB
 METRIC = "H.x basis states/s"
 
 
@@ -68,6 +74,7 @@ def parse_args():
     ap.add_argument("--sample-rows", type=int, default=2048, help="rows per rank checked against the oracle")
     ap.add_argument("--cpu-seconds", type=float, default=12.0, help="budget of the cpu_baseline leg")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write y of the last timed step (sampled rows) as .npy files")
     return ap.parse_args()
 
 
@@ -219,11 +226,13 @@ def count_terms_cpu(arm: CpuArm) -> int:
 # GPU arm
 # ------------------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """SM clock and throttle reasons sampled DURING the timed region (NVML, every DMV_CLOCK_PERIOD_MS = 5 ms)."""
+    """SM clock and throttle reasons sampled DURING the timed region (NVML, every DMV_CLOCK_PERIOD_MS = 5 ms), with the
+    card's name and power limit: a time measured on a power-capped card is a different number."""
 
     def __init__(self, index: int):
         self.index = index
         self.sm, self.reasons, self.sm_max = [], set(), None
+        self.gpu, self.power_limit_w = None, None
         self._stop = threading.Event()
         self._thread = None
 
@@ -240,6 +249,9 @@ class ClockSampler:
                     pass
             h = nv.nvmlDeviceGetHandleByIndex(idx)
             self.sm_max = float(nv.nvmlDeviceGetMaxClockInfo(h, nv.NVML_CLOCK_SM))
+            name = nv.nvmlDeviceGetName(h)
+            self.gpu = name.decode() if isinstance(name, bytes) else name
+            self.power_limit_w = nv.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
             bits = {"hw_slowdown": nv.nvmlClocksEventReasonHwSlowdown,
                     "hw_thermal_slowdown": nv.nvmlClocksEventReasonHwThermalSlowdown,
                     "sw_thermal_slowdown": nv.nvmlClocksEventReasonSwThermalSlowdown,
@@ -253,11 +265,13 @@ class ClockSampler:
                 self._stop.wait(1e-3 * float(os.environ.get("DMV_CLOCK_PERIOD_MS", "5")))
         except Exception as e:  # NVML missing: fall back to one nvidia-smi query
             try:
-                out = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=clocks.sm,clocks.max.sm",
+                out = subprocess.run(["nvidia-smi", f"--id={self.index}",
+                                      "--query-gpu=clocks.sm,clocks.max.sm,name,power.limit",
                                       "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=5)
-                a, b = [float(v) for v in out.stdout.strip().split(",")]
-                self.sm.append(a)
-                self.sm_max = b
+                a, b, name, limit = [v.strip() for v in out.stdout.strip().split(",")]
+                self.sm.append(float(a))
+                self.sm_max = float(b)
+                self.gpu, self.power_limit_w = name, float(limit)
             except Exception:
                 self.reasons.add(f"unsampled ({type(e).__name__})")
 
@@ -272,20 +286,12 @@ class ClockSampler:
         self._thread.join(timeout=10)
 
     def summary(self):
+        card = {"gpu": self.gpu, "power_limit_w": self.power_limit_w}
         if not self.sm:
-            return {"sm_mhz": None, "sm_max_mhz": self.sm_max, "reasons": sorted(self.reasons) or ["unsampled"]}
+            return {"sm_mhz": None, "sm_max_mhz": self.sm_max, "reasons": sorted(self.reasons) or ["unsampled"], **card}
         sm = sorted(self.sm)
         return {"sm_mhz": sm[len(sm) // 2], "sm_min_mhz": sm[0], "sm_max_mhz": self.sm_max,
-                "reasons": sorted(self.reasons), "samples": len(sm)}
-
-
-def ncu_constants(key: str):
-    """Per-launch figures of the dominant kernel from the committed ncu capture (profiles/ncu_constants.json)."""
-    path = os.path.join(ROOT, "profiles", "ncu_constants.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            return json.load(f).get(key)
-    return None
+                "reasons": sorted(self.reasons), "samples": len(sm), **card}
 
 
 def measured_peaks():
@@ -293,7 +299,7 @@ def measured_peaks():
     if os.path.exists(path):
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "datasheet (H100 SXM HBM3)"
 
 
 class Workload:
@@ -394,7 +400,8 @@ class Workload:
         self.op.close()
 
 
-def time_products(w: Workload, steps: int, warmup: int, flush, barrier, dist, local_rank: int, sample_clocks: bool):
+def time_products(w: Workload, steps: int, warmup: int, flush, barrier, dist, local_rank: int, sample_clocks: bool,
+                  keep_last: bool = False):
     import torch
     from distributed_matvec_b200 import _native as nat
     for _ in range(max(warmup, 3)):
@@ -417,6 +424,8 @@ def time_products(w: Workload, steps: int, warmup: int, flush, barrier, dist, lo
         w.product()
         ends[k].record()
     barrier()
+    if keep_last:          # y of the last timed step, before the products below overwrite it
+        w.y_last = w.y_dev.cpu().numpy()
     if sampler:
         sampler.__exit__()
     launches = nat.lib().dmv_launch_count() - launches0
@@ -445,33 +454,37 @@ def time_products(w: Workload, steps: int, warmup: int, flush, barrier, dist, lo
     return float(t[0]), float(t[1]), kernel_ms, int(launches), (sampler.summary() if sampler else None)
 
 
-def roofline_of(w: Workload, kernel_ms: float, clocks: dict | None, dtype: str) -> dict:
+def roofline_of(w: Workload, kernel_ms: float) -> dict:
     peak, peak_kind = measured_peaks()
     bytes_alg = w.n_local * (8 + 2 * w.E) + w.nnz_local * (8 + 2 * w.E)
     achieved = bytes_alg / (kernel_ms * 1e-3) / 1e9
     kernel = w.kernel_name()
-    const = ncu_constants(f"{kernel}:{w.name}:{dtype}") if w.world == 1 else None
     out = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-           "traffic": const.get("dram_bytes") if const else None, "peak_kind": peak_kind, "kernel": kernel,
+           "peak_kind": peak_kind, "kernel": kernel,
            "kernel_ms": kernel_ms, "table_refill_ms": getattr(w, "table_refill_ms", 0.0),
            "algorithmic_bytes": int(bytes_alg),
            "model": "SURVEY 8(d): N (8 + 2E) + nnz (8 + 2E) bytes per product"}
     limiter = {}
-    if const:
-        if const.get("dram_bytes"):
-            limiter["dram_frac_of_peak"] = const["dram_bytes"] / (kernel_ms * 1e-3) / 1e9 / peak
-            limiter["traffic_over_algorithmic"] = const["dram_bytes"] / bytes_alg
-        if const.get("warp_instructions") and clocks and clocks.get("sm_mhz"):
-            limiter["issue_slot_frac"] = const["warp_instructions"] / (kernel_ms * 1e-3 * 148 * 4 * clocks["sm_mhz"] * 1e6)
-        limiter["source"] = const.get("source")
-        for k in ("l1_wavefront_pct", "note"):
-            if k in const:
-                limiter[k] = const[k]
     if w.group_order > 1:
         limiter["group_order"] = w.group_order
         limiter["orbit_elements_per_s"] = (w.nnz_local + w.n_local) * w.group_order / (kernel_ms * 1e-3)
     out["limiter"] = limiter
     return out
+
+
+def dump_outputs(w: Workload, out_dir: str):
+    """y of the last timed step at a fixed, seeded sample of this rank's rows (global indices), as float64 arrays."""
+    y = w.y_last
+    pick = np.arange(y.shape[0])
+    if y.shape[0] > DUMP_ROWS:
+        pick = np.sort(np.random.default_rng(20240611).choice(y.shape[0], size=DUMP_ROWS, replace=False))
+    suffix = f".rank{w.rank}" if w.world > 1 else ""
+    os.makedirs(out_dir, exist_ok=True)
+    ys = y[pick]
+    np.save(os.path.join(out_dir, f"rows{suffix}.npy"), w.local_rows[pick].astype(np.float64))
+    np.save(os.path.join(out_dir, f"y_re{suffix}.npy"), np.ascontiguousarray(ys.real, dtype=np.float64))
+    np.save(os.path.join(out_dir, f"y_im{suffix}.npy"), np.ascontiguousarray(ys.imag if np.iscomplexobj(ys) else
+                                                                               np.zeros_like(ys), dtype=np.float64))
 
 
 def main():
@@ -498,7 +511,7 @@ def main():
         torch.cuda.synchronize()
 
     cplx = args.dtype == "c128"
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")  # > 50 MB L2 of an H100
     check_threads = max(1, host_threads() // world)
 
     w = Workload(args.workload, cplx, world, rank, local_rank)
@@ -509,7 +522,9 @@ def main():
     assert n_total == w.n_total
 
     ms_per_step, ms_best, kernel_ms, launches, clocks = time_products(w, args.steps, args.warmup, flush, barrier, dist,
-                                                                     local_rank, True)
+                                                                     local_rank, True, keep_last=bool(args.dump_outputs))
+    if args.dump_outputs:
+        dump_outputs(w, args.dump_outputs)
 
     # ---- e2e: pinned host x -> public call -> host y; wall clock around the blocking call
     for _ in range(2):
@@ -555,7 +570,7 @@ def main():
                 "h2d_bytes_per_step": int(w.n_local * w.E), "d2h_bytes_per_step": int(w.n_local * w.E),
                 "stages_ms": stage},
         "gpu_launches": int(launches),
-        "roofline": roofline_of(w, kernel_ms, clocks, args.dtype),
+        "roofline": roofline_of(w, kernel_ms),
         "clocks": clocks,
     }
 

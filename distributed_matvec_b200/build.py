@@ -1,4 +1,4 @@
-"""Build recipe of libdmv_b200.so: nvcc for sm_100a, in-tree (the .so travels to the GPU box)."""
+"""Build recipe of libdmv_b200.so: nvcc for sm_90a (H100), in-tree next to the package."""
 from __future__ import annotations
 
 import os
@@ -11,7 +11,8 @@ LIB = os.path.join(HERE, "libdmv_b200.so")
 SOURCES = ["dmv_kernels.cu", "dmv_gather.cu", "dmv_solver.cu", "dmv_group.cu", "dmv_api.cu", "dmv_exchange.cu",
            "dmv_lanczos.cu", "dmv_plugin.cu"]
 HEADERS = ["dmv_device.cuh", "dmv_host.h", "dmv_context.h", os.path.join("..", "..", "include", "dmv_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = "arch=compute_90a,code=sm_90a"
+NVCC_FLAGS = ["-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "--expt-relaxed-constexpr"]
 
 
@@ -45,7 +46,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         if p.returncode != 0:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
     tmp = f"{LIB}.tmp{os.getpid()}"   # link into a private file, then rename: a reader never sees a half-written library
-    link = ["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", tmp, *objs, "-lcudart", "-ldl"]
+    link = ["nvcc", "-gencode", ARCH, "-shared", "-o", tmp, *objs, "-lcudart", "-ldl"]
     try:
         subprocess.run(link, check=True)
         os.replace(tmp, LIB)

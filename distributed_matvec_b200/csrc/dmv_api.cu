@@ -1011,7 +1011,7 @@ int dmv_set_option(dmv_context *ctx, const char *name, int64_t value) {
     if (value < -1 || value > 1) throw std::runtime_error("rows_batch: -1 auto / 1 k_rows_batch for batched products, 0 vector by vector");
     ctx->opt_rows_batch = (int)value;
   } else if (key == "rows_ctas") {
-    ctx->opt_rows_ctas = (value == 2 || value == 4) ? (int)value : 3;
+    ctx->opt_rows_ctas = (value == 3 || value == 4) ? (int)value : 2;
     if (ctx->global) ctx->global->opt_rows_ctas = ctx->opt_rows_ctas;
   } else if (key == "rows_index") {
     if (value < -1 || value > 1) throw std::runtime_error("rows_index: -1 auto / 0 open-addressing table, 1 dense index (perfect hash)");
@@ -1134,7 +1134,7 @@ int dmv_basis_build(dmv_context *ctx) {
   const uint64_t first_rank = fixed ? fixed_hamming_rank(lo) : lo;
   const uint64_t last_rank = fixed ? fixed_hamming_rank(hi) : hi;
   const uint64_t total = last_rank - first_rank + 1;
-  uint64_t chunk_len = total / (148ull * 128 * 16);
+  uint64_t chunk_len = total / (132ull * 128 * 16);
   chunk_len = std::min<uint64_t>(std::max<uint64_t>(chunk_len, 64), 4096);
   const int64_t n_chunks = (int64_t)((total + chunk_len - 1) / chunk_len);
   std::vector<uint64_t> h_first((size_t)n_chunks), h_last((size_t)n_chunks);
@@ -1360,8 +1360,8 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
     // (host vectors -- what PRIMME hands over -- are staged a batch at a time)
     const int per = 6 / elt;
     const bool on_host = !is_device_pointer(x);
-    // (a batch costs 1.5 - 1.6 single products on the 6x6 square -- 64-byte buckets, one request per lane in flight:
-    // profiles/r02_rows_batch_6x6.md -- so it pays from two vectors on)
+    // (a batch shares the orbit minimum and the look-up of a term between its vectors -- 64-byte buckets, one request
+    // per lane in flight -- so it pays from two vectors on)
     while ((num_vectors - k) * elt >= ctx->opt_rows_batch_min && num_vectors - k >= 2) {
       const int nv = std::min(per, num_vectors - k);
       const void *xk = xb + (size_t)k * vec_bytes;

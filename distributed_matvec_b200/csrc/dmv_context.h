@@ -191,15 +191,15 @@ struct dmv_context {
   // hash table over this context's representatives (see table_slot in dmv_device.cuh)
   bool rows_ok = false;
   int opt_rows = -1;        // -1 auto (k_rows when it applies), 0 the queued k_pull
-  int opt_rows_ctas = 3;    // k_rows: resident CTAs per SM: 3 (80 registers, default) | 2 (122 registers) | 4 (64 registers)
+  int opt_rows_ctas = 2;    // k_rows: resident CTAs per SM: 2 (122 registers, default) | 3 (80 registers) | 4 (64 registers)
   int opt_gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
                             // (measured slower), 2 per-lane walk from the bottom bit (round 1)
   DevBuf<unsigned char> d_table;
   DevBuf<unsigned char> d_mph_blocks, d_dense;   // dense index: perfect-hash blocks, dense table of (key, value) slots
   PerfectHash mph{};
   bool dense_index = false;
-  int opt_rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (measured slower:
-                             // profiles/r02_rows_pipelines.md)
+  int opt_rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (kept for reference:
+                             // the dense table is still many times L2, so a look-up still costs a random sector)
   DevBuf<uint32_t> d_slot_of;
   uint32_t table_slots = 0;
   int table_elt = 0;        // element type the slots are laid out for (0: not built)

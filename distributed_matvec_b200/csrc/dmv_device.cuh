@@ -1,4 +1,4 @@
-// dmv_device.cuh -- device-side data structures and helpers of the H.x hot path (sm_100a).
+// dmv_device.cuh -- device-side data structures and helpers of the H.x hot path (sm_90a).
 //
 // Everything here is integer / bit-twiddling + sparse FP64 FMA: no tensor cores (north_star).
 #pragma once
@@ -253,10 +253,10 @@ __device__ __forceinline__ int64_t locate(const StateIndex &ix, uint64_t key) {
 // array + directory needs  directory -> several probes -> norm -> x  dependent loads per term, and orbit minima
 // cluster at small values, which unbalances any directory over the top bits; here a term costs the 32-byte sector of
 // its bucket.  The values are refreshed once per product
-// (k_table_fill: x[i] * norm[i] at slot_of[i]).  180 GB of HBM pays for the 64 .. 256 bytes per state.
-// A bucket is ONE 32-byte sector, fetched with one 256-bit load: HBM3e serves about 30 G random sectors per second
-// whatever their size up to 64 bytes (tools/random_access.cu, profiles/r02_random_access.md), so the look-up costs
-// what its sectors cost.  A state goes to the first bucket from its home with a free slot; a look-up that finds its
+// (k_table_fill: x[i] * norm[i] at slot_of[i]).  The table takes 64 .. 256 bytes per state (fewer when
+// free memory is short: ensure_table).  A bucket is ONE 32-byte sector, fetched with two independent 128-bit loads:
+// random look-ups are bound by the rate at which HBM serves random sectors (tools/random_access.cu measures it), so
+// the look-up costs what its sector costs.  A state goes to the first bucket from its home with a free slot; a look-up that finds its
 // bucket taken by other states moves on to the next one (7 % of the look-ups for complex128, 2 % for float64).
 //   complex128: bucket = one slot  { key, spare, re, im },            8 buckets per state
 //   float64:    bucket = two slots { key0, key1, value0, value1 },    2 buckets per state
@@ -269,12 +269,12 @@ __host__ __device__ __forceinline__ uint32_t table_slot(uint64_t key, uint32_t n
 
 // ---------------------------------------------------------------------------------------------
 // Dense index for k_rows: a two-level perfect hash over the representatives.  The open-addressing table above is bound by
-// the rate at which HBM serves RANDOM sectors, and that rate falls from ~70 G/s to ~30 G/s as the table grows from 2 x L2
-// to gigabytes (profiles/r02_random_access.md); a perfect hash needs no empty slots, so the table of (key, value) slots
+// the rate at which HBM serves RANDOM sectors, and that rate falls as the table grows from a few times
+// the L2 to gigabytes; a perfect hash needs no empty slots, so the table of (key, value) slots
 // shrinks from 256 N to 32 N bytes.  Level l is an array of 32-byte blocks { w0, w1, w2, prefix }: 192 bits of which bit
 // p is set iff exactly ONE state hashes to p at this level (then it owns the slot prefix + popcount of the set bits
 // before p in the block); states that collide at level 0 try level 1, the few per cent left over live in the
-// open-addressing table.  Both blocks of a look-up are requested together (two 256-bit loads that hit L2: 5 bits per
+// open-addressing table.  Both blocks of a look-up are requested together (two 32-byte blocks that hit L2: 5 bits per
 // state), the slot one pipeline step later.
 // ---------------------------------------------------------------------------------------------
 struct PerfectHash {

@@ -89,8 +89,8 @@ void setup_exchange(dmv_context *ctx) {
 }
 
 // -------------------------------------------------------------------------------------------------
-// Replicated-x product.  With 180 GB of HBM per GPU every basis of BASELINE.json fits on ONE device many times
-// over, so for operators k_gather applies to, the ranks can trade the reference's record exchange (24 bytes per
+// Replicated-x product.  With 80 GB of HBM per GPU every basis of BASELINE.json fits on ONE device (the set-up below
+// checks the free memory), so for operators k_gather applies to, the ranks can trade the reference's record exchange (24 bytes per
 // off-diagonal term over NVLink, DMV:313-436) for one all-gather of x (E bytes per STATE): every rank keeps the
 // whole sorted basis (a single-rank twin context), gathers x from all ranks into slots of equal size, and computes
 // ITS rows by the atomics-free row traversal.  The hash partition of x, y and the representatives -- the layout the

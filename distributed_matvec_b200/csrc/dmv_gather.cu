@@ -7,7 +7,7 @@
 // The same arithmetic as localDiagonal + computeOffDiag + localProcess (reference
 // src/DistributedMatrixVector.chpl:36-127), but every y element is produced by ONE lane and stored once:
 // no (beta, c) records, no shared-memory queue, no FP64 atomics (the L2 atomic unit is the busiest unit of
-// the scatter form, profiles/r01_push_chain24_c128_final.md), and the result is bit-reproducible.
+// the scatter form), and the result is bit-reproducible.
 // One lane owns one row: 8/16-byte coalesced loads of sigma_b and x_b, the emit mask of all groups from a few
 // masked shifts (BpWord), then a walk over the set bits two at a time -- two index look-ups and two x gathers
 // in flight per lane.  With <= 32 sites and <= 32 groups the whole row runs in 32-bit registers (NARROW).
@@ -237,10 +237,9 @@ __global__ void __launch_bounds__(kThreads) k_gather(const KernelParams p) {
       if (S == 1 && p.gather_walk == 1) {
         // GROUP-MAJOR walk (option "gather_walk" = 1), warp-uniform, four groups per trip: all 32 lanes handle the same
         // group at the same time.  For a fixed flip mask consecutive rows map to (nearly) consecutive indices, so the 32
-        // gathers of a group fall into a few 128-byte lines instead of 32.  Measured (profiles/r02_gather_walks.md): the
-        // L1 wavefront share drops from 81 % to 45 % as intended, but every lane now walks all emitting groups of the
-        // warp (24 instead of its own ~12.5): 35 % more instructions, and the kernel ends up SLOWER (0.150 vs 0.131 ms
-        // on chain_24 c128).  Kept for reference; the per-lane walk below is the default.
+        // gathers of a group fall into a few 128-byte lines instead of 32.  But every
+        // lane now walks all emitting groups of the warp (24 instead of its own ~12.5 on chain_24): 35 % more
+        // instructions, which cost more than the fewer L1 wavefronts save.  Kept for reference; the per-lane walk below is the default.
         W any;
         if constexpr (sizeof(W) == 4) any = __reduce_or_sync(0xffffffffu, mask);
         else {
@@ -363,7 +362,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -475,7 +474,7 @@ __global__ void __launch_bounds__(256) k_push_block(const T *__restrict__ x, int
     for (int q = 0; q < num_ranks; ++q) peer_slot[q][i] = v;
   }
   // one system-scope fence per CTA, after the CTA barrier (cumulative: it covers the stores of the whole CTA); a fence in
-  // every warp costs ~0.7 ms per product on eight GPUs (measured: profiles/r02_scaling.md)
+  // every warp serialises every warp of the CTA behind a system-scope fence
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence_system();

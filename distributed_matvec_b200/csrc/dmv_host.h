@@ -113,7 +113,7 @@ struct KernelParams {
   // `table` then only holds the few per cent of the states the two levels could not place
   PerfectHash mph;
   const void *dense;
-  int32_t rows_ctas;           // k_rows / k_rows_batch: resident CTAs per SM the kernel is compiled for (3 default | 2 | 4)
+  int32_t rows_ctas;           // k_rows / k_rows_batch: resident CTAs per SM the kernel is compiled for (2 default | 3 | 4)
 };
 
 // launchers (dmv_kernels.cu)

@@ -1,4 +1,4 @@
-// dmv_kernels.cu -- hand-written sm_100a kernels of the distributed matrix-free H.x product.
+// dmv_kernels.cu -- hand-written sm_90a kernels of the distributed matrix-free H.x product.
 //
 //   k_generate   : diagonal + off-diagonal term generation (BatchedOperator.computeOffDiag, reference
 //                  src/BatchedOperator.chpl:82-213) fused with the destination hash (localeIdxOf,
@@ -853,20 +853,27 @@ __global__ void __launch_bounds__(kThreads) k_pull(const KernelParams p) {
 // orbit minimum in registers (canonical form, dmv_device.cuh), then ONE dependent memory access -- the slot of the
 // representative in a hash table that carries the scaled vector element (table_slot) -- and that access is software
 // pipelined: the slot of term j is requested right after its orbit minimum and consumed after the orbit minimum of
-// term j + 2, so its latency hides behind ~10^3 integer instructions of the same lane.  (Deeper pipelines were measured
-// and are slower -- four requests per lane through prefetch.global.L2 or through cp.async into shared memory: 58 / 46 ms
-// against 29 ms on the 6x6 square; the look-ups are bound by the rate of random 64-byte requests the memory system takes,
-// not by their latency: profiles/r02_rows_pipelines.md.)
+// term j + 2, so its latency hides behind ~10^3 integer instructions of the same lane.  (Deeper pipelines -- four requests per
+// lane through prefetch.global.L2 or through cp.async into shared memory -- were slower: the look-ups are bound by the
+// rate of random requests the memory system takes, not by their latency.)
 // -------------------------------------------------------------------------------------------------
-// one bucket = two slots (layout: table_slot in dmv_device.cuh); all loads of a bucket are independent
-// 256-bit loads (sm_100: LDG.E.256), not allocated in L1: a bucket is touched once per product, and 50 GB of them
-// streaming through L1 would evict the small tables the orbit minimum reads from global memory
+// one bucket = two slots (layout: table_slot in dmv_device.cuh); a bucket is one 32-byte sector, read as two independent
+// 128-bit loads (the widest global load sm_90 has; both halves of the sector are in flight together), not allocated in
+// L1: a bucket is touched once per product, and gigabytes of them streaming through L1 would evict the small tables the
+// orbit minimum reads from global memory
 __device__ __forceinline__ void load256(const unsigned char *q, uint64_t &a, uint64_t &b, uint64_t &c, uint64_t &d) {
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(q));
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(q));
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u64 {%0, %1}, [%2+16];" : "=l"(c), "=l"(d) : "l"(q));
 }
 // the same through L1 (perfect-hash blocks: a few bits per state, read by every look-up)
 __device__ __forceinline__ void load256_cached(const unsigned char *q, uint64_t &a, uint64_t &b, uint64_t &c, uint64_t &d) {
-  asm volatile("ld.global.nc.v4.u64 {%0, %1, %2, %3}, [%4];" : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(q));
+  asm volatile("ld.global.nc.v2.u64 {%0, %1}, [%2];" : "=l"(a), "=l"(b) : "l"(q));
+  asm volatile("ld.global.nc.v2.u64 {%0, %1}, [%2+16];" : "=l"(c), "=l"(d) : "l"(q));
+}
+// one 32-byte sector written whole by one thread (two 128-bit stores): a full-sector write needs no read-modify-write
+__device__ __forceinline__ void store256(unsigned char *q, uint64_t a, uint64_t b, uint64_t c, uint64_t d) {
+  asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(q), "l"(a), "l"(b) : "memory");
+  asm volatile("st.global.v2.u64 [%0+16], {%1, %2};" ::"l"(q), "l"(c), "l"(d) : "memory");
 }
 template <bool CE>
 __device__ __forceinline__ void bucket_load(const unsigned char *__restrict__ table, uint32_t b, ulonglong2 &keys,
@@ -1070,10 +1077,9 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
 // (reference src/Diagonalize.chpl:134-162: PRIMME hands `blockSize` vectors to one matvec call).  The orbit minimum and the
 // look-up of a term are shared by the vectors: one bucket = 64 bytes = { key, d[0..5], spare }, d = the scaled elements of
 // the vectors at that state (three (re, im) pairs or six reals: the operator is real, so every double is treated alike),
-// fetched with two independent 256-bit loads.  One request per lane in flight, consumed after the orbit minimum of the
+// fetched as two 32-byte halves (load256 each).  One request per lane in flight, consumed after the orbit minimum of the
 // NEXT term; a bucket taken by another state continues with the next bucket through the same slot.
-// Cost model: one 64-byte request per term (17.8 G/s for tables >> L2, profiles/r02_random_access.md) against one 32-byte
-// request per term AND vector in k_rows.
+// Cost model: one 64-byte request per term against one 32-byte request per term AND vector in k_rows.
 // -------------------------------------------------------------------------------------------------
 template <int TK, int CTAS>
 __global__ void __launch_bounds__(kThreads, CTAS) k_rows_batch(const KernelParams p) {
@@ -1201,7 +1207,7 @@ __global__ void k_table_insert(const uint64_t *__restrict__ reps, int64_t n, uns
 }
 
 // per product: value of slot_of[i] = x[src(i)] * norm[i]   (src(i) = pos ? pos[i] : i).  complex128 rewrites the WHOLE
-// 32-byte slot {key, spare, re, im} with one 256-bit store: a full-sector write needs no read-modify-write in DRAM.
+// 32-byte slot {key, spare, re, im} with store256: a full-sector write needs no read-modify-write in DRAM.
 // slot_of[i] < 2^31: slot of the dense table (perfect hash); else 0x80000000 | slot of the open-addressing table.
 template <bool CE>
 __global__ void k_table_fill(int64_t n, const void *__restrict__ x, const double *__restrict__ norms,
@@ -1219,7 +1225,7 @@ __global__ void k_table_fill(int64_t n, const void *__restrict__ x, const double
       const double2 v = __ldg(reinterpret_cast<const double2 *>(x) + src);
       const uint64_t re = (uint64_t)__double_as_longlong(v.x * nrm), im = (uint64_t)__double_as_longlong(v.y * nrm);
       unsigned char *q = in_table ? table + (size_t)(s >> 1) * 32 : dense + (size_t)s * 32;
-      asm volatile("st.global.v4.u64 [%0], {%1, %2, %3, %4};" ::"l"(q), "l"(key), "l"(0ull), "l"(re), "l"(im) : "memory");
+      store256(q, key, 0ull, re, im);
     } else {
       const double v = __ldg(reinterpret_cast<const double *>(x) + src) * nrm;
       if (in_table) *reinterpret_cast<double *>(table + (size_t)(s >> 1) * 32 + 16 + 8 * (s & 1)) = v;
@@ -1229,7 +1235,7 @@ __global__ void k_table_fill(int64_t n, const void *__restrict__ x, const double
 }
 
 // per batched product: bucket slot_of[i] / 2 of the 64-byte table <- { key, x_v[i] * norm[i] for the vectors v, 0 ... }
-// (two 256-bit stores = two full sectors)
+// (two store256 = two full sectors)
 __global__ void k_table_fill_batch(int64_t n, int nd, int elt, const double *__restrict__ x, int64_t stride,
                                    const double *__restrict__ norms, const uint32_t *__restrict__ slot_of,
                                    const uint64_t *__restrict__ reps, unsigned char *table) {
@@ -1245,8 +1251,8 @@ __global__ void k_table_fill_batch(int64_t n, int nd, int elt, const double *__r
     }
     unsigned char *q = table + (size_t)(__ldg(slot_of + i) >> 1) * 64;
     const uint64_t key = __ldg(reps + i);
-    asm volatile("st.global.v4.u64 [%0], {%1, %2, %3, %4};" ::"l"(q), "l"(key), "l"(d[0]), "l"(d[1]), "l"(d[2]) : "memory");
-    asm volatile("st.global.v4.u64 [%0], {%1, %2, %3, %4};" ::"l"(q + 32), "l"(d[3]), "l"(d[4]), "l"(d[5]), "l"(0ull) : "memory");
+    store256(q, key, d[0], d[1], d[2]);
+    store256(q + 32, d[3], d[4], d[5], 0ull);
   }
 }
 
@@ -1506,7 +1512,7 @@ int choose_row_split(int64_t rows, int n_groups) {
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  if (n <= 0) n = 148;
+  if (n <= 0) n = 132;
   int s = 1;
   while (s < 32 && 2 * s <= n_groups && (rows * s) / 32 < (int64_t)n * 16) s *= 2;
   return s;
@@ -1516,7 +1522,7 @@ int planned_grid(int64_t rows, int row_split) {   // grid of the planned launche
   int dev = 0, n = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  if (n <= 0) n = 148;
+  if (n <= 0) n = 132;
   const int rows_per_tile = 32 / (row_split > 1 ? row_split : 1);
   int64_t b = ((rows + rows_per_tile - 1) / rows_per_tile + kWarps - 1) / kWarps;
   if (b < 1) b = 1;
@@ -1531,7 +1537,7 @@ int sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -1550,7 +1556,7 @@ void launch_generate_t(const KernelParams &p, cudaStream_t stream) {
   if (per_sm < 1) per_sm = 1;
   const int rpt = 32 / (p.row_split > 1 ? p.row_split : 1);
   const int64_t tiles = (p.row_end - p.row_begin + rpt - 1) / rpt;
-  // grid = a whole number of waves of resident CTAs (148 SMs x per_sm), or fewer when the work is small
+  // grid = a whole number of waves of resident CTAs (SMs x per_sm), or fewer when the work is small
   const int blocks = p.grid_blocks > 0 ? p.grid_blocks : grid_for(tiles, kWarps, sm_count() * per_sm);
   kernel<<<blocks, kThreads, L.total, stream>>>(p);
   DMV_CUDA_CHECK(cudaGetLastError());
@@ -1636,10 +1642,10 @@ void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
     else launch_rows_t<CE, 0, true>(p, stream);
     return;
   }
-  if (p.rows_ctas == 2) {   // two CTAs per SM: 122 registers, nothing spills
-    if (k == 6) launch_rows_t<CE, 6, false>(p, stream);
-    else if (k == 4) launch_rows_t<CE, 4, false>(p, stream);
-    else launch_rows_t<CE, 0, false>(p, stream);
+  if (p.rows_ctas == 3) {   // three CTAs per SM: 80 registers, a few words of the pipeline state spill
+    if (k == 6) launch_rows_t<CE, 6, false, 3>(p, stream);
+    else if (k == 4) launch_rows_t<CE, 4, false, 3>(p, stream);
+    else launch_rows_t<CE, 0, false, 3>(p, stream);
     return;
   }
   if (p.rows_ctas == 4) {   // four CTAs per SM: 64 registers
@@ -1647,11 +1653,11 @@ void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
     else launch_rows_t<CE, 0, false, 4>(p, stream);
     return;
   }
-  // default: three CTAs per SM (80 registers; a few words of the pipeline state spill, 24 warps per SM more than pay for it:
-  // 6x6 24.9 -> 22.3 ms, chain_36_symm 53.5 -> 44.0 ms, profiles/r02_rows_pipelines.md)
-  if (k == 6) launch_rows_t<CE, 6, false, 3>(p, stream);
-  else if (k == 4) launch_rows_t<CE, 4, false, 3>(p, stream);
-  else launch_rows_t<CE, 0, false, 3>(p, stream);
+  // default: two CTAs per SM (122 registers, nothing spills).  On an H100 (400 W, L2 flushed between products) three CTAs
+  // tie on the 6x6 square (31.1 / 31.5 ms against 31.5 ms, complex128) and lose on chain_36_symm (79.4 ms against 71.3)
+  if (k == 6) launch_rows_t<CE, 6, false>(p, stream);
+  else if (k == 4) launch_rows_t<CE, 4, false>(p, stream);
+  else launch_rows_t<CE, 0, false>(p, stream);
 }
 }  // namespace
 
@@ -1682,7 +1688,7 @@ void launch_rows_batch(const KernelParams &p, cudaStream_t stream) {
   const OrbitProgram &o = p.orbit;
   const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
   // two CTAs per SM (120-128 registers: the eight words of the request stay in registers; at 80 registers part of them
-  // spills and the batch is 4 % slower: profiles/r02_rows_batch_6x6.md)
+  // spills)
   if (k == 6) launch_rows_batch_t<6, 2>(p, stream);
   else if (k == 4) launch_rows_batch_t<4, 2>(p, stream);
   else launch_rows_batch_t<0, 2>(p, stream);

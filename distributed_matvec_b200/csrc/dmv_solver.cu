@@ -103,7 +103,7 @@ int blocks_for(int64_t n) {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   int64_t b = (n + kThreads - 1) / kThreads;
   if (b < 1) b = 1;
   if (b > (int64_t)sms * 8) b = (int64_t)sms * 8;

@@ -1,5 +1,5 @@
 /*
- * dmv_b200.h -- C ABI of libdmv_b200.so: the B200-native distributed matrix-free H.x hot path.
+ * dmv_b200.h -- C ABI of libdmv_b200.so: the distributed matrix-free H.x hot path for Hopper (sm_90a).
  *
  * This is the drop-in boundary for the reference's hot path (SURVEY.md section 8b).  Plain pointers
  * and sizes only; no torch / C++ types.  Every entry point names the reference interface it replaces.
@@ -81,8 +81,9 @@ int dmv_synchronize(dmv_context *ctx);
  *          "rows"     = -1 auto | 0 use the queued k_pull instead of k_rows
  *          "rows_index" = -1 auto, 0 open-addressing table with the vector element in the slot | 1 dense table behind a
  *                        two-level perfect hash (5 bits per state; measured slower, kept for reference)
- *          "rows_ctas" = 3 (default) | 2 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread 80 | 122 |
- *                        64; at 80 a few words of the pipeline state spill and the extra warps more than pay for it)
+ *          "rows_ctas" = 2 (default) | 3 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread
+ *                        122 | 80 | 64; at 80 and 64 words of the pipeline state spill, and on an H100 the extra warps do
+ *                        not pay for it)
  *          "rows_batch" = -1 auto, 1: dmv_matvec_batch on bases with permutation symmetries takes up to six doubles per
  *                        state (six real / three complex vectors) through k_rows_batch | 0 vector by vector;
  *                        "rows_batch_min" = doubles per state (vectors x element width, default 2) from which it is used
@@ -166,7 +167,7 @@ int dmv_outgoing(dmv_context *ctx, int dest, const uint64_t **betas, const doubl
 int dmv_accumulate(dmv_context *ctx, int elt, int64_t count, const uint64_t *betas,
                    const double *coeffs, void *y);
 
-/* ---- replicated-x form of the distributed product (B200-first alternative to the record exchange of DMV:313-436,
+/* ---- replicated-x form of the distributed product (alternative to the record exchange of DMV:313-436,
  * chosen automatically by dmv_matvec -- option "exchange" = -1 / 2 -- when the whole basis fits on one device): every
  * rank keeps the whole sorted basis, x is all-gathered (E bytes per state instead of 8 + E bytes per off-diagonal term
  * over NVLink) into slots of dmv_get_info(ctx, "replicated_block") elements per rank, and each rank computes ITS rows by

@@ -3,13 +3,12 @@
 
 The model inputs are data, not code: the basis description (number of spins, Hamming weight, spin
 inversion, symmetry generators) and the Hamiltonian term list (expression + site tuples) of each
-/root/reference/data/*.yaml.  This script extracts that semantic content and re-emits it in a
-normalised layout (no anchors, no comments, no solver-only keys such as `observables`,
-`number_vectors`, `output`, `max_primme_*`), so that tests, bench.py and smoke() can run on the GPU
-box where /root/reference does not exist.  tests/test_host.py (test_model_inputs_equal_the_reference_inputs) re-checks semantic equality against
-/root/reference whenever it is present.
+reference's data/*.yaml (kept verbatim in tests/golden/reference_data.tar.xz).  This script extracts that semantic
+content and re-emits it in a normalised layout (no anchors, no comments, no solver-only keys such as `observables`,
+`number_vectors`, `output`, `max_primme_*`).  tests/test_host.py (test_model_inputs_equal_the_reference_inputs)
+re-checks semantic equality against the stored copies.
 
-Usage:  python tools/gen_models.py [/root/reference/data] [data]
+Usage:  python tools/gen_models.py REFERENCE_DATA_DIR [data]
 """
 import glob
 import os
@@ -53,7 +52,9 @@ def normalise(conf: dict) -> dict:
 
 
 def main():
-    src = sys.argv[1] if len(sys.argv) > 1 else "/root/reference/data"
+    if len(sys.argv) < 2:
+        raise SystemExit(__doc__)
+    src = sys.argv[1]
     dst = sys.argv[2] if len(sys.argv) > 2 else os.path.join(os.path.dirname(__file__), "..", "data")
     os.makedirs(dst, exist_ok=True)
     for path in sorted(glob.glob(os.path.join(src, "*.yaml"))):

@@ -1,5 +1,6 @@
 #!/usr/bin/env python3
-"""Parity of the real multi-GPU product (one process per GPU, NCCL / NVLink inside libdmv_b200) against the CPU oracle.
+"""Parity of the real multi-GPU product (one process per rank, NCCL / NVLink inside libdmv_b200) against the CPU oracle.
+With fewer GPUs than ranks, ranks share devices (round robin): the same exchanges run through CUDA IPC on one device.
 
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port 29511 tools/multi_gpu_check.py [workload ...]
@@ -9,9 +10,10 @@ DMV_PEER_GATHER = 0 forces the NCCL all-gather in the replicated-x form.  Small 
 with the oracle's P-locale product; models of 10^5 .. 10^7 states per rank through sampled rows (oracle_expected_rows).
 Also covered: the collective block <-> hashed redistribution, Lanczos across the ranks, and the host-owned products
 (HostExchangedProduct / HostReplicatedProduct) with the real Operator under the NCCL backend.  Used by
-tests/test_multi_gpu.py (self-skips below two GPUs).
+tests/test_multi_gpu.py.
 """
 import os
+import socket
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -43,6 +45,13 @@ def close(a, b):
 
 def main():
     rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); local = int(os.environ["LOCAL_RANK"])
+    local %= torch.cuda.device_count()          # fewer GPUs than ranks: several ranks share a device
+    if torch.cuda.device_count() < world:
+        # NCCL refuses two ranks of one host on one device; as ranks of distinct hosts they talk over loopback sockets
+        # (the library's own NCCL communicator reads the same variables)
+        os.environ["NCCL_HOSTID"] = f"{socket.gethostname()}-rank{rank}"
+        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
+        os.environ.setdefault("NCCL_IB_DISABLE", "1")
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     po.set_num_threads(max(1, len(os.sched_getaffinity(0)) // world))

@@ -1,7 +1,7 @@
-// Random-access ceiling of HBM3e on this GPU: every thread issues U independent loads of `BYTES` bytes at hashed,
+// Random-access ceiling of HBM on this GPU: every thread issues U independent loads of `BYTES` bytes at hashed,
 // BYTES-aligned offsets of a table of T bytes, over and over.  Prints effective GB/s (useful bytes) per configuration:
 // the roofline of the hash-table look-ups of k_rows (one 64-byte bucket per off-diagonal term).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 tools/random_access.cu -o /tmp/random_access && /tmp/random_access
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 tools/random_access.cu -o /tmp/random_access && /tmp/random_access
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>

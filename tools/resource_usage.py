@@ -36,7 +36,7 @@ def main():
             rows.append((fn, int(m.group(1)), int(m.group(2)), int(m.group(3))))
             fn = None
     names = demangle([r[0] for r in rows])
-    print("# Static resources of the kernels in libdmv_b200.so (cuobjdump -res-usage, sm_100a)\n")
+    print("# Static resources of the kernels in libdmv_b200.so (cuobjdump -res-usage, sm_90a)\n")
     print("Registers per thread, stack bytes per thread (spills + local arrays) and STATIC shared memory; the dynamic shared "
           "memory (operator / orbit tables) comes from `smem_layout` at launch. 256 threads per CTA: 80 registers = 3 CTAs "
           "per SM, 128 = 2, 64 = 4 (65 536 registers per SM).\n")

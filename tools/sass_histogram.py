@@ -25,7 +25,7 @@ for line in out.splitlines():
         base = op.split(".")[0]
         key = op if base in ("LDG", "STG", "RED", "ATOMG", "ATOMS", "UBLKCP", "LDGSTS", "LDS", "STS", "SYNCS", "CCTL", "MEMBAR", "ST", "LD") else base
         hist[fam][key] += 1
-print("# SASS opcode histogram of libdmv_b200.so (cuobjdump -sass, sm_100a), static instruction counts per kernel family\n")
+print("# SASS opcode histogram of libdmv_b200.so (cuobjdump -sass, sm_90a), static instruction counts per kernel family\n")
 interesting = ["UBLKCP", "SYNCS", "LDGSTS", "LDG", "STG", "ST", "RED", "ATOMG", "ATOMS", "LDS", "STS", "MEMBAR", "DFMA", "DMUL", "DADD",
                "IMAD", "LOP3", "SHF", "POPC", "FLO", "BREV", "ISETP", "VIMNMX", "SEL", "PRMT", "REDUX", "VOTE", "SHFL", "MATCH", "BAR"]
 for f in sorted(hist):
