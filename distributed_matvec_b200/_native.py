@@ -95,6 +95,8 @@ _SIGNATURES = [
     ("dmv_debug_tridiagonal_lowest", C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.POINTER(C.c_double), C.c_void_p]),
     ("dmv_debug_compile_group", C.c_int, [C.POINTER(BasisDesc), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                           C.c_void_p]),
+    ("dmv_debug_ordered_table", C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]),
 ]
 
 EXPORTED_SYMBOLS = [s[0] for s in _SIGNATURES]

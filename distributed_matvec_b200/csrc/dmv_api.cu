@@ -636,17 +636,32 @@ void ensure_table(dmv_context *ctx, int elt) {
     CUDA_CHECK(cudaMemsetAsync(ctx->d_dense.ptr, 0xff, dense_bytes, st));
   }
   // ---- open-addressing table over the states that are left (all of them without the dense index)
-  // complex128: one-slot buckets, 8 per state (1.07 probes per look-up) while the table stays below a quarter of the
-  // free memory, else 4 or 2 per state; float64: two-slot buckets, 2 per state
+  // complex128, hashed: one-slot buckets, 8 per state (1.07 probes per look-up); ordered: opt_rows_table_buckets per
+  // state.  Either while the table stays below a quarter of the free memory, else halved down to 2 per state.
+  // float64: two-slot buckets, 2 per state.  The perfect hash's leftover keys are not sorted: they keep the hashed home.
+  const bool ordered = !ctx->dense_index && ctx->opt_rows_table == 1 && n >= 1;
   size_t free_b = 0, total_b = 0;
   CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-  int64_t per_state = ce ? 8 : 2;
+  int64_t per_state = ce ? (ordered ? ctx->opt_rows_table_buckets : 8) : 2;
   while (per_state > 2 && (double)per_state * n_left * 32.0 > 0.25 * (double)free_b) per_state /= 2;
   if (per_state * n_left + 16 >= 2147483647ll) throw std::runtime_error("k_rows: table of more than 2^31 buckets");
-  const uint32_t slots = (uint32_t)std::max<int64_t>(16, per_state * n_left);
+  // (the ordered directory ends at exactly per_state * n buckets)
+  const uint32_t slots = (uint32_t)(ordered ? per_state * n : std::max<int64_t>(16, per_state * n_left));
   ctx->d_table.alloc((size_t)slots * 32);
   ctx->d_slot_of.alloc((size_t)std::max<int64_t>(1, n));
   CUDA_CHECK(cudaMemsetAsync(ctx->d_table.ptr, 0xff, (size_t)slots * 32, st));
+  ctx->table_dir = OrderedDir{};
+  if (ordered) {
+    uint64_t k_lo = 0, k_hi = 0;
+    CUDA_CHECK(cudaMemcpyAsync(&k_lo, ctx->d_reps.ptr, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaMemcpyAsync(&k_hi, ctx->d_reps.ptr + (n - 1), 8, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    OrderedDir D = ordered_plan(k_lo, k_hi, ctx->opt_rows_table_bits);
+    ctx->d_table_dir.alloc((size_t)D.last + 2);
+    D.dir = ctx->d_table_dir.ptr;
+    launch_ordered_dir(ctx->d_reps.ptr, n, D, (uint32_t)per_state, st);
+    ctx->table_dir = D;
+  }
   if (ctx->dense_index) {
     DevBuf<uint32_t> d_tmp;
     d_tmp.alloc((size_t)std::max<int64_t>(1, n_left));
@@ -655,7 +670,8 @@ void ensure_table(dmv_context *ctx, int elt) {
                      ctx->d_status.ptr, st);
     CUDA_CHECK(cudaStreamSynchronize(st));
   } else {
-    launch_table_insert(ctx->d_reps.ptr, n, ctx->d_table.ptr, slots, ce ? 1 : 2, ctx->d_slot_of.ptr, st);
+    launch_table_insert(ctx->d_reps.ptr, n, ctx->d_table.ptr, slots, ce ? 1 : 2, ctx->d_slot_of.ptr, st, 32,
+                        ctx->table_dir);
   }
   ctx->table_slots = slots;
   ctx->table_elt = elt;
@@ -681,6 +697,7 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   p.uni_re = basis->gather_uni[0]; p.uni_im = basis->gather_uni[1];
   p.table = basis->d_table.ptr;
   p.table_slots = basis->table_slots;
+  p.table_dir = basis->table_dir;
   p.mph = basis->mph;
   p.dense = basis->dense_index ? basis->d_dense.ptr : nullptr;
   p.row_split = 1;
@@ -1018,6 +1035,20 @@ int dmv_set_option(dmv_context *ctx, const char *name, int64_t value) {
     ctx->opt_rows_index = (int)value;
     ctx->table_elt = 0;
     if (ctx->global) { ctx->global->opt_rows_index = (int)value; ctx->global->table_elt = 0; }
+  } else if (key == "rows_table" || key == "rows_table_bits" || key == "rows_table_buckets") {
+    if (key == "rows_table" && (value < 0 || value > 1))
+      throw std::runtime_error("rows_table: 0 hashed home, 1 ordered by key prefix");
+    if (key == "rows_table_bits" && (value < 1 || value > 14))
+      throw std::runtime_error("rows_table_bits: 1 .. 14 (the directory of 2^bits blocks lives in shared memory)");
+    if (key == "rows_table_buckets" && value != 2 && value != 4 && value != 8)
+      throw std::runtime_error("rows_table_buckets: 2, 4 or 8 buckets per state");
+    for (dmv_context *c : {ctx, ctx->global}) {
+      if (!c) continue;
+      if (key == "rows_table") c->opt_rows_table = (int)value;
+      else if (key == "rows_table_bits") c->opt_rows_table_bits = (int)value;
+      else c->opt_rows_table_buckets = (int)value;
+      c->table_elt = 0;
+    }
   } else if (key == "rounds") {
     if (value < -1 || value > 64) throw std::runtime_error("rounds: -1 auto, 0 / 1 one-shot exchange, R <= 64 overlapped rounds");
     ctx->opt_rounds = (int)value;
@@ -1528,6 +1559,39 @@ int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t 
     }
     if (reps) reps[k] = r.rep;
     if (stab) stab[k] = r.stab;
+  }
+  API_END
+}
+
+int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
+                            uint32_t *home, uint32_t *probes) {
+  API_BEGIN
+  if (n < 1 || !reps || bits < 1 || bits > 14 || buckets_per_state < 2) throw std::runtime_error("bad arguments");
+  for (int64_t k = 1; k < n; ++k)
+    if (reps[k] <= reps[k - 1]) throw std::runtime_error("representatives must be ascending");
+  OrderedDir D = ordered_plan(reps[0], reps[n - 1], bits);
+  std::vector<uint32_t> dir((size_t)D.last + 2);
+  for (uint32_t p = 0; p <= D.last + 1; ++p) dir[p] = ordered_dir_entry(reps, n, D, (uint32_t)buckets_per_state, p);
+  D.dir = dir.data();
+  const uint32_t n_buckets = (uint32_t)(buckets_per_state * n);
+  if (dir[D.last + 1] != n_buckets) throw std::runtime_error("directory does not end at the table size");
+  std::vector<uint64_t> keys(n_buckets, kEmptyKey);
+  for (int64_t k = 0; k < n; ++k) {   // k_table_insert, one slot per bucket
+    uint32_t b = table_home(reps[k], n_buckets, D);
+    while (keys[b] != kEmptyKey) b = b + 1 == n_buckets ? 0 : b + 1;
+    keys[b] = reps[k];
+  }
+  for (int64_t k = 0; k < n; ++k) {   // the look-up of k_rows
+    const uint32_t h = table_home(reps[k], n_buckets, D);
+    uint32_t b = h, count = 1;
+    while (keys[b] != reps[k]) {
+      if (keys[b] == kEmptyKey) throw std::runtime_error("ordered table: a representative is not found");
+      b = b + 1 == n_buckets ? 0 : b + 1;
+      ++count;
+    }
+    if (block) block[k] = ordered_block(reps[k], D.k_lo, D.shift, D.last);
+    if (home) home[k] = h;
+    if (probes) probes[k] = count;
   }
   API_END
 }

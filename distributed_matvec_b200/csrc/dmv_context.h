@@ -202,6 +202,18 @@ struct dmv_context {
                              // the dense table is still many times L2, so a look-up still costs a random sector)
   DevBuf<uint32_t> d_slot_of;
   uint32_t table_slots = 0;
+  // layout of the open-addressing table without the dense index: 0 hashed home (table_slot), 1 ordered by key prefix
+  // (ordered_block in dmv_device.cuh; its directory of at most 2^bits blocks lives in shared memory, so bits <= 14),
+  // complex128 with `buckets` one-slot buckets per state (float64: two-slot buckets, 2 per state, in both layouts).
+  // Ordered, 2^14 blocks and 8 buckets per state: on an H100 (700 W, L2 flushed) 6.6 % faster than hashed on the 6x6
+  // square, 3.4 % on chain_32_symm and 7.3 % on chain_36_symm (complex128), 1.7 / 0.3 / 5.5 % (float64).  With 4 or 2
+  // buckets per state the extra probes of linear probing (1.17 / 1.5 per look-up against 1.07) cost more than the
+  // smaller table saves: 5-15 % / 35-60 % slower (profiles/h100_rows_table_sweep*.log)
+  int opt_rows_table = 1;
+  int opt_rows_table_bits = 14;
+  int opt_rows_table_buckets = 8;
+  DevBuf<uint32_t> d_table_dir;
+  OrderedDir table_dir{};
   int table_elt = 0;        // element type the slots are laid out for (0: not built)
   // k_rows_batch: 64-byte buckets { key, six doubles, spare }, eight per state (fewer when memory is short); built on the first
   // batched product

@@ -253,8 +253,8 @@ __device__ __forceinline__ int64_t locate(const StateIndex &ix, uint64_t key) {
 // array + directory needs  directory -> several probes -> norm -> x  dependent loads per term, and orbit minima
 // cluster at small values, which unbalances any directory over the top bits; here a term costs the 32-byte sector of
 // its bucket.  The values are refreshed once per product
-// (k_table_fill: x[i] * norm[i] at slot_of[i]).  The table takes 64 .. 256 bytes per state (fewer when
-// free memory is short: ensure_table).  A bucket is ONE 32-byte sector, fetched with two independent 128-bit loads:
+// (k_table_fill: x[i] * norm[i] at slot_of[i]).  The table takes 64 .. 256 bytes per state (ensure_table: fewer
+// for the ordered layout below and when free memory is short).  A bucket is ONE 32-byte sector, fetched with two independent 128-bit loads:
 // random look-ups are bound by the rate at which HBM serves random sectors (tools/random_access.cu measures it), so
 // the look-up costs what its sector costs.  A state goes to the first bucket from its home with a free slot; a look-up that finds its
 // bucket taken by other states moves on to the next one (7 % of the look-ups for complex128, 2 % for float64).
@@ -265,6 +265,57 @@ constexpr uint64_t kEmptyKey = ~0ull;
 __host__ __device__ __forceinline__ uint32_t table_slot(uint64_t key, uint32_t n_buckets) {
   const uint64_t h = key * 0x9E3779B97F4A7C15ull;
   return (uint32_t)(((h >> 32) * (uint64_t)n_buckets) >> 32);
+}
+
+// Ordered layout of the same table (k_rows, rows_table = 1).  The hash above scatters the representatives over the
+// whole table, so no row order gives L2 reuse.  But most off-diagonal targets of a row share its leading key bits
+// (tools/lookup_locality.py), and the rows run in ascending key order.  So the table is cut into blocks by key prefix:
+// block p = (key - k_lo) >> shift holds buckets [dir[p], dir[p + 1]), buckets_per_state times the number of
+// representatives with that prefix, and a state's home is hashed inside its block.  The part of the table that the rows
+// in flight read is then a narrow window that the L2 holds.  Linear probing, the empty key and the look-up are as in
+// the hashed layout.  dir[p] = buckets_per_state * (first representative >= k_lo + (p << shift)) in the sorted basis.
+struct OrderedDir {
+  const uint32_t *dir;   // last + 2 bucket offsets; null: hashed layout
+  uint64_t k_lo;         // smallest representative
+  uint32_t shift, last;  // block of a key = min((key - k_lo) >> shift, last)
+};
+__host__ __device__ __forceinline__ uint32_t ordered_block(uint64_t key, uint64_t k_lo, uint32_t shift, uint32_t last) {
+  const uint64_t q = (key - k_lo) >> shift;   // keys below k_lo wrap to large values and go to the last block
+  return q < last ? (uint32_t)q : last;
+}
+__host__ __device__ __forceinline__ uint32_t ordered_slot(uint64_t key, uint32_t lo, uint32_t hi) {
+  return lo + table_slot(key, hi - lo);       // an empty block (hi = lo) sends its keys to the next block's start
+}
+// home bucket of a key in either layout
+__host__ __device__ __forceinline__ uint32_t table_home(uint64_t key, uint32_t n_buckets, const OrderedDir &D) {
+  if (D.dir == nullptr) return table_slot(key, n_buckets);
+  const uint32_t p = ordered_block(key, D.k_lo, D.shift, D.last);
+  return ordered_slot(key, D.dir[p], D.dir[p + 1]);
+}
+// first index of the sorted a[0, n) with a[i] >= v
+__host__ __device__ __forceinline__ int64_t lower_bound_u64(const uint64_t *a, int64_t n, uint64_t v) {
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if (a[mid] < v) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+// directory entry p of the ordered layout over the sorted representatives reps[0, n)
+__host__ __device__ __forceinline__ uint32_t ordered_dir_entry(const uint64_t *reps, int64_t n, const OrderedDir &D,
+                                                               uint32_t buckets_per_state, uint32_t p) {
+  const int64_t first = p > D.last ? n : lower_bound_u64(reps, n, D.k_lo + ((uint64_t)p << D.shift));
+  return (uint32_t)(buckets_per_state * first);
+}
+// at most 2^bits blocks over the representatives k_lo .. k_hi (dir left null)
+inline OrderedDir ordered_plan(uint64_t k_lo, uint64_t k_hi, int bits) {
+  const uint64_t range = k_hi - k_lo;
+  int used = 0;
+  while (used < 64 && (range >> used) != 0) ++used;
+  OrderedDir D{nullptr, k_lo, used > bits ? (uint32_t)(used - bits) : 0u, 0u};
+  D.last = (uint32_t)(range >> D.shift);
+  return D;
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -126,6 +126,9 @@ void setup_replicated(dmv_context *ctx) {
     g->opt_rows = ctx->opt_rows;
     g->opt_gather_walk = ctx->opt_gather_walk;
     g->opt_rows_index = ctx->opt_rows_index;
+    g->opt_rows_table = ctx->opt_rows_table;
+    g->opt_rows_table_bits = ctx->opt_rows_table_bits;
+    g->opt_rows_table_buckets = ctx->opt_rows_table_buckets;
     g->opt_rows_ctas = ctx->opt_rows_ctas;
     if (ctx->opt_canon != g->opt_canon && g->proj == PROJ_GROUP) { g->opt_canon = ctx->opt_canon; upload_orbit(g); }
     if (dmv_basis_build(g) != 0) throw std::runtime_error(g_last_error);

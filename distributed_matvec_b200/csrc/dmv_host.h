@@ -109,6 +109,7 @@ struct KernelParams {
   // vector element in the slot (see table_slot in dmv_device.cuh)
   const void *table;
   uint32_t table_slots;
+  OrderedDir table_dir;        // ordered layout of `table` (rows_table = 1; see ordered_block), dir null: hashed layout
   // ... or, with a dense index: perfect hash -> slot of `dense` (32 bytes: {key, spare, re, im} / 16 bytes: {key, value});
   // `table` then only holds the few per cent of the states the two levels could not place
   PerfectHash mph;
@@ -130,7 +131,9 @@ void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stre
 // hash table of k_rows: insert every state (slot_of[i] = its slot), then per product table[slot_of[i]] = x[src(i)] * norm[i]
 // with src(i) = pos ? pos[i] : i
 void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t n_buckets, int slots_per_bucket,
-                         uint32_t *slot_of, cudaStream_t stream, int bucket_bytes = 32);
+                         uint32_t *slot_of, cudaStream_t stream, int bucket_bytes = 32, OrderedDir ord = OrderedDir{});
+// directory of the ordered layout over the sorted representatives: ord.dir[0 .. ord.last + 1]
+void launch_ordered_dir(const uint64_t *reps, int64_t n, OrderedDir ord, uint32_t buckets_per_state, cudaStream_t stream);
 // k_rows on several vectors at once: 64-byte buckets { key, six doubles, spare } shared by the vectors of the batch
 void launch_rows_batch(const KernelParams &p, cudaStream_t stream);
 void launch_table_fill_batch(int64_t n, int num_vectors, int elt, const void *x, int64_t stride, const double *norms,

@@ -895,12 +895,16 @@ __device__ __forceinline__ void axpy(double2 &acc, double c, double2 v) { acc.x 
 
 // two CTAs per SM: the pipeline state must stay in registers (a spilled request waits for its load at once), and the
 // latency is hidden inside the lane, not by occupancy
-template <bool CE, int TK, bool MPH, int CTAS>
+// ORD: ordered table layout (see ordered_block); its directory is staged into shared memory behind the other tables, so
+// a home costs two shared-memory reads and adds no dependent global access to the pipeline
+template <bool CE, int TK, bool MPH, int CTAS, bool ORD>
 __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   using E = typename ValT<CE>::type;
   extern __shared__ __align__(16) unsigned char smem[];
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
   const Tables<false> T = stage_tables<PROJ_GROUP, false>(p, smem, L);   // p.groups / p.lut: row-traversal tables
+  uint32_t *sdir = reinterpret_cast<uint32_t *>(smem + align_up(L.total, 16));
+  if constexpr (ORD) stage(sdir, p.table_dir.dir, (int)p.table_dir.last + 2);
   __syncthreads();
   const OrbitProgram &orbit = T.orbit;
   const unsigned lane = threadIdx.x & 31u;
@@ -1044,7 +1048,12 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
         const uint64_t raw = b ^ flip;
         if constexpr (TK > 0) want0 = orbit_min_torus_sq<TK>(orbit, raw);
         else want0 = orbit_representative(orbit, raw);
-        b0 = table_slot(want0, n_buckets);
+        if constexpr (ORD) {
+          const uint32_t blk = ordered_block(want0, p.table_dir.k_lo, p.table_dir.shift, p.table_dir.last);
+          b0 = ordered_slot(want0, sdir[blk], sdir[blk + 1]);
+        } else {
+          b0 = table_slot(want0, n_buckets);
+        }
         bucket_load<CE>(table, b0, k0, v00, v01);
         live0 = true;
       } else {
@@ -1186,11 +1195,11 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows_batch(const KernelParam
 // hash table set-up: claim a slot per state (keys pre-set to kEmptyKey; slot 0 of a bucket, then slot 1 when the bucket
 // has two, then the next bucket), remember it in slot_of (= 2 bucket + slot)
 __global__ void k_table_insert(const uint64_t *__restrict__ reps, int64_t n, unsigned char *table, uint32_t n_buckets,
-                               int slots_per_bucket, uint32_t *slot_of, int bucket_bytes) {
+                               int slots_per_bucket, uint32_t *slot_of, int bucket_bytes, OrderedDir ord) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint64_t key = reps[i];
-  uint32_t b = table_slot(key, n_buckets);
+  uint32_t b = table_home(key, n_buckets, ord);
   for (;;) {
     unsigned long long *q = reinterpret_cast<unsigned long long *>(table + (size_t)b * bucket_bytes);
     if (atomicCAS(q, (unsigned long long)kEmptyKey, (unsigned long long)key) == (unsigned long long)kEmptyKey) {
@@ -1204,6 +1213,12 @@ __global__ void k_table_insert(const uint64_t *__restrict__ reps, int64_t n, uns
     }
     b = b + 1 == n_buckets ? 0 : b + 1;
   }
+}
+
+__global__ void k_ordered_dir(const uint64_t *__restrict__ reps, int64_t n, OrderedDir ord, uint32_t buckets_per_state,
+                              uint32_t *dir) {
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p <= (int64_t)ord.last + 1) dir[p] = ordered_dir_entry(reps, n, ord, buckets_per_state, (uint32_t)p);
 }
 
 // per product: value of slot_of[i] = x[src(i)] * norm[i]   (src(i) = pos ? pos[i] : i).  complex128 rewrites the WHOLE
@@ -1616,11 +1631,11 @@ void launch_accumulate_p(const KernelParams &p, bool cv, bool ce, int64_t count,
 }  // namespace
 
 namespace {
-template <bool CE, int TK, bool MPH, int CTAS = 2>
+template <bool CE, int TK, bool MPH, int CTAS = 2, bool ORD = false>
 void launch_rows_t(const KernelParams &p, cudaStream_t stream) {
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
-  const size_t smem_bytes = L.total;
-  auto kernel = k_rows<CE, TK, MPH, CTAS>;
+  const size_t smem_bytes = ORD ? align_up(L.total, 16) + 4 * ((size_t)p.table_dir.last + 2) : L.total;
+  auto kernel = k_rows<CE, TK, MPH, CTAS, ORD>;
   if (smem_bytes > 48 * 1024)
     DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
   int per_sm = 0;
@@ -1640,6 +1655,21 @@ void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
     if (k == 6) launch_rows_t<CE, 6, true>(p, stream);
     else if (k == 4) launch_rows_t<CE, 4, true>(p, stream);
     else launch_rows_t<CE, 0, true>(p, stream);
+    return;
+  }
+  if (p.table_dir.dir != nullptr) {   // ordered table layout
+    if (p.rows_ctas == 3) {
+      if (k == 6) launch_rows_t<CE, 6, false, 3, true>(p, stream);
+      else if (k == 4) launch_rows_t<CE, 4, false, 3, true>(p, stream);
+      else launch_rows_t<CE, 0, false, 3, true>(p, stream);
+    } else if (p.rows_ctas == 4) {
+      if (k == 6) launch_rows_t<CE, 6, false, 4, true>(p, stream);
+      else launch_rows_t<CE, 0, false, 4, true>(p, stream);
+    } else {
+      if (k == 6) launch_rows_t<CE, 6, false, 2, true>(p, stream);
+      else if (k == 4) launch_rows_t<CE, 4, false, 2, true>(p, stream);
+      else launch_rows_t<CE, 0, false, 2, true>(p, stream);
+    }
     return;
   }
   if (p.rows_ctas == 3) {   // three CTAs per SM: 80 registers, a few words of the pipeline state spill
@@ -1711,10 +1741,18 @@ void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stre
 }
 
 void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t n_buckets, int slots_per_bucket,
-                         uint32_t *slot_of, cudaStream_t stream, int bucket_bytes) {
+                         uint32_t *slot_of, cudaStream_t stream, int bucket_bytes, OrderedDir ord) {
   if (n <= 0) return;
   k_table_insert<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reps, n, reinterpret_cast<unsigned char *>(table),
-                                                                 n_buckets, slots_per_bucket, slot_of, bucket_bytes);
+                                                                 n_buckets, slots_per_bucket, slot_of, bucket_bytes, ord);
+  DMV_CUDA_CHECK(cudaGetLastError());
+  g_launches++;
+}
+
+void launch_ordered_dir(const uint64_t *reps, int64_t n, OrderedDir ord, uint32_t buckets_per_state, cudaStream_t stream) {
+  const int64_t entries = (int64_t)ord.last + 2;
+  k_ordered_dir<<<(unsigned)((entries + 255) / 256), 256, 0, stream>>>(reps, n, ord, buckets_per_state,
+                                                                        const_cast<uint32_t *>(ord.dir));
   DMV_CUDA_CHECK(cudaGetLastError());
   g_launches++;
 }

@@ -81,6 +81,11 @@ int dmv_synchronize(dmv_context *ctx);
  *          "rows"     = -1 auto | 0 use the queued k_pull instead of k_rows
  *          "rows_index" = -1 auto, 0 open-addressing table with the vector element in the slot | 1 dense table behind a
  *                        two-level perfect hash (5 bits per state; measured slower, kept for reference)
+ *          "rows_table" = 1 (default) open-addressing table of k_rows laid out by key prefix, so that the look-ups of
+ *                        neighbouring rows share L2 | 0 homes hashed over the whole table (the perfect hash's leftover
+ *                        states always use hashed homes)
+ *          "rows_table_bits" = 1 .. 14 (default 14): the ordered layout's directory has at most 2^bits blocks
+ *          "rows_table_buckets" = 2 | 4 | 8 (default 8): complex128 buckets per state of the ordered layout
  *          "rows_ctas" = 2 (default) | 3 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread
  *                        122 | 80 | 64; at 80 and 64 words of the pipeline state spill, and on an H100 the extra warps do
  *                        not pay for it)
@@ -277,10 +282,16 @@ void ls_chpl_enumerate_representatives(const void *ls_hs_basis_ptr, uint64_t low
  * dmv_debug_compile_group: compiles the symmetry group of `basis` into the device orbit program, verifies it against
  *   bit-by-bit permutation and evaluates the compiled program (the device functions themselves, compiled for the host)
  *   for `count` states: reps[k] = min_g g(s_k), stab[k] = |{g : g(s_k) = s_k}|.
- *   info[0..5] = {n_q, n_stages, n_t, n_left, n_right, has_flip}. */
+ *   info[0..5] = {n_q, n_stages, n_t, n_left, n_right, has_flip}.
+ * dmv_debug_ordered_table: builds the ordered layout of the k_rows table (complex128: one-slot buckets,
+ *   `buckets_per_state` per state, at most 2^bits blocks) over the `n` ascending representatives `reps` with the device
+ *   functions compiled for the host, inserts them in order and looks every one up again: block[k] = prefix block of
+ *   reps[k], home[k] = its home bucket, probes[k] = buckets its look-up reads.  Fails when a state is not found. */
 int dmv_debug_tridiagonal_lowest(int k, const double *diag, const double *offdiag, double *eigenvalue, double *vector);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
+int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
+                            uint32_t *home, uint32_t *probes);
 
 #ifdef __cplusplus
 }

@@ -56,7 +56,7 @@ void run(const uint4 *table, size_t table_bytes, int blocks_per_sm, uint64_t *si
 int main() {
   uint64_t *sink;
   cudaMalloc(&sink, 8);
-  for (size_t mb : {256ul, 1024ul, 2048ul, 8192ul, 32768ul}) {
+  for (size_t mb : {256ul, 1024ul, 4096ul, 16384ul}) {
     uint4 *table;
     if (cudaMalloc(&table, mb << 20) != cudaSuccess) { printf("alloc %zu MB failed\n", mb); continue; }
     cudaMemset(table, 1, mb << 20);

@@ -1,0 +1,99 @@
+#!/usr/bin/env python3
+"""Time k_rows with the hashed and the ordered layout of its look-up table (rows_table = 0 / 1), the ordered one at
+several directory sizes (rows_table_bits) and, for complex128, buckets per state (rows_table_buckets).  The
+configurations alternate in rounds; each product is timed with CUDA events, the L2 flushed before it, and every
+configuration's y is compared with the hashed layout's by the element criterion of bench.py.
+Usage: python tools/rows_table_sweep.py [--rounds R] [--products K] [workload ...]"""
+import argparse
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from distributed_matvec_b200 import Operator, load_config_from_yaml  # noqa: E402
+
+def card():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip()
+    except OSError as e:
+        return f"nvidia-smi unavailable ({e})"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=2)
+    ap.add_argument("--products", type=int, default=6, help="timed products per configuration and round")
+    ap.add_argument("--dtypes", default="c128,f64")
+    ap.add_argument("--bits", default="10,12,14", help="directory sizes of the ordered layout (rows_table_bits)")
+    ap.add_argument("--buckets", default="2,4,8", help="complex128 buckets per state of the ordered layout")
+    ap.add_argument("workloads", nargs="*", default=["heisenberg_square_6x6", "heisenberg_chain_32_symm",
+                                                     "heisenberg_chain_36_symm"])
+    args = ap.parse_args()
+    print("card:", card(), flush=True)
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device="cuda")
+    for name in args.workloads:
+        basis, matrix = load_config_from_yaml(os.path.join(ROOT, "data", name + ".yaml"))
+        op = Operator(matrix)
+        op.basis.build()
+        n = op.basis.numberStates()
+        op.use_torch_stream()
+        print(f"== {name}: N={n}", flush=True)
+        rng = np.random.default_rng(42)
+        for dt in args.dtypes.split(","):
+            cplx = dt == "c128"
+            x = rng.random(n) - 0.5
+            if cplx:
+                x = x + 1j * (rng.random(n) - 0.5)
+            xd = torch.from_numpy(x).cuda()
+            yd = torch.zeros_like(xd)
+            # (float64: two-slot buckets, 2 per state in both layouts)
+            configs = [("hashed", 0, 14, 8)] + [(f"ordered D={d} b={b}", 1, int(d), int(b))
+                                                for d in args.bits.split(",")
+                                                for b in (args.buckets.split(",") if cplx else ["2"])]
+            times = {c[0]: [] for c in configs}
+            worst = {c[0]: 0.0 for c in configs}
+            ref = None
+            for _ in range(args.rounds):
+                for label, table, bits, buckets in configs:
+                    op.set_option("rows_table", table)
+                    op.set_option("rows_table_bits", bits)
+                    op.set_option("rows_table_buckets", buckets)
+                    for _ in range(2):   # the first product rebuilds the table
+                        op.matvec(xd, yd)
+                    torch.cuda.synchronize()
+                    assert op.info("rows") == 1, "k_rows does not apply"
+                    for k in range(args.products):
+                        flush.fill_(k)
+                        s = torch.cuda.Event(enable_timing=True)
+                        e = torch.cuda.Event(enable_timing=True)
+                        s.record()
+                        op.matvec(xd, yd)
+                        e.record()
+                        torch.cuda.synchronize()
+                        times[label].append(s.elapsed_time(e))
+                    op.synchronize()
+                    if ref is None:
+                        ref = yd.clone()
+                    diff = (yd - ref).abs()
+                    bound = torch.clamp(1e-12 * torch.maximum(yd.abs(), ref.abs()), min=1e-14)
+                    bad = int((diff > bound).sum())
+                    if bad:
+                        raise SystemExit(f"{label}: {bad} elements differ from the hashed layout")
+                    worst[label] = max(worst[label], float(diff.max() / ref.abs().max()))
+            base = float(np.median(times["hashed"]))
+            for label, *_ in configs:
+                t = np.array(times[label])
+                med = float(np.median(t))
+                print(f"  {dt:4s} {label:20s} median {med:8.3f} ms  min {t.min():8.3f}  max {t.max():8.3f}  "
+                      f"({len(t)} products)  vs hashed {100 * (med / base - 1):+6.1f} %  max rel diff {worst[label]:.1e}",
+                      flush=True)
+        op.close()
+
+
+if __name__ == "__main__":
+    main()
