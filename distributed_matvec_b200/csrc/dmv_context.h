@@ -164,7 +164,7 @@ struct dmv_context {
   DevBuf<uint64_t> d_canon_masks, d_cc_mask;
   DevBuf<uint32_t> d_canon_lut2;
   DevBuf<int32_t> d_cc_begin, d_cc_delta;
-  DevBuf<uint16_t> d_tor_lutm;
+  DevBuf<uint32_t> d_tor_lutm;
   DevBuf<uint8_t> d_tor_frow;
   DevBuf<uint32_t> d_tor_luts;
   DevBuf<uint64_t> d_tor_net_mask;

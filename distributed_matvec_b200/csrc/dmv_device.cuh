@@ -123,13 +123,15 @@ struct OrbitProgram {
   // canonical form under the FULL space group of an R x k torus (sites numbered row by row, trivial characters):
   //   G = {block rotations} x {1, rho} x {1, sigma} [x {1, tau}] [x {1, flip}]
   // rho = reverse the bits inside every row, sigma = reverse the order of the rows, tau = transpose (R == k).
-  // Every image is "a row pair on top": tor_lutm[hi << k | lo] is the smallest top pair over the 2k (x2 with the flip)
-  // maps F = flip^f . rho^e . rot_a applied to both rows, tor_luts the set of (f, e, a) reaching it (bit (2f + e) k + a);
-  // only the few (row pair, F) whose top pair is the global minimum are expanded.  See orbit_min_torus().
+  // Every image is "a row pair on top": m(hi, lo) is the smallest top pair over the 2k (x2 with the flip) maps
+  // F = flip^f . rho^e . rot_a applied to both rows, tor_luts[hi << k | lo] the set of (f, e, a) reaching it
+  // (bit (2f + e) k + a); only the few (row pair, F) whose top pair is the global minimum are expanded.  See
+  // orbit_min_torus().  tor_lutm[hi << k | lo] = m(hi, lo) | m(lo, hi) << 16 holds both orders of the pair, so one
+  // look-up per pair of adjacent rows serves both directions.
   int32_t tor_mode;            // 0: off; 1: rho and sigma (4 cosets of the block rotations); 2: and tau (8 cosets)
   int32_t tor_rho_n, tor_tau_n;   // delta-swap stages of rho / tau inside tor_net_*: rho first, then tau
   int32_t tor_div_r;           // floor(bit / R) = (bit * tor_div_r) >> 16 for bit < 32
-  const uint16_t *tor_lutm;    // [2^(2k)]
+  const uint32_t *tor_lutm;    // [2^(2k)]
   const uint32_t *tor_luts;    // [2^(2k)]  (stays in global memory: read about once per state)
   const uint8_t *tor_frow;     // [4 k][2^k]: image of one row under F = flip^f rho^e rot_a, F = (2 f + e) k + a
   const uint64_t *tor_net_mask;
@@ -697,7 +699,8 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus(const OrbitProgram 
     uint32_t bit_u = bit << R;
     for (int y = 0; y < R; ++y) {
       const uint32_t hi = ((uint32_t)wy & bm) << k;
-      const uint32_t md = P.tor_lutm[hi | ((uint32_t)wd & bm)], mu = P.tor_lutm[hi | ((uint32_t)wu & bm)];
+      const uint32_t md = P.tor_lutm[hi | ((uint32_t)wd & bm)] & 0xffffu;
+      const uint32_t mu = P.tor_lutm[hi | ((uint32_t)wu & bm)] & 0xffffu;
       cand = md < mstar ? bit : (md == mstar ? (cand | bit) : cand);
       mstar = md < mstar ? md : mstar;
       cand = mu < mstar ? bit_u : (mu == mstar ? (cand | bit_u) : cand);
@@ -747,7 +750,8 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus(const OrbitProgram 
 }
 
 // The same for a K x K torus with the transposition in the group (tor_mode == 2), rows and columns in registers:
-// pass 1 is fully unrolled, 32-bit, with one shared-memory look-up per adjacent (row, row) / (column, column) pair.
+// pass 1 is fully unrolled, 32-bit, with one shared-memory look-up per adjacent (row, row) / (column, column) pair,
+// which gives the pair's minimum in both orders (2K look-ups in all).
 // Column a of the lattice (= row a of the transposed image) comes out of one masked multiply:
 //   t = (w >> a) & STRIDE has site (y, a) at bit K y; t * CMUL puts it at bit S + y (S = (K-1)^2; no two partial
 //   products meet, so there are no carries).
@@ -768,17 +772,19 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgr
   for (int y = 0; y < K; ++y) rows[0][y] = (uint32_t)(w >> (K * y)) & BM;
 #pragma unroll
   for (int a = 0; a < K; ++a) rows[1][a] = ((((uint32_t)(w >> a) & stride) * cmul) >> S) & BM;
+  const uint32_t *lutm = P.tor_lutm;
+  const uint8_t *frow = P.tor_frow;
   uint32_t md[2][K], mu[2][K];
   uint32_t mstar = 0xffffffffu;
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
 #pragma unroll
-    for (int y = 0; y < K; ++y) {
-      const uint32_t hi = rows[t][y] << K;
-      md[t][y] = P.tor_lutm[hi | rows[t][(y + K - 1) % K]];
-      mu[t][y] = P.tor_lutm[hi | rows[t][(y + 1) % K]];
-      mstar = md[t][y] < mstar ? md[t][y] : mstar;
+    for (int y = 0; y < K; ++y) {   // the pair (row y, row y+1): row y on top descending, row y+1 on top ascending
+      const uint32_t m2 = lutm[rows[t][y] << K | rows[t][(y + 1) % K]];
+      mu[t][y] = m2 & 0xffffu;
+      md[t][(y + 1) % K] = m2 >> 16;
       mstar = mu[t][y] < mstar ? mu[t][y] : mstar;
+      mstar = md[t][(y + 1) % K] < mstar ? md[t][(y + 1) % K] : mstar;
     }
   }
   uint32_t cand = 0;
@@ -826,7 +832,7 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgr
       const int sb = __builtin_ffs((int)Sset) - 1;
 #endif
       Sset &= Sset - 1;
-      const uint8_t *fr = P.tor_frow + (sb << K);
+      const uint8_t *fr = frow + (sb << K);
       uint32_t img = 0;
 #pragma unroll
       for (int q = 0; q < K - 2; ++q) {

@@ -468,7 +468,7 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
                 if (f) v ^= bm;
                 H.tor_frow[((size_t)((2 * f + e) * k + a) << k) + r] = (uint8_t)v;
               }
-        H.tor_lutm.resize((size_t)1 << (2 * k));
+        std::vector<uint16_t> lutm((size_t)1 << (2 * k));
         H.tor_luts.resize((size_t)1 << (2 * k));
         for (uint32_t hi = 0; hi <= bm; ++hi)
           for (uint32_t lo = 0; lo <= bm; ++lo) {
@@ -484,9 +484,14 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
                   if (v < best_v) { best_v = v; set = bit; }
                   else if (v == best_v) set |= bit;
                 }
-            H.tor_lutm[(hi << k) | lo] = (uint16_t)best_v;
+            lutm[(hi << k) | lo] = (uint16_t)best_v;
             H.tor_luts[(hi << k) | lo] = set;
           }
+        // both orders of a pair in one entry: one look-up per adjacent pair of rows gives the minimum of either order
+        H.tor_lutm.resize(lutm.size());
+        for (uint32_t hi = 0; hi <= bm; ++hi)
+          for (uint32_t lo = 0; lo <= bm; ++lo)
+            H.tor_lutm[(hi << k) | lo] = lutm[(hi << k) | lo] | (uint32_t)lutm[(lo << k) | hi] << 16;
       }
     }
   }

@@ -32,7 +32,7 @@ struct HostOrbitProgram {
   std::vector<int32_t> cc_begin, cc_delta;   // coset chain of the canonical-form scan
   std::vector<uint64_t> cc_mask;
   int32_t tor_mode = 0, tor_rho_n = 0, tor_tau_n = 0, tor_div_r = 0;   // full-space-group canonical form of a torus
-  std::vector<uint16_t> tor_lutm;
+  std::vector<uint32_t> tor_lutm;
   std::vector<uint32_t> tor_luts;
   std::vector<uint8_t> tor_frow;
   std::vector<uint64_t> tor_net_mask;

@@ -112,11 +112,11 @@ __host__ __device__ inline SmemLayout smem_layout(const KernelParams &p, int pro
   off = align_up(off, 8);
   L.canon = off;
   if (proj == PROJ_GROUP && p.orbit.canon_mode != 0 && p.orbit.tor_mode != 0) {
-    // full-space-group canonical form: delta-swap stages of rho / tau and the 16-bit pair table
+    // full-space-group canonical form: delta-swap stages of rho / tau and the 32-bit pair table
     const size_t n_st = (size_t)(p.orbit.tor_rho_n + p.orbit.tor_tau_n);
     off += 8 * n_st + 4 * n_st;
     off = align_up(off, 16);                                    // bulk copies need 16-byte aligned destinations
-    off += 2 * ((size_t)1 << (2 * p.orbit.canon_k));            // tor_lutm
+    off += 4 * ((size_t)1 << (2 * p.orbit.canon_k));            // tor_lutm
     off += align_up((size_t)4 * p.orbit.canon_k << p.orbit.canon_k, 16);   // tor_frow
     off += 16;                                                  // mbarrier of the bulk copies
     off = align_up(off, 8);
@@ -236,12 +236,12 @@ __device__ __forceinline__ Tables<CV> stage_tables(const KernelParams &p, unsign
     const int n_st = T.orbit.tor_rho_n + T.orbit.tor_tau_n;
     uint64_t *nm = reinterpret_cast<uint64_t *>(base);
     int32_t *nd = reinterpret_cast<int32_t *>(base + 8 * (size_t)n_st);
-    uint16_t *lm = reinterpret_cast<uint16_t *>(smem + align_up((size_t)(base - smem) + 12 * (size_t)n_st, 16));
+    uint32_t *lm = reinterpret_cast<uint32_t *>(smem + align_up((size_t)(base - smem) + 12 * (size_t)n_st, 16));
     stage(nm, p.orbit.tor_net_mask, n_st);
     stage(nd, p.orbit.tor_net_delta, n_st);
-    // the pair table (8 KB for k = 6) and the row table arrive as two TMA bulk copies (cp.async.bulk, one elected
+    // the pair table (16 KB for k = 6) and the row table arrive as two TMA bulk copies (cp.async.bulk, one elected
     // thread, completion on an mbarrier) instead of a strided loop of every thread
-    const uint32_t lut_bytes = 2u << (2 * T.orbit.canon_k);
+    const uint32_t lut_bytes = 4u << (2 * T.orbit.canon_k);
     const uint32_t frow_bytes = (uint32_t)align_up((size_t)4 * T.orbit.canon_k << T.orbit.canon_k, 16);
     uint8_t *fr = reinterpret_cast<uint8_t *>(lm) + lut_bytes;
     uint64_t *mbar = reinterpret_cast<uint64_t *>(fr + frow_bytes);
@@ -907,6 +907,12 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   if constexpr (ORD) stage(sdir, p.table_dir.dir, (int)p.table_dir.last + 2);
   __syncthreads();
   const OrbitProgram &orbit = T.orbit;
+  if constexpr (TK > 0) {
+    // stage_tables has put the pair and row tables of the square-torus form in shared memory: say so, and the look-ups
+    // of orbit_min_torus_sq compile to LDS instead of generic loads that resolve their address space at run time
+    __builtin_assume(__isShared(orbit.tor_lutm));
+    __builtin_assume(__isShared(orbit.tor_frow));
+  }
   const unsigned lane = threadIdx.x & 31u;
   const unsigned warp = threadIdx.x >> 5;
   const bool any_s_out = p.any_s_out != 0;
@@ -1097,6 +1103,12 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows_batch(const KernelParam
   const Tables<false> T = stage_tables<PROJ_GROUP, false>(p, smem, L);
   __syncthreads();
   const OrbitProgram &orbit = T.orbit;
+  if constexpr (TK > 0) {
+    // stage_tables has put the pair and row tables of the square-torus form in shared memory: say so, and the look-ups
+    // of orbit_min_torus_sq compile to LDS instead of generic loads that resolve their address space at run time
+    __builtin_assume(__isShared(orbit.tor_lutm));
+    __builtin_assume(__isShared(orbit.tor_frow));
+  }
   const unsigned lane = threadIdx.x & 31u;
   const unsigned warp = threadIdx.x >> 5;
   const bool any_s_out = p.any_s_out != 0;
