@@ -1096,6 +1096,7 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "bp_pairs") { int64_t n = 0; for (auto &w : ctx->h_push.bp) n += w.n0 + w.n1; return n; }
   if (key == "canon_mode") return ctx->orbit.canon_mode;
   if (key == "torus_mode") return ctx->orbit.tor_mode;
+  if (key == "rows_tk") return rows_torus_k(ctx->orbit, ctx->opt_rows_index == 1, ctx->opt_rows_ctas);
   if (key == "rows")
     return ((use_pull(ctx) && !use_gather(ctx) && use_rows(ctx)) ||
             (ctx->replicated && ctx->global && !use_gather(ctx->global) && use_rows(ctx->global))) ? 1 : 0;

@@ -128,6 +128,8 @@ void launch_gather(const KernelParams &p, bool inversion, bool complex_values, b
                    bool narrow, bool lin, bool uniform, cudaStream_t stream);
 // k_rows applies to real operators with a bit-parallel emit test on bases with trivial characters
 void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream);
+// side of the square-torus orbit minimum k_rows is compiled for (4 | 6), 0: the generic orbit walk
+int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas);
 // hash table of k_rows: insert every state (slot_of[i] = its slot), then per product table[slot_of[i]] = x[src(i)] * norm[i]
 // with src(i) = pos ? pos[i] : i
 void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t n_buckets, int slots_per_bucket,

@@ -1661,8 +1661,7 @@ void launch_rows_t(const KernelParams &p, cudaStream_t stream) {
 }
 template <bool CE>
 void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
-  const OrbitProgram &o = p.orbit;
-  const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
+  const int k = rows_torus_k(p.orbit, p.dense != nullptr, p.rows_ctas);
   if (p.dense != nullptr) {   // dense index (perfect hash)
     if (k == 6) launch_rows_t<CE, 6, true>(p, stream);
     else if (k == 4) launch_rows_t<CE, 4, true>(p, stream);
@@ -1702,6 +1701,13 @@ void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
   else launch_rows_t<CE, 0, false>(p, stream);
 }
 }  // namespace
+
+int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {
+  const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
+  if (k != 4 && k != 6) return 0;
+  if (k == 4 && !dense && rows_ctas == 4) return 0;   // no 4x4 build at 64 registers: the generic walk
+  return k;
+}
 
 namespace {
 template <int TK, int CTAS>

@@ -107,7 +107,8 @@ int dmv_synchronize(dmv_context *ctx);
  *                        (generate everything, fence, accumulate) | R <= 64 rounds
  * dmv_get_info: "index_mode", "pull", "gather", "rows", "rows_ok", "projection", "n_groups", "orbit_n_q", "orbit_n_t",
  *               "canon_mode", "torus_mode", "peer_direct", "replicated", "replicated_block", "peer_gather", "rounds",
- *               "global_states", "complex_coefficients", ... (-1: unknown) */
+ *               "global_states", "complex_coefficients", "rows_tk" (side of the square-torus orbit minimum k_rows is
+ *               compiled for with the current options: 4 | 6, 0 the generic walk), ... (-1: unknown) */
 int dmv_set_option(dmv_context *ctx, const char *name, int64_t value);
 int64_t dmv_get_info(const dmv_context *ctx, const char *name);
 
