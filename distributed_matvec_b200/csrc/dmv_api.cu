@@ -167,6 +167,11 @@ void use_device(const dmv_context *ctx) { CUDA_CHECK(cudaSetDevice(ctx->device))
 
 bool complex_values(const dmv_context *ctx, int elt) { return elt == DMV_C128 || ctx->complex_coefficients; }
 
+int gather_row_split(const dmv_context *g, int64_t rows) {
+  if (g->opt_gather_split > 0) return g->opt_gather_split;
+  return choose_row_split(rows, (int)g->h_pull.groups.size());
+}
+
 KernelParams base_params(dmv_context *ctx) {
   KernelParams p{};
   p.index.reps = ctx->d_reps.ptr;
@@ -749,7 +754,7 @@ void do_generate(dmv_context *ctx, int elt, const void *x_dev, void *y_dev,
     if (row_end > row_begin) { p.row_begin = row_begin; p.row_end = row_end; }
     if (use_gather(ctx)) {
       select_tables(ctx, p, true, ctx->complex_coefficients);
-      p.row_split = choose_row_split(ctx->n_states, (int)ctx->h_pull.groups.size());
+      p.row_split = gather_row_split(ctx, ctx->n_states);
       p.uni_re = ctx->gather_uni[0]; p.uni_im = ctx->gather_uni[1];
       launch_gather(p, ctx->proj == PROJ_INVERSION, ctx->complex_coefficients, elt == DMV_C128,
                     ctx->gather_narrow, ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);
@@ -1055,8 +1060,15 @@ int dmv_set_option(dmv_context *ctx, const char *name, int64_t value) {
     ctx->rounds.tried = false;
     ctx->rounds.ready = false;
   } else if (key == "gather_walk") {
-    ctx->opt_gather_walk = (value >= 0 && value <= 2) ? (int)value : 0;
+    if (value < 0 || value > 2)
+      throw std::runtime_error("gather_walk: 0 per-lane from the top bit, 1 group-major, 2 per-lane from the bottom bit");
+    ctx->opt_gather_walk = (int)value;
     if (ctx->global) ctx->global->opt_gather_walk = ctx->opt_gather_walk;
+  } else if (key == "gather_split") {
+    if (value != -1 && value != 1 && value != 2 && value != 4 && value != 8 && value != 16 && value != 32)
+      throw std::runtime_error("gather_split: -1 auto, else 1, 2, 4, 8, 16 or 32 lanes per row of k_gather");
+    ctx->opt_gather_split = (int)value;
+    if (ctx->global) ctx->global->opt_gather_split = ctx->opt_gather_split;
   } else if (key == "peer_gather") {
     if (value < -1 || value > 0) throw std::runtime_error("peer_gather: -1 auto, 0 NCCL all-gather of x");
     ctx->opt_peer_gather = (int)value;
@@ -1086,6 +1098,7 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
     return ((use_pull(ctx) && use_gather(ctx)) || (ctx->replicated && ctx->global && use_gather(ctx->global))) ? 1 : 0;
   if (key == "gather_narrow") return ctx->gather_narrow ? 1 : 0;
   if (key == "gather_uniform") return ctx->gather_uniform ? 1 : 0;
+  if (key == "gather_split") return gather_row_split(ctx, ctx->n_states);
   if (key == "peer_direct") return ctx->peer_direct ? 1 : 0;
   if (key == "replicated") return ctx->replicated ? 1 : 0;
   if (key == "replicated_block") return ctx->repl_block;
@@ -1380,7 +1393,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
       p.batch = 4;
       p.batch_stride = ctx->n_states;
       select_tables(ctx, p, true, ctx->complex_coefficients);
-      p.row_split = choose_row_split(ctx->n_states, (int)ctx->h_pull.groups.size());
+      p.row_split = gather_row_split(ctx, ctx->n_states);
       p.uni_re = ctx->gather_uni[0]; p.uni_im = ctx->gather_uni[1];
       launch_gather(p, ctx->proj == PROJ_INVERSION, ctx->complex_coefficients, elt == DMV_C128, ctx->gather_narrow,
                     ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);

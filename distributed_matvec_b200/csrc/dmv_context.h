@@ -194,6 +194,7 @@ struct dmv_context {
   int opt_rows_ctas = 2;    // k_rows: resident CTAs per SM: 2 (122 registers, default) | 3 (80 registers) | 4 (64 registers)
   int opt_gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
                             // (measured slower), 2 per-lane walk from the bottom bit (round 1)
+  int opt_gather_split = -1;  // k_gather: lanes per row, -1 auto (choose_row_split), else 1 | 2 | 4 | 8 | 16 | 32
   DevBuf<unsigned char> d_table;
   DevBuf<unsigned char> d_mph_blocks, d_dense;   // dense index: perfect-hash blocks, dense table of (key, value) slots
   PerfectHash mph{};
@@ -382,6 +383,9 @@ const Binomials &binom();
 void select_index_mode(dmv_context *ctx);
 void install_directory(dmv_context *ctx);
 void upload_orbit(dmv_context *ctx);
+// lanes per row of a k_gather launch over `rows` rows with the tables of `g`: option "gather_split", else
+// choose_row_split (every k_gather launch and info("gather_split") take it from here)
+int gather_row_split(const dmv_context *g, int64_t rows);
 uint64_t fixed_hamming_rank(uint64_t s);
 uint64_t fixed_hamming_unrank(uint64_t r, int weight);
 void zero_y_if_diag(dmv_context *ctx, int elt, void *y);

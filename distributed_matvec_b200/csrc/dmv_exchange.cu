@@ -125,6 +125,7 @@ void setup_replicated(dmv_context *ctx) {
     ctx->global = g;
     g->opt_rows = ctx->opt_rows;
     g->opt_gather_walk = ctx->opt_gather_walk;
+    g->opt_gather_split = ctx->opt_gather_split;
     g->opt_rows_index = ctx->opt_rows_index;
     g->opt_rows_table = ctx->opt_rows_table;
     g->opt_rows_table_bits = ctx->opt_rows_table_bits;
@@ -177,7 +178,7 @@ void replicated_rows(dmv_context *ctx, int elt, const void *x_cat, void *y_dev) 
   p.x_row_offset = (int64_t)ctx->rank * ctx->repl_block;
   if (use_gather(g)) {
     select_tables(g, p, true, g->complex_coefficients);
-    p.row_split = choose_row_split(ctx->n_states, (int)g->h_pull.groups.size());
+    p.row_split = gather_row_split(g, ctx->n_states);
     p.uni_re = g->gather_uni[0]; p.uni_im = g->gather_uni[1];
     launch_gather(p, g->proj == PROJ_INVERSION, g->complex_coefficients, elt == DMV_C128, g->gather_narrow,
                   g->index_mode == INDEX_LIN, g->gather_uniform, ctx->stream);

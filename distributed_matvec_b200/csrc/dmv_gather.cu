@@ -285,13 +285,23 @@ __global__ void __launch_bounds__(kThreads) k_gather(const KernelParams p) {
       }
 
     if (valid && slice == 0) {
-      // diagonal (DMV:36-53) and the single store of y[i]; without diagonal terms y is accumulated into
+      // diagonal (DMV:36-53) and the single store of y[i]; without diagonal terms y is accumulated into.  A class
+      // holds up to 64 zz terms whatever the row width (NARROW counts sites and flip-mask groups, not zz terms): one of
+      // more than 32 terms is evaluated in 64 bits, else terms 32-63 would drop out of the mask and count as parallel
       double dre = 0.0, dim = 0.0;
       if (p.n_diag > 0) {
         for (int c = 0; c < p.n_diag_classes; ++c) {
           const DiagClass &D = s_dclass[c];
-          const W d0 = bp_gather<W>(D.p0, D.n0, b), d1 = bp_gather<W>(D.p1, D.n1, b);
-          const double wgt = (double)(D.count - 2 * popc_w((W)((d0 ^ d1) & (W)D.mask)));
+          int anti;
+          if (sizeof(W) == 8 || (D.mask >> 32) == 0) {
+            const W d0 = bp_gather<W>(D.p0, D.n0, b), d1 = bp_gather<W>(D.p1, D.n1, b);
+            anti = popc_w((W)((d0 ^ d1) & (W)D.mask));
+          } else {
+            const uint64_t d0 = bp_gather<uint64_t>(D.p0, D.n0, (uint64_t)b);
+            const uint64_t d1 = bp_gather<uint64_t>(D.p1, D.n1, (uint64_t)b);
+            anti = __popcll((d0 ^ d1) & D.mask);
+          }
+          const double wgt = (double)(D.count - 2 * anti);
           dre += wgt * D.v_re;
           dim += wgt * D.v_im;
         }

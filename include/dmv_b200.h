@@ -93,7 +93,11 @@ int dmv_synchronize(dmv_context *ctx);
  *                        state (six real / three complex vectors) through k_rows_batch | 0 vector by vector;
  *                        "rows_batch_min" = doubles per state (vectors x element width, default 2) from which it is used
  *          "gather_walk" = 0 every lane walks its emitting groups from the top bit | 1 group-major warp-uniform walk
- *                        (measured slower) | 2 from the bottom bit (round 1)
+ *                        (measured slower; only at row split 1, else walk 0) | 2 from the bottom bit (round 1); other
+ *                        values raise
+ *          "gather_split" = -1 auto (more lanes per row of k_gather on bases of fewer than 16 warps of rows per SM, never
+ *                        more lanes than flip-mask groups) | 1, 2, 4, 8, 16 or 32 lanes per row, each walking every
+ *                        S-th group; other values raise.  Applies to the single, batched and replicated-x products
  *          "index"    = -1 auto (identity / Lin tables / directory) | 0 directory + binary search | 2 combinadic rank
  *                        | 3 Lin tables (full fixed-Hamming bases)
  *          "bitparallel" = 1 | 0 walk the flip-mask groups one by one
@@ -108,7 +112,8 @@ int dmv_synchronize(dmv_context *ctx);
  * dmv_get_info: "index_mode", "pull", "gather", "rows", "rows_ok", "projection", "n_groups", "orbit_n_q", "orbit_n_t",
  *               "canon_mode", "torus_mode", "peer_direct", "replicated", "replicated_block", "peer_gather", "rounds",
  *               "global_states", "complex_coefficients", "rows_tk" (side of the square-torus orbit minimum k_rows is
- *               compiled for with the current options: 4 | 6, 0 the generic walk), ... (-1: unknown) */
+ *               compiled for with the current options: 4 | 6, 0 the generic walk), "gather_split" (lanes per row the next
+ *               single-rank k_gather launch uses), ... (-1: unknown) */
 int dmv_set_option(dmv_context *ctx, const char *name, int64_t value);
 int64_t dmv_get_info(const dmv_context *ctx, const char *name);
 
