@@ -1124,6 +1124,8 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "orbit_n_stages") return ctx->host_orbit.n_stages;
   if (key == "group_order") return ctx->host_orbit.group_order;
   if (key == "n_buckets") return (int64_t)ctx->n_buckets;
+  if (key == "expm_dot_vectors") return ctx->kr_dot_vectors;
+  if (key == "expm_combine_vectors") return ctx->kr_combine_vectors;
   return -1;
 }
 

@@ -328,6 +328,9 @@ struct dmv_context {
   // Lanczos work space (dmv_lanczos)
   DevBuf<double> lz_v[4];
   DevBuf<double> lz_scal;
+  // Krylov work space (dmv_expm_multiply): one allocation of (krylov_dim + 1) vectors, kept and reused between calls
+  DevBuf<double> kr_basis, kr_scal, kr_partials;
+  int64_t kr_dot_vectors = 0, kr_combine_vectors = 0;   // vector passes of the last call's block kernels
 
   ~dmv_context() {
     delete global;

@@ -196,6 +196,18 @@ void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const do
                            const double *coef2, double *out1, cudaStream_t s);
 void launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s);
 void launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s);
+// Krylov block kernels (dmv_solver.cu, used by dmv_expm_multiply): the stored vectors travel as a kernel parameter
+constexpr int kMaxBlockVectors = 65;
+struct VecList { const double *p[kMaxBlockVectors]; };
+// CTAs of the largest block launch over n elements: `partials` must hold that many * (J + 1) * 2 doubles
+int block_partials_grid(int64_t n, bool complex_elements);
+// h[2k], h[2k + 1] = <V_k, w> for k < J (real vectors: imaginary part 0), h[2J] = |w|^2; w is read once
+void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
+                      double *h, cudaStream_t s);
+// out = a w - sum_{k < J} c_k V_k (c: J interleaved complex coefficients in device memory; w may be null, out may alias
+// w), nrm2[0] = |out|^2
+void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
+                          const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s);
 int64_t launch_counter();
 int planned_grid(int64_t rows, int row_split);
 int choose_row_split(int64_t rows, int n_groups);

@@ -1,0 +1,282 @@
+// dmv_krylov.cu -- dmv_expm_multiply: y = exp(z H) x for a Hermitian H by the Lanczos approximation with adaptive
+// sub-steps (Saad 1992; Hochbruck & Lubich 1997).  Every vector stays in HBM; the Krylov basis is orthogonalised in
+// full with the fused block kernels of dmv_solver.cu, and only the reduced scalars of each step visit the host, where
+// the small tridiagonal problem is solved.
+#include <cfloat>
+#include <complex>
+
+#include "dmv_context.h"
+
+namespace dmv { namespace host {
+
+using cplx = std::complex<double>;
+
+// Eigen-decomposition T = Q diag(lam) Q^T of the symmetric tridiagonal T (diagonal a[0..k), off-diagonal b[0..k-1)) by
+// the implicit QL method with Wilkinson shifts; q[r * k + i] = component r of eigenvector i.
+struct TridiagonalEigen {
+  int k = 0;
+  std::vector<double> lam, q;
+  TridiagonalEigen(const std::vector<double> &a, const std::vector<double> &b) {
+    k = (int)a.size();
+    lam = a;
+    std::vector<double> e(k, 0.0);
+    for (int i = 0; i + 1 < k; ++i) e[i] = b[i];
+    q.assign((size_t)k * k, 0.0);
+    for (int i = 0; i < k; ++i) q[(size_t)i * k + i] = 1.0;
+    std::vector<double> &d = lam;
+    for (int l = 0; l < k; ++l) {
+      for (int iter = 0;; ++iter) {
+        int m = l;
+        for (; m + 1 < k; ++m)   // the first negligible off-diagonal element at or below l splits the matrix
+          if (std::fabs(e[m]) <= DBL_EPSILON * (std::fabs(d[m]) + std::fabs(d[m + 1]))) break;
+        if (m == l) break;
+        if (iter == 200) throw std::runtime_error("tridiagonal eigensolver did not converge");
+        double g = (d[l + 1] - d[l]) / (2.0 * e[l]);   // Wilkinson shift from the leading 2 x 2 block
+        double r = std::hypot(g, 1.0);
+        g = d[m] - d[l] + e[l] / (g + std::copysign(r, g));
+        double s = 1.0, c = 1.0, p = 0.0;
+        bool underflow = false;
+        for (int i = m - 1; i >= l; --i) {   // chase the bulge up with plane rotations
+          double f = s * e[i];
+          const double bb = c * e[i];
+          r = std::hypot(f, g);
+          e[i + 1] = r;
+          if (r == 0.0) { d[i + 1] -= p; e[m] = 0.0; underflow = true; break; }
+          s = f / r;
+          c = g / r;
+          g = d[i + 1] - p;
+          r = (d[i] - g) * s + 2.0 * c * bb;
+          p = s * r;
+          d[i + 1] = g + p;
+          g = c * r - bb;
+          for (int t = 0; t < k; ++t) {
+            double *row = &q[(size_t)t * k];
+            f = row[i + 1];
+            row[i + 1] = s * row[i] + c * f;
+            row[i] = c * row[i] - s * f;
+          }
+        }
+        if (underflow) continue;
+        d[l] -= p;
+        e[l] = g;
+        e[m] = 0.0;
+      }
+    }
+  }
+  // c = exp(w T) e_1
+  void exp_e1(cplx w, std::vector<cplx> &c) const {
+    c.assign(k, cplx(0.0, 0.0));
+    for (int i = 0; i < k; ++i) {
+      const cplx f = std::exp(w * lam[i]) * q[i];   // q[0 * k + i]: first component of eigenvector i
+      for (int r = 0; r < k; ++r) c[r] += q[(size_t)r * k + i] * f;
+    }
+  }
+  // e_k^T phi_1(w T) e_1 with phi_1(x) = (e^x - 1) / x
+  cplx phi1_last(cplx w) const {
+    cplx s(0.0, 0.0);
+    for (int i = 0; i < k; ++i) s += q[(size_t)(k - 1) * k + i] * q[i] * phi1(w * lam[i]);
+    return s;
+  }
+  static cplx phi1(cplx x) {
+    if (std::abs(x) >= 0.5) return (std::exp(x) - 1.0) / x;
+    cplx s(1.0, 0.0);   // Taylor series sum_j x^j / (j + 1)!, Horner form; |x| < 0.5: the term j = 17 is < 1e-22
+    for (int j = 17; j >= 1; --j) s = 1.0 + s * x / (double)(j + 1);
+    return s;
+  }
+};
+
+} }  // namespace dmv::host
+
+extern "C" {
+
+// ---- y = exp(z H) x on the device (DESIGN.md section 3, "dmv_expm_multiply").  Per sub-step of length h (a fraction of z):
+// Lanczos with full (DGKS) reorthogonalisation builds V_0 .. V_{k-1} and T_k from w / |w|; on the host,
+// c = exp(h z T_k) e_1 and the error estimate  beta * beta_k * |h z| * |e_k^T phi_1(h z T_k) e_1|  (Saad's corrected
+// estimate: the norm of the next term of the Krylov expansion); h is halved until the estimate is <= tol * h * beta, and
+// w <- beta * sum_j c_j V_j.  The Krylov space is built once per sub-step: shrinking h costs host arithmetic only.
+int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const void *x, void *y, int krylov_dim,
+                      double tol, int *products, double *error_estimate) {
+  API_BEGIN
+  if (products) *products = 0;
+  if (error_estimate) *error_estimate = 0.0;
+  use_device(ctx);
+  require_states(ctx);
+  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  if (krylov_dim != 0 && (krylov_dim < 2 || krylov_dim > kMaxBlockVectors - 1))
+    throw std::runtime_error("krylov_dim must be 0 (default 30) or between 2 and 64");
+  if (!(tol > 0.0) || !std::isfinite(tol)) throw std::runtime_error("tol must be positive and finite");
+  if (!std::isfinite(z_re) || !std::isfinite(z_im)) throw std::runtime_error("z must be finite");
+  if (elt == DMV_F64 && z_im != 0.0)
+    throw std::runtime_error("a complex z needs complex vectors (DMV_C128)");
+  if (elt == DMV_F64 && ctx->complex_coefficients)
+    throw std::runtime_error("the operator or its characters are complex: use complex vectors (DMV_C128)");
+  if (!x || !y) throw std::runtime_error("x and y must not be null");
+  const int P = ctx->num_ranks;
+  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_expm_multiply on several ranks needs dmv_comm_init");
+  const int m = krylov_dim == 0 ? 30 : krylov_dim;
+  const int64_t n = ctx->n_states;
+  const size_t words = (size_t)n * elt;
+  const bool ce = elt == DMV_C128;
+  const cplx z(z_re, z_im);
+  cudaStream_t st = ctx->stream;
+  ctx->kr_dot_vectors = ctx->kr_combine_vectors = 0;
+  if (z == cplx(0.0, 0.0)) {   // exp(0) = 1: x itself, bit for bit
+    if (x != y && words) CUDA_CHECK(cudaMemcpyAsync(y, x, words * 8, cudaMemcpyDefault, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    return 0;
+  }
+  // the basis: one allocation of m + 1 vectors, kept for the next call; never shrunk silently to what fits
+  const size_t basis_words = (size_t)(m + 1) * std::max<size_t>(words, 1);
+  if (ctx->kr_basis.count < basis_words) {
+    ctx->kr_basis.release();
+    size_t free_b = 0, total_b = 0;
+    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    const size_t need = basis_words * sizeof(double);
+    if (need > free_b)
+      throw std::runtime_error("dmv_expm_multiply: the Krylov basis of krylov_dim + 1 = " + std::to_string(m + 1) +
+                               " vectors of " + std::to_string(n) + " elements needs " + std::to_string(need) +
+                               " bytes, but only " + std::to_string(free_b) +
+                               " bytes are free on the device; use a smaller krylov_dim");
+    ctx->kr_basis.alloc(basis_words);
+  }
+  // scalars: [0, 2 * 66) block dot results, [132, 134) |out|^2 of a combine, [136, 136 + 2 * 65) host coefficients
+  constexpr int kNrm = 2 * (kMaxBlockVectors + 1), kCoef = kNrm + 4;
+  ctx->kr_scal.alloc(kCoef + 2 * kMaxBlockVectors);
+  ctx->kr_partials.alloc((size_t)block_partials_grid(n, ce) * (kMaxBlockVectors + 1) * 2);
+  double *scal = ctx->kr_scal.ptr, *partials = ctx->kr_partials.ptr;
+  std::vector<double *> vp(m + 1);
+  for (int k = 0; k <= m; ++k) vp[k] = ctx->kr_basis.ptr + (size_t)k * words;
+  VecList list{};
+  auto set_list = [&](int J) { for (int k = 0; k < J; ++k) list.p[k] = vp[k]; };
+  // sum `count` scalars at `d` over the ranks (NCCL, on the device buffer)
+  auto all_reduce = [&](double *d, int count) {
+    if (P > 1) NCCL_CHECK(nccl().AllReduce(d, d, (size_t)count, ncclDouble, ncclSum, ctx->comm, st));
+  };
+  auto fetch = [&](double *h, const double *d, int count) {
+    CUDA_CHECK(cudaMemcpyAsync(h, d, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
+  };
+  auto product = [&](const double *in, double *out) {
+    CUDA_CHECK(cudaMemsetAsync(out, 0, words * 8, st));   // operators without a diagonal accumulate into y (DMV:1062-1069)
+    const int rc = P == 1 ? dmv_local_matvec(ctx, elt, in, out) : dmv_matvec(ctx, elt, in, out);
+    if (rc) throw std::runtime_error(g_last_error);
+  };
+  // Krylov space exhausted at the GLOBAL dimension: every rank takes the same decision (as dmv_lanczos)
+  int64_t n_global = n;
+  if (P > 1) {
+    const double mine = (double)n;
+    CUDA_CHECK(cudaMemcpyAsync(scal, &mine, sizeof(double), cudaMemcpyHostToDevice, st));
+    all_reduce(scal, 1);
+    double g = 0.0;
+    fetch(&g, scal, 1);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    n_global = (int64_t)std::llround(g);
+  }
+  // w = x (host or device; y may alias x: x is read in full before y is written)
+  if (words) CUDA_CHECK(cudaMemcpyAsync(vp[0], x, words * 8, cudaMemcpyDefault, st));
+  std::vector<double> hh(kNrm + 2), h2(kNrm + 2);
+  launch_block_dot(n, ce, list, 0, vp[0], partials, scal, st);
+  ctx->kr_dot_vectors += 1;
+  all_reduce(scal, 2);
+  fetch(hh.data(), scal, 2);
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  double beta = std::sqrt(std::max(0.0, hh[0]));
+  double remaining = 1.0, err_sum = 0.0;
+  int prods = 0;
+  std::vector<double> alpha, betas, coef(2 * kMaxBlockVectors);
+  std::vector<cplx> c;
+  while (remaining > 0.0 && beta > 0.0 && std::isfinite(beta)) {
+    launch_scale((int64_t)words, 1.0 / beta, vp[0], vp[0], false, st);   // V_0 = w / beta
+    alpha.clear();
+    betas.clear();
+    int k = 0;
+    double beta_k = 0.0;
+    bool exact = false;
+    for (int j = 0; j < m; ++j) {
+      double *u = vp[j + 1];
+      product(vp[j], u);
+      ++prods;
+      const int J = j + 1;
+      set_list(J);
+      // h = V^H u (and |u|^2), reduced over the ranks on the device; u -= V h reads h from there: no host round trip
+      launch_block_dot(n, ce, list, J, u, partials, scal, st);
+      all_reduce(scal, 2 * (J + 1));
+      launch_block_combine(n, ce, 1.0, u, list, J, scal, u, partials, scal + kNrm, st);
+      all_reduce(scal + kNrm, 2);
+      ctx->kr_dot_vectors += J + 1;
+      ctx->kr_combine_vectors += J + 2;
+      fetch(hh.data(), scal, 2 * (J + 1));
+      fetch(hh.data() + kNrm, scal + kNrm, 2);
+      CUDA_CHECK(cudaStreamSynchronize(st));
+      const double before = std::sqrt(std::max(0.0, hh[2 * J]));
+      double after = std::sqrt(std::max(0.0, hh[kNrm]));
+      double a_j = hh[2 * j];
+      if (after < 0.7 * before) {   // DGKS: the pass cancelled most of u, so orthogonalise once more
+        launch_block_dot(n, ce, list, J, u, partials, scal, st);
+        all_reduce(scal, 2 * (J + 1));
+        launch_block_combine(n, ce, 1.0, u, list, J, scal, u, partials, scal + kNrm, st);
+        all_reduce(scal + kNrm, 2);
+        ctx->kr_dot_vectors += J + 1;
+        ctx->kr_combine_vectors += J + 2;
+        fetch(h2.data(), scal, 2 * (J + 1));
+        fetch(h2.data() + kNrm, scal + kNrm, 2);
+        CUDA_CHECK(cudaStreamSynchronize(st));
+        a_j += h2[2 * j];
+        after = std::sqrt(std::max(0.0, h2[kNrm]));
+      }
+      alpha.push_back(a_j);
+      k = J;
+      beta_k = after;
+      // happy breakdown: H V_j lies in the span (to rounding), or the space is the whole basis -- the step is exact
+      if (after <= 1e-14 * before || (int64_t)k >= n_global) { exact = true; break; }
+      if (J < m) {
+        betas.push_back(after);
+        launch_scale((int64_t)words, 1.0 / after, u, u, false, st);
+      }
+    }
+    const dmv::host::TridiagonalEigen T(alpha, betas);
+    double h = remaining, err = 0.0;
+    if (!exact) {
+      for (int halvings = 0;; ++halvings) {
+        err = beta * beta_k * std::abs(h * z) * std::abs(T.phi1_last(h * z));
+        if (err <= tol * h * beta) break;
+        if (halvings == 200)
+          throw std::runtime_error("dmv_expm_multiply: no sub-step of at least 2^-200 of z meets tol; raise "
+                                   "krylov_dim or tol");
+        h *= 0.5;
+      }
+    }
+    T.exp_e1(h * z, c);
+    for (int i = 0; i < k; ++i) { coef[2 * i] = -beta * c[i].real(); coef[2 * i + 1] = -beta * c[i].imag(); }
+    CUDA_CHECK(cudaMemcpyAsync(scal + kCoef, coef.data(), sizeof(double) * 2 * k, cudaMemcpyHostToDevice, st));
+    set_list(k);
+    launch_block_combine(n, ce, 0.0, nullptr, list, k, scal + kCoef, vp[m], partials, scal + kNrm, st);
+    ctx->kr_combine_vectors += k + 1;
+    all_reduce(scal + kNrm, 2);
+    fetch(hh.data() + kNrm, scal + kNrm, 2);
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    std::swap(vp[0], vp[m]);   // w = beta sum_j c_j V_j becomes the start of the next sub-step
+    beta = std::sqrt(std::max(0.0, hh[kNrm]));
+    err_sum += err;
+    remaining = h == remaining ? 0.0 : remaining - h;
+  }
+  if (words) CUDA_CHECK(cudaMemcpyAsync(y, vp[0], words * 8, cudaMemcpyDefault, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  if (products) *products = prods;
+  if (error_estimate) *error_estimate = err_sum;
+  check_status(ctx);
+  API_END
+}
+
+// host-only self-check entry for the tridiagonal exponential behind dmv_expm_multiply (no device needed)
+int dmv_debug_tridiagonal_expm(int k, const double *a, const double *b, double z_re, double z_im, double *c) {
+  API_BEGIN
+  if (k < 1) throw std::runtime_error("empty matrix");
+  std::vector<double> av(a, a + k), bv(b, b + (k - 1));
+  const dmv::host::TridiagonalEigen T(av, bv);
+  std::vector<dmv::host::cplx> out;
+  T.exp_e1(dmv::host::cplx(z_re, z_im), out);
+  for (int i = 0; i < k; ++i) { c[2 * i] = out[i].real(); c[2 * i + 1] = out[i].imag(); }
+  API_END
+}
+
+}  // extern "C"

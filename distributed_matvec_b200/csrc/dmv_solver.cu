@@ -1,8 +1,10 @@
 // dmv_solver.cu -- vector kernels of the device-resident Lanczos iteration (the consumer of the hot path; the reference
 // drives its product from PRIMME's matvec callback, src/Diagonalize.chpl:134-225, src/PRIMME.chpl:267-373).
 // Everything stays in HBM between products: y = H v, alpha = <v, y>, y -= alpha v + beta v_prev, beta' = |y|.
+// Also the block kernels of dmv_expm_multiply (dmv_krylov.cu): h = V^H w and out = a w - V c over many stored vectors.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <stdexcept>
 #include <string>
 
@@ -99,6 +101,174 @@ __global__ void __launch_bounds__(kThreads) k_fill(int64_t m, uint64_t seed, uin
   }
 }
 
+// ---- block kernels of dmv_expm_multiply (full reorthogonalisation against up to kMaxBlockVectors stored vectors).
+// Every reduction is deterministic: each CTA sums its warps in a fixed order into its own slot of `partials`, and
+// k_reduce_partials sums the CTAs in a fixed order -- no floating-point atomics, so a repeated call is bit-identical.
+
+// elements per thread and tile of k_block_dot: 32 bytes of every vector per thread and tile
+template <bool CE> __host__ __device__ constexpr int dot_elems() { return CE ? 2 : 4; }
+constexpr int kDotChunk = 8;   // vectors whose accumulators are held in registers at once
+
+// partials[(blockIdx * (J + 1) + k) * 2 + {0, 1}] = this CTA's share of <V_k, w> (k < J) and of |w|^2 (k == J)
+template <bool CE>
+__global__ void __launch_bounds__(kThreads) k_block_dot(int64_t n, VecList V, int J, const double *__restrict__ w,
+                                                        double *__restrict__ partials) {
+  constexpr int E = dot_elems<CE>();
+  __shared__ double s_acc[kThreads / 32][kMaxBlockVectors + 1][2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int k = lane; k <= J; k += 32) s_acc[warp][k][0] = s_acc[warp][k][1] = 0.0;   // warp-private rows
+  __syncwarp();
+  const int64_t tile = (int64_t)kThreads * E;
+  for (int64_t base = (int64_t)blockIdx.x * tile; base < n; base += (int64_t)gridDim.x * tile) {
+    double wr[E], wi[E];
+    unsigned in = 0;   // bit e: element e of this thread's tile exists
+    double nrm = 0.0;
+#pragma unroll
+    for (int e = 0; e < E; ++e) {   // w is read once per tile; the vectors stream past it in chunks
+      const int64_t i = base + (int64_t)e * kThreads + threadIdx.x;
+      wr[e] = wi[e] = 0.0;
+      if (i < n) {
+        in |= 1u << e;
+        if (CE) { const double2 t = reinterpret_cast<const double2 *>(w)[i]; wr[e] = t.x; wi[e] = t.y; }
+        else wr[e] = w[i];
+      }
+      nrm += wr[e] * wr[e] + wi[e] * wi[e];
+    }
+    nrm = warp_sum(nrm);
+    if (lane == 0) s_acc[warp][J][0] += nrm;
+    for (int k0 = 0; k0 < J; k0 += kDotChunk) {
+      double ar[kDotChunk], ai[kDotChunk];
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {
+        ar[kk] = ai[kk] = 0.0;
+        if (k0 + kk < J) {
+          const double *v = V.p[k0 + kk];
+#pragma unroll
+          for (int e = 0; e < E; ++e) {
+            if (!(in >> e & 1u)) continue;
+            const int64_t i = base + (int64_t)e * kThreads + threadIdx.x;
+            if (CE) {   // conj(v) * w
+              const double2 t = __ldg(reinterpret_cast<const double2 *>(v) + i);
+              ar[kk] += t.x * wr[e] + t.y * wi[e];
+              ai[kk] += t.x * wi[e] - t.y * wr[e];
+            } else {
+              ar[kk] += __ldg(v + i) * wr[e];
+            }
+          }
+        }
+      }
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {
+        if (k0 + kk >= J) break;
+        const double r = warp_sum(ar[kk]);
+        const double im = CE ? warp_sum(ai[kk]) : 0.0;
+        if (lane == 0) { s_acc[warp][k0 + kk][0] += r; s_acc[warp][k0 + kk][1] += im; }
+      }
+    }
+  }
+  __syncthreads();
+  for (int k = threadIdx.x; k <= J; k += blockDim.x) {
+    double re = 0.0, im = 0.0;
+#pragma unroll
+    for (int q = 0; q < kThreads / 32; ++q) { re += s_acc[q][k][0]; im += s_acc[q][k][1]; }
+    partials[((int64_t)blockIdx.x * (J + 1) + k) * 2] = re;
+    partials[((int64_t)blockIdx.x * (J + 1) + k) * 2 + 1] = im;
+  }
+}
+
+// out = a w - sum_k c_k V_k (w may be null: a w = 0; out may alias w), c interleaved (re, im) in device memory (real
+// vectors use the real parts); partials[blockIdx * 2] = this CTA's share of |out|^2
+template <bool CE>
+__global__ void __launch_bounds__(kThreads) k_block_combine(int64_t n, double a, const double *w, VecList V, int J,
+                                                            const double *__restrict__ coef, double *out,
+                                                            double *__restrict__ partials) {
+  __shared__ double s_c[kMaxBlockVectors][2];
+  __shared__ double s[kThreads / 32];
+  for (int k = threadIdx.x; k < J; k += blockDim.x) { s_c[k][0] = coef[2 * k]; s_c[k][1] = coef[2 * k + 1]; }
+  __syncthreads();
+  double nrm = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    double re = 0.0, im = 0.0;
+    if (w) {
+      if (CE) { const double2 t = reinterpret_cast<const double2 *>(w)[i]; re = a * t.x; im = a * t.y; }
+      else re = a * w[i];
+    }
+    for (int k0 = 0; k0 < J; k0 += kDotChunk) {
+      double vr[kDotChunk], vi[kDotChunk];
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {   // issue the chunk's loads before the first use
+        vr[kk] = vi[kk] = 0.0;
+        if (k0 + kk < J) {
+          if (CE) { const double2 t = __ldg(reinterpret_cast<const double2 *>(V.p[k0 + kk]) + i); vr[kk] = t.x; vi[kk] = t.y; }
+          else vr[kk] = __ldg(V.p[k0 + kk] + i);
+        }
+      }
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {
+        if (k0 + kk >= J) break;
+        const double cr = s_c[k0 + kk][0], ci = s_c[k0 + kk][1];
+        if (CE) { re -= cr * vr[kk] - ci * vi[kk]; im -= cr * vi[kk] + ci * vr[kk]; }
+        else re -= cr * vr[kk];
+      }
+    }
+    if (CE) reinterpret_cast<double2 *>(out)[i] = make_double2(re, im);
+    else out[i] = re;
+    nrm += re * re + im * im;
+  }
+  nrm = warp_sum(nrm);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) s[warp] = nrm;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) t += s[q];
+    partials[2 * blockIdx.x] = t;
+    partials[2 * blockIdx.x + 1] = 0.0;
+  }
+}
+
+// out[2k + {0, 1}] = sum over the `blocks` CTAs of partials[(b * width + k) * 2 + {0, 1}], in a fixed order; one CTA per k
+__global__ void __launch_bounds__(kThreads) k_reduce_partials(int blocks, int width, const double *__restrict__ partials,
+                                                              double *__restrict__ out) {
+  const int k = blockIdx.x;
+  double re = 0.0, im = 0.0;
+  for (int b = threadIdx.x; b < blocks; b += blockDim.x) {
+    re += partials[((int64_t)b * width + k) * 2];
+    im += partials[((int64_t)b * width + k) * 2 + 1];
+  }
+  __shared__ double s_re[kThreads / 32], s_im[kThreads / 32];
+  re = warp_sum(re);
+  im = warp_sum(im);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { s_re[warp] = re; s_im[warp] = im; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double r = 0.0, i = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) { r += s_re[q]; i += s_im[q]; }
+    out[2 * k] = r;
+    out[2 * k + 1] = i;
+  }
+}
+
+int sm_count() {
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return sms > 0 ? sms : 132;
+}
+
+// one wave of resident CTAs (at least one, so that an empty block still writes its partials)
+template <typename K>
+int one_wave(K kernel, int64_t work_items) {
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
+  if (per_sm < 1) per_sm = 1;
+  int64_t b = (work_items + kThreads - 1) / kThreads;
+  b = std::min<int64_t>(std::max<int64_t>(b, 1), (int64_t)sm_count() * per_sm);
+  return (int)b;
+}
+
 int blocks_for(int64_t n) {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
@@ -144,6 +314,46 @@ void launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaS
   if (words <= 0) return;
   k_fill<<<blocks_for(words), kThreads, 0, s>>>(words, seed, offset, x);
   check("k_fill");
+}
+
+int block_partials_grid(int64_t n, bool complex_elements) {
+  const int64_t tiles = (std::max<int64_t>(n, 0) + (complex_elements ? 2 : 4) - 1) / (complex_elements ? 2 : 4);
+  const int a = complex_elements ? one_wave(k_block_dot<true>, tiles) : one_wave(k_block_dot<false>, tiles);
+  const int b = complex_elements ? one_wave(k_block_combine<true>, n) : one_wave(k_block_combine<false>, n);
+  return std::max(a, b);
+}
+
+void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
+                      double *h, cudaStream_t s) {
+  if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_dot: bad number of vectors");
+  const int64_t tiles = (std::max<int64_t>(n, 0) + (complex_elements ? 2 : 4) - 1) / (complex_elements ? 2 : 4);
+  int grid;
+  if (complex_elements) {
+    grid = one_wave(k_block_dot<true>, tiles);
+    k_block_dot<true><<<grid, kThreads, 0, s>>>(n, V, J, w, partials);
+  } else {
+    grid = one_wave(k_block_dot<false>, tiles);
+    k_block_dot<false><<<grid, kThreads, 0, s>>>(n, V, J, w, partials);
+  }
+  check("k_block_dot");
+  k_reduce_partials<<<J + 1, kThreads, 0, s>>>(grid, J + 1, partials, h);
+  check("k_reduce_partials");
+}
+
+void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
+                          const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s) {
+  if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_combine: bad number of vectors");
+  int grid;
+  if (complex_elements) {
+    grid = one_wave(k_block_combine<true>, n);
+    k_block_combine<true><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
+  } else {
+    grid = one_wave(k_block_combine<false>, n);
+    k_block_combine<false><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
+  }
+  check("k_block_combine");
+  k_reduce_partials<<<1, kThreads, 0, s>>>(grid, 1, partials, nrm2);
+  check("k_reduce_partials");
 }
 
 }  // namespace dmv

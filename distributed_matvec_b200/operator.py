@@ -307,6 +307,24 @@ class Operator:
                                         vec.ctypes.data if eigenvector else None, C.byref(it), C.byref(res)))
         return float(e.value), vec, int(it.value), float(res.value)
 
+    def expm_multiply(self, x, z, krylov_dim: int = 0, tol: float = 1e-10):
+        """y = exp(z H) x on the device (dmv_expm_multiply): real time is z = -1j * t, imaginary time z = -tau.
+        x: numpy array or torch CUDA tensor (float64 only for a real z and a real operator); y has the same kind.
+        Collective when num_ranks > 1.  -> (y, products of H applied, sum of the local error estimates)"""
+        elt = _elt_of(x)
+        self._check_vec(x, "x")
+        z = complex(z)
+        if _is_torch(x):
+            import torch
+            self.use_torch_stream()
+            y = torch.empty_like(x)
+        else:
+            y = np.empty_like(x)
+        prods, err = C.c_int(), C.c_double()
+        nat.check(nat.lib().dmv_expm_multiply(self._ctx, elt, z.real, z.imag, _ptr(x), _ptr(y), int(krylov_dim),
+                                              float(tol), C.byref(prods), C.byref(err)))
+        return y, int(prods.value), float(err.value)
+
     # -- replicated-x form of the distributed product (dmv_replicated_*), for hosts that own the all-gather -------
     def replicated_setup(self) -> int:
         """Build the whole basis and the slot table on this rank; returns the slot size (elements per rank)."""

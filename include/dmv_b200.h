@@ -234,6 +234,21 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
 int dmv_lanczos(dmv_context *ctx, int elt, int max_iters, double tol, uint64_t seed, double *eigenvalue,
                 void *eigenvector, int *iterations, double *residual);
 
+/* ---- time evolution on the device: y = exp(z H) x for a Hermitian H (every model the reference takes) by the Lanczos
+ * approximation with adaptive sub-steps and full reorthogonalisation; the Krylov basis stays in HBM, dot products are
+ * reduced over the ranks with NCCL and only a few scalars per step visit the host.  z = (z_re, z_im): real time is
+ * z = -i t, imaginary time is z = -tau.  elt = DMV_C128 always; DMV_F64 only when z_im == 0 and the operator and
+ * characters are real (info "complex_coefficients" == 0).  x, y: host or device pointers of dmv_number_states elements;
+ * y may alias x.  krylov_dim: 0 = default (30), else 2..64; the basis is one context-owned allocation of
+ * (krylov_dim + 1) * dmv_number_states elements, kept for later calls, and the call fails (naming the bytes needed)
+ * when it does not fit.  tol > 0: bound on the estimated error per unit of z, relative to the norm of the vector each
+ * sub-step starts from.  Collective when num_ranks > 1 (needs dmv_comm_init), like dmv_lanczos.
+ * products (may be NULL): products of H applied; error_estimate (may be NULL): sum of the local estimates.
+ * dmv_get_info "expm_dot_vectors" / "expm_combine_vectors": vectors read or written by the block kernels of the last
+ * call (for bandwidth accounting). */
+int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const void *x, void *y,
+                      int krylov_dim, double tol, int *products, double *error_estimate);
+
 /* ---- per-stage timings of the last product, in milliseconds (the reference's timing tree,
  * DMV:1028-1052).  names: see dmv_timing_name(i); returns the number of stages. */
 int dmv_last_timings(dmv_context *ctx, double *ms, int capacity);
@@ -294,6 +309,9 @@ void ls_chpl_enumerate_representatives(const void *ls_hs_basis_ptr, uint64_t low
  *   functions compiled for the host, inserts them in order and looks every one up again: block[k] = prefix block of
  *   reps[k], home[k] = its home bucket, probes[k] = buckets its look-up reads.  Fails when a state is not found. */
 int dmv_debug_tridiagonal_lowest(int k, const double *diag, const double *offdiag, double *eigenvalue, double *vector);
+/* dmv_debug_tridiagonal_expm: host half of dmv_expm_multiply, c = exp(z T) e_1 for the symmetric tridiagonal T
+ *   (diag a[0..k), off-diag b[0..k-1)), c interleaved (re, im), 2k doubles */
+int dmv_debug_tridiagonal_expm(int k, const double *a, const double *b, double z_re, double z_im, double *c);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
