@@ -149,18 +149,18 @@ HostTables build_tables(const std::map<uint64_t, std::vector<OffTerm>> &by_x) {
 }
 
 bool use_gather(const dmv_context *ctx) {   // the lean row-gather kernel applies and is not switched off
-  return ctx->gather_ok && ctx->opt_gather != 0 && ctx->opt_bitparallel != 0 && ctx->proj != PROJ_GROUP;
+  return ctx->gather_ok && ctx->opt.gather != 0 && ctx->opt.bitparallel != 0 && ctx->proj != PROJ_GROUP;
 }
 bool use_rows(const dmv_context *ctx) {   // the pipelined row kernel for bases with permutation symmetries
-  return ctx->rows_ok && ctx->opt_rows != 0 && ctx->opt_bitparallel != 0 && ctx->orbit.trivial_characters;
+  return ctx->rows_ok && ctx->opt.rows != 0 && ctx->opt.bitparallel != 0 && ctx->orbit.trivial_characters;
 }
 bool use_pull(const dmv_context *ctx) {
   // auto: one rank, bit-parallel operator, no permutation symmetries -> k_gather (rows, no atomics, see
   // dmv_gather.cu); everything else -> push (k_generate).  "mode" = 1 forces the row traversal (k_gather
   // when it applies, else the queued k_pull), "mode" = 0 the scatter form.
   if (ctx->num_ranks != 1) return false;
-  if (ctx->opt_mode == 1) return true;
-  return ctx->opt_mode == -1 && (use_gather(ctx) || use_rows(ctx));
+  if (ctx->opt.mode == 1) return true;
+  return ctx->opt.mode == -1 && (use_gather(ctx) || use_rows(ctx));
 }
 
 void use_device(const dmv_context *ctx) { CUDA_CHECK(cudaSetDevice(ctx->device)); }
@@ -168,7 +168,7 @@ void use_device(const dmv_context *ctx) { CUDA_CHECK(cudaSetDevice(ctx->device))
 bool complex_values(const dmv_context *ctx, int elt) { return elt == DMV_C128 || ctx->complex_coefficients; }
 
 int gather_row_split(const dmv_context *g, int64_t rows) {
-  if (g->opt_gather_split > 0) return g->opt_gather_split;
+  if (g->opt.gather_split > 0) return g->opt.gather_split;
   return choose_row_split(rows, (int)g->h_pull.groups.size());
 }
 
@@ -212,8 +212,8 @@ KernelParams base_params(dmv_context *ctx) {
   p.status = ctx->d_status.ptr;
   p.row_begin = 0;
   p.row_end = ctx->n_states;
-  p.gather_walk = ctx->opt_gather_walk;
-  p.rows_ctas = ctx->opt_rows_ctas;
+  p.gather_walk = ctx->opt.gather_walk;
+  p.rows_ctas = ctx->opt.rows_ctas;
   return p;
 }
 
@@ -282,7 +282,7 @@ void select_tables(dmv_context *ctx, KernelParams &p, bool pull, bool complex_va
   p.terms = d.terms.ptr; p.n_terms = (int)h.terms.size();
   p.any_generic = h.any_generic ? 1 : 0;
   p.any_s_out = h.any_s_out ? 1 : 0;
-  p.bp = d.bp.ptr; p.n_bp = (ctx->opt_bitparallel != 0) ? (int)h.bp.size() : 0;
+  p.bp = d.bp.ptr; p.n_bp = (ctx->opt.bitparallel != 0) ? (int)h.bp.size() : 0;
 }
 
 void require_states(const dmv_context *ctx) {
@@ -315,7 +315,7 @@ void select_index_mode(dmv_context *ctx) {
   ctx->index_mode = INDEX_DIRECTORY;
   if (ctx->identity_index && ctx->num_ranks == 1) { ctx->index_mode = INDEX_IDENTITY; return; }
   const int n = ctx->n_sites, w = ctx->hamming_weight;
-  const int want = ctx->opt_index;
+  const int want = ctx->opt.index;
   if (want == 0) return;
   const bool eligible = ctx->num_ranks == 1 && w >= 0 && ctx->proj != PROJ_GROUP;
   if (!eligible) return;
@@ -446,9 +446,9 @@ void upload_orbit(dmv_context *ctx) {
   P.tor_frow = ctx->d_tor_frow.ptr;
   P.tor_net_mask = ctx->d_tor_net_mask.ptr;
   P.tor_net_delta = ctx->d_tor_net_delta.ptr;
-  if (ctx->opt_canon >= 0) { P.tor_mode = 0; P.chain_dihedral = 0; }   // 1: round-1 forms (coset chain / four run searches)
-  if (ctx->opt_canon == 2) { P.canon_lut2 = nullptr; P.cc_n = 0; P.cc_stages = 0; }   // first version: single-block LUT, independent networks
-  if (ctx->opt_canon == 0) P.canon_mode = 0;
+  if (ctx->opt.canon >= 0) { P.tor_mode = 0; P.chain_dihedral = 0; }   // 1: round-1 forms (coset chain / four run searches)
+  if (ctx->opt.canon == 2) { P.canon_lut2 = nullptr; P.cc_n = 0; P.cc_stages = 0; }   // first version: single-block LUT, independent networks
+  if (ctx->opt.canon == 0) P.canon_mode = 0;
   ctx->orbit = P;
 }
 
@@ -588,7 +588,7 @@ void ensure_table(dmv_context *ctx, int elt) {
   const uint64_t *left_keys = ctx->d_reps.ptr;
   int64_t n_left = n;
   DevBuf<uint64_t> d_left[2];
-  ctx->dense_index = ctx->opt_rows_index == 1 && n >= 1;
+  ctx->dense_index = ctx->opt.rows_index == 1 && n >= 1;
   ctx->mph = PerfectHash{};
   if (ctx->dense_index) {
     if (n >= 2147483647ll) throw std::runtime_error("k_rows: more than 2^31 states");
@@ -641,13 +641,13 @@ void ensure_table(dmv_context *ctx, int elt) {
     CUDA_CHECK(cudaMemsetAsync(ctx->d_dense.ptr, 0xff, dense_bytes, st));
   }
   // ---- open-addressing table over the states that are left (all of them without the dense index)
-  // complex128, hashed: one-slot buckets, 8 per state (1.07 probes per look-up); ordered: opt_rows_table_buckets per
+  // complex128, hashed: one-slot buckets, 8 per state (1.07 probes per look-up); ordered: opt.rows_table_buckets per
   // state.  Either while the table stays below a quarter of the free memory, else halved down to 2 per state.
   // float64: two-slot buckets, 2 per state.  The perfect hash's leftover keys are not sorted: they keep the hashed home.
-  const bool ordered = !ctx->dense_index && ctx->opt_rows_table == 1 && n >= 1;
+  const bool ordered = !ctx->dense_index && ctx->opt.rows_table == 1 && n >= 1;
   size_t free_b = 0, total_b = 0;
   CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-  int64_t per_state = ce ? (ordered ? ctx->opt_rows_table_buckets : 8) : 2;
+  int64_t per_state = ce ? (ordered ? ctx->opt.rows_table_buckets : 8) : 2;
   while (per_state > 2 && (double)per_state * n_left * 32.0 > 0.25 * (double)free_b) per_state /= 2;
   if (per_state * n_left + 16 >= 2147483647ll) throw std::runtime_error("k_rows: table of more than 2^31 buckets");
   // (the ordered directory ends at exactly per_state * n buckets)
@@ -661,7 +661,7 @@ void ensure_table(dmv_context *ctx, int elt) {
     CUDA_CHECK(cudaMemcpyAsync(&k_lo, ctx->d_reps.ptr, 8, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaMemcpyAsync(&k_hi, ctx->d_reps.ptr + (n - 1), 8, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
-    OrderedDir D = ordered_plan(k_lo, k_hi, ctx->opt_rows_table_bits);
+    OrderedDir D = ordered_plan(k_lo, k_hi, ctx->opt.rows_table_bits);
     ctx->d_table_dir.alloc((size_t)D.last + 2);
     D.dir = ctx->d_table_dir.ptr;
     launch_ordered_dir(ctx->d_reps.ptr, n, D, (uint32_t)per_state, st);
@@ -855,6 +855,71 @@ void collect_timings(dmv_context *ctx) {
   }
 }
 
+namespace {
+
+// what a change of an option makes stale
+enum Stale : unsigned {
+  STALE_TABLE = 1,      // the keys of k_rows' table
+  STALE_PLAN = 2,       // the record plan of the push traversal
+  STALE_EXCHANGE = 4,   // the choice of exchange (the next collective product decides again)
+  STALE_ROUNDS = 8,     // the set-up of the overlapped rounds
+  STALE_ORBIT = 16,     // the orbit program on the device (bases with permutation symmetries)
+  STALE_INDEX = 32,     // the state -> index mode (once the basis is built)
+};
+
+// One row per option of dmv_set_option.  Accepted values: lo .. hi, or exactly those of `only` when it is not empty.
+using OptionField = int Options::*;
+struct OptionRow {
+  const char *name;
+  OptionField field;
+  int lo, hi;
+  std::vector<int> only;
+  unsigned stale;
+  const char *values;   // the accepted values in words, for the error message
+};
+
+const OptionRow kOptionTable[] = {
+    {"mode", &Options::mode, -1, 1, {}, 0, "-1 auto, 0 push, 1 pull"},
+    {"index", &Options::index, 0, 0, {-1, 0, 2, 3}, STALE_INDEX,
+     "-1 auto, 0 directory, 2 combinadic rank, 3 Lin tables"},
+    {"exchange", &Options::exchange, -1, 2, {}, STALE_PLAN | STALE_EXCHANGE | STALE_ROUNDS,
+     "-1 auto, 0 NCCL send/recv, 1 peer-direct records, 2 replicated x (all-gather)"},
+    {"gather", &Options::gather, -1, 0, {}, 0, "-1 auto, 0 off (queued k_pull for mode = 1)"},
+    {"rows_batch_min", &Options::rows_batch_min, 2, 6, {}, 0, "2 .. 6 doubles per state"},
+    {"rows_batch", &Options::rows_batch, -1, 1, {}, 0,
+     "-1 auto / 1 k_rows_batch for batched products, 0 vector by vector"},
+    {"rows_ctas", &Options::rows_ctas, 2, 4, {}, 0, "2, 3 or 4 resident CTAs per SM of k_rows"},
+    {"rows_index", &Options::rows_index, -1, 1, {}, STALE_TABLE,
+     "-1 auto / 0 open-addressing table, 1 dense index (perfect hash)"},
+    {"rows_table", &Options::rows_table, 0, 1, {}, STALE_TABLE, "0 hashed home, 1 ordered by key prefix"},
+    {"rows_table_bits", &Options::rows_table_bits, 1, 14, {}, STALE_TABLE,
+     "1 .. 14 (the directory of 2^bits blocks lives in shared memory)"},
+    {"rows_table_buckets", &Options::rows_table_buckets, 0, 0, {2, 4, 8}, STALE_TABLE, "2, 4 or 8 buckets per state"},
+    {"rounds", &Options::rounds, -1, 64, {}, STALE_ROUNDS,
+     "-1 auto, 0 / 1 one-shot exchange, R <= 64 overlapped rounds"},
+    {"gather_walk", &Options::gather_walk, 0, 2, {}, 0,
+     "0 per-lane from the top bit, 1 group-major, 2 per-lane from the bottom bit"},
+    {"gather_split", &Options::gather_split, 0, 0, {-1, 1, 2, 4, 8, 16, 32}, 0,
+     "-1 auto, else 1, 2, 4, 8, 16 or 32 lanes per row of k_gather"},
+    {"peer_gather", &Options::peer_gather, -1, 0, {}, STALE_EXCHANGE, "-1 auto, 0 NCCL all-gather of x"},
+    {"rows", &Options::rows, -1, 0, {}, 0, "-1 auto, 0 off (queued k_pull / k_generate for symmetric bases)"},
+    {"canon", &Options::canon, -1, 2, {}, STALE_ORBIT,
+     "-1 auto, 0 walk the group chain, 1 round-1 forms, 2 single-block LUT + independent networks"},
+    {"bitparallel", &Options::bitparallel, 0, 1, {}, STALE_PLAN, "1 on, 0 walk the flip-mask groups one by one"},
+};
+
+void invalidate(dmv_context *c, unsigned stale) {
+  if (stale & STALE_TABLE) c->table_elt = 0;
+  if (stale & STALE_PLAN) c->planned = false;
+  if (stale & STALE_EXCHANGE) { c->exchange_decided = false; c->replicated = false; }
+  if (stale & STALE_ROUNDS) { c->rounds.tried = false; c->rounds.ready = false; }
+  // device tables that queued work may still read are rewritten: wait for the stream first
+  if ((stale & STALE_ORBIT) && c->proj == PROJ_GROUP) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); upload_orbit(c); }
+  if ((stale & STALE_INDEX) && c->n_states >= 0) { CUDA_CHECK(cudaStreamSynchronize(c->stream)); select_index_mode(c); }
+}
+
+}  // namespace
+
 } }  // namespace dmv::host
 
 extern "C" {
@@ -1006,85 +1071,18 @@ int dmv_set_option(dmv_context *ctx, const char *name, int64_t value) {
   API_BEGIN
   use_device(ctx);
   const std::string key(name ? name : "");
-  if (key == "mode") {
-    if (value < -1 || value > 1) throw std::runtime_error("mode: -1 auto, 0 push, 1 pull");
-    ctx->opt_mode = (int)value;
-  } else if (key == "index") {
-    if (value != -1 && value != 0 && value != 2 && value != 3)
-      throw std::runtime_error("index: -1 auto, 0 directory, 2 combinadic rank, 3 Lin tables");
-    ctx->opt_index = (int)value;
-    if (ctx->n_states >= 0) { CUDA_CHECK(cudaStreamSynchronize(ctx->stream)); select_index_mode(ctx); }
-  } else if (key == "exchange") {
-    if (value < -1 || value > 2)
-      throw std::runtime_error("exchange: -1 auto, 0 NCCL send/recv, 1 peer-direct records, 2 replicated x (all-gather)");
-    ctx->opt_exchange = (int)value;
-    ctx->planned = false;
-    ctx->exchange_decided = false;
-    ctx->replicated = false;
-    ctx->rounds.tried = false;
-    ctx->rounds.ready = false;
-  } else if (key == "gather") {
-    if (value < -1 || value > 0) throw std::runtime_error("gather: -1 auto, 0 off (queued k_pull for mode = 1)");
-    ctx->opt_gather = (int)value;
-  } else if (key == "rows_batch_min") {
-    if (value < 2 || value > 6) throw std::runtime_error("rows_batch_min: 2 .. 6 doubles per state");
-    ctx->opt_rows_batch_min = (int)value;
-  } else if (key == "rows_batch") {
-    if (value < -1 || value > 1) throw std::runtime_error("rows_batch: -1 auto / 1 k_rows_batch for batched products, 0 vector by vector");
-    ctx->opt_rows_batch = (int)value;
-  } else if (key == "rows_ctas") {
-    ctx->opt_rows_ctas = (value == 3 || value == 4) ? (int)value : 2;
-    if (ctx->global) ctx->global->opt_rows_ctas = ctx->opt_rows_ctas;
-  } else if (key == "rows_index") {
-    if (value < -1 || value > 1) throw std::runtime_error("rows_index: -1 auto / 0 open-addressing table, 1 dense index (perfect hash)");
-    ctx->opt_rows_index = (int)value;
-    ctx->table_elt = 0;
-    if (ctx->global) { ctx->global->opt_rows_index = (int)value; ctx->global->table_elt = 0; }
-  } else if (key == "rows_table" || key == "rows_table_bits" || key == "rows_table_buckets") {
-    if (key == "rows_table" && (value < 0 || value > 1))
-      throw std::runtime_error("rows_table: 0 hashed home, 1 ordered by key prefix");
-    if (key == "rows_table_bits" && (value < 1 || value > 14))
-      throw std::runtime_error("rows_table_bits: 1 .. 14 (the directory of 2^bits blocks lives in shared memory)");
-    if (key == "rows_table_buckets" && value != 2 && value != 4 && value != 8)
-      throw std::runtime_error("rows_table_buckets: 2, 4 or 8 buckets per state");
-    for (dmv_context *c : {ctx, ctx->global}) {
-      if (!c) continue;
-      if (key == "rows_table") c->opt_rows_table = (int)value;
-      else if (key == "rows_table_bits") c->opt_rows_table_bits = (int)value;
-      else c->opt_rows_table_buckets = (int)value;
-      c->table_elt = 0;
-    }
-  } else if (key == "rounds") {
-    if (value < -1 || value > 64) throw std::runtime_error("rounds: -1 auto, 0 / 1 one-shot exchange, R <= 64 overlapped rounds");
-    ctx->opt_rounds = (int)value;
-    ctx->rounds.tried = false;
-    ctx->rounds.ready = false;
-  } else if (key == "gather_walk") {
-    if (value < 0 || value > 2)
-      throw std::runtime_error("gather_walk: 0 per-lane from the top bit, 1 group-major, 2 per-lane from the bottom bit");
-    ctx->opt_gather_walk = (int)value;
-    if (ctx->global) ctx->global->opt_gather_walk = ctx->opt_gather_walk;
-  } else if (key == "gather_split") {
-    if (value != -1 && value != 1 && value != 2 && value != 4 && value != 8 && value != 16 && value != 32)
-      throw std::runtime_error("gather_split: -1 auto, else 1, 2, 4, 8, 16 or 32 lanes per row of k_gather");
-    ctx->opt_gather_split = (int)value;
-    if (ctx->global) ctx->global->opt_gather_split = ctx->opt_gather_split;
-  } else if (key == "peer_gather") {
-    if (value < -1 || value > 0) throw std::runtime_error("peer_gather: -1 auto, 0 NCCL all-gather of x");
-    ctx->opt_peer_gather = (int)value;
-    ctx->exchange_decided = false;
-  } else if (key == "rows") {
-    if (value < -1 || value > 0) throw std::runtime_error("rows: -1 auto, 0 off (queued k_pull / k_generate for symmetric bases)");
-    ctx->opt_rows = (int)value;
-    if (ctx->global) ctx->global->opt_rows = (int)value;
-  } else if (key == "canon") {
-    ctx->opt_canon = (value >= 0 && value <= 2) ? (int)value : -1;
-    if (ctx->proj == PROJ_GROUP) { CUDA_CHECK(cudaStreamSynchronize(ctx->stream)); upload_orbit(ctx); }
-  } else if (key == "bitparallel") {
-    ctx->opt_bitparallel = value != 0;
-    ctx->planned = false;
-  } else {
-    throw std::runtime_error("unknown option '" + key + "'");
+  const OptionRow *row = nullptr;
+  for (const OptionRow &r : kOptionTable)
+    if (key == r.name) row = &r;
+  if (!row) throw std::runtime_error("unknown option '" + key + "'");
+  const bool ok = row->only.empty() ? (value >= row->lo && value <= row->hi)
+                                    : std::find(row->only.begin(), row->only.end(), value) != row->only.end();
+  if (!ok) throw std::runtime_error(key + ": " + row->values + " (got " + std::to_string(value) + ")");
+  // the rank first: the twin's products run on the rank's stream, which invalidate() waits for before the twin's tables
+  for (dmv_context *c : {ctx, ctx->global}) {
+    if (!c) continue;
+    c->opt.*row->field = (int)value;
+    invalidate(c, row->stale);
   }
   API_END
 }
@@ -1092,6 +1090,7 @@ int dmv_set_option(dmv_context *ctx, const char *name, int64_t value) {
 int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   const std::string key(name ? name : "");
   if (!ctx) return -1;
+  if (key.compare(0, 7, "global.") == 0) return ctx->global ? dmv_get_info(ctx->global, key.c_str() + 7) : -1;
   if (key == "index_mode") return ctx->index_mode;
   if (key == "pull") return use_pull(ctx) ? 1 : 0;
   if (key == "gather")
@@ -1109,7 +1108,7 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "bp_pairs") { int64_t n = 0; for (auto &w : ctx->h_push.bp) n += w.n0 + w.n1; return n; }
   if (key == "canon_mode") return ctx->orbit.canon_mode;
   if (key == "torus_mode") return ctx->orbit.tor_mode;
-  if (key == "rows_tk") return rows_torus_k(ctx->orbit, ctx->opt_rows_index == 1, ctx->opt_rows_ctas);
+  if (key == "rows_tk") return rows_torus_k(ctx->orbit, ctx->opt.rows_index == 1, ctx->opt.rows_ctas);
   if (key == "rows")
     return ((use_pull(ctx) && !use_gather(ctx) && use_rows(ctx)) ||
             (ctx->replicated && ctx->global && !use_gather(ctx->global) && use_rows(ctx->global))) ? 1 : 0;
@@ -1401,7 +1400,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
                     ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);
     }
   }
-  if (ctx->num_ranks == 1 && use_pull(ctx) && !use_gather(ctx) && use_rows(ctx) && ctx->opt_rows_batch != 0 &&
+  if (ctx->num_ranks == 1 && use_pull(ctx) && !use_gather(ctx) && use_rows(ctx) && ctx->opt.rows_batch != 0 &&
       is_device_pointer(x) == is_device_pointer(y)) {
     // bases with permutation symmetries: up to six doubles per state share one orbit minimum and one look-up per term
     // (host vectors -- what PRIMME hands over -- are staged a batch at a time)
@@ -1409,7 +1408,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
     const bool on_host = !is_device_pointer(x);
     // (a batch shares the orbit minimum and the look-up of a term between its vectors -- 64-byte buckets, one request
     // per lane in flight -- so it pays from two vectors on)
-    while ((num_vectors - k) * elt >= ctx->opt_rows_batch_min && num_vectors - k >= 2) {
+    while ((num_vectors - k) * elt >= ctx->opt.rows_batch_min && num_vectors - k >= 2) {
       const int nv = std::min(per, num_vectors - k);
       const void *xk = xb + (size_t)k * vec_bytes;
       void *yk = yb + (size_t)k * vec_bytes;

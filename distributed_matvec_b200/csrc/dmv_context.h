@@ -147,6 +147,39 @@ struct DevTables {
 } }  // namespace dmv::host
 using namespace dmv::host;
 
+// Options of dmv_set_option (include/dmv_b200.h), each named like its field; the accepted values and what a change
+// invalidates are in the table of dmv_set_option.  The whole-basis twin of the replicated-x product carries a copy.
+struct Options {
+  int canon = -1;    // -1 auto (block-rotation canonical form when the chain subgroup allows it), 0 walk the chain
+  int mode = -1;     // -1 auto (pull when one rank owns the basis), 0 push (scatter), 1 pull (gather)
+  int index = -1;    // -1 auto, 0 directory search, 2 combinadic rank, 3 Lin tables
+  int bitparallel = 1;  // 0: walk the groups one by one even when the bit-parallel test applies
+  int gather = -1;      // row traversal kernel: -1 auto (k_gather when it applies), 0 always the queued k_pull
+  int rows = -1;        // -1 auto (k_rows when it applies), 0 the queued k_pull
+  int rows_ctas = 2;    // k_rows: resident CTAs per SM: 2 (122 registers, default) | 3 (80 registers) | 4 (64 registers)
+  int gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
+                        // (measured slower), 2 per-lane walk from the bottom bit (round 1)
+  int gather_split = -1;  // k_gather: lanes per row, -1 auto (choose_row_split), else 1 | 2 | 4 | 8 | 16 | 32
+  int rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (kept for reference:
+                         // the dense table is still many times L2, so a look-up still costs a random sector)
+  // layout of the open-addressing table without the dense index: 0 hashed home (table_slot), 1 ordered by key prefix
+  // (ordered_block in dmv_device.cuh; its directory of at most 2^bits blocks lives in shared memory, so bits <= 14),
+  // complex128 with `buckets` one-slot buckets per state (float64: two-slot buckets, 2 per state, in both layouts).
+  // Ordered, 2^14 blocks and 8 buckets per state: on an H100 (700 W, L2 flushed) 6.6 % faster than hashed on the 6x6
+  // square, 3.4 % on chain_32_symm and 7.3 % on chain_36_symm (complex128), 1.7 / 0.3 / 5.5 % (float64).  With 4 or 2
+  // buckets per state the extra probes of linear probing (1.17 / 1.5 per look-up against 1.07) cost more than the
+  // smaller table saves: 5-15 % / 35-60 % slower (profiles/h100_rows_table_sweep*.log)
+  int rows_table = 1;
+  int rows_table_bits = 14;
+  int rows_table_buckets = 8;
+  int rows_batch_min = 2;   // doubles per state (vectors x element width) from which a batch goes through k_rows_batch
+  int rows_batch = -1;      // -1 / 1: batched products of symmetric bases go through k_rows_batch | 0: vector by vector
+  int exchange = -1;        // -1 auto (replicated x, else peer-direct when possible), 0 NCCL send/recv, 1 peer-direct,
+                            // 2 replicated x
+  int peer_gather = -1;     // -1 auto, 0 NCCL all-gather
+  int rounds = -1;          // -1 auto, 0 / 1 off (generate everything, fence, accumulate), R > 1
+};
+
 struct dmv_context {
   int device = 0, rank = 0, num_ranks = 1;
   // basis
@@ -169,7 +202,6 @@ struct dmv_context {
   DevBuf<uint32_t> d_tor_luts;
   DevBuf<uint64_t> d_tor_net_mask;
   DevBuf<int32_t> d_tor_net_delta;
-  int opt_canon = -1;    // -1 auto (block-rotation canonical form when the chain subgroup allows it), 0 walk the chain
   OrbitProgram orbit{};  // device view
   // operator
   std::vector<DiagTerm> h_diag;
@@ -180,39 +212,18 @@ struct dmv_context {
   DevBuf<DiagClass> d_diag_classes;
   int n_diag_rest = 0;
   size_t h_diag_kept = 0;   // number of diagonal terms of the operator (h_diag itself only keeps the non-class rest)
-  // options
-  int opt_mode = -1;    // -1 auto (pull when one rank owns the basis), 0 push (scatter), 1 pull (gather)
-  int opt_index = -1;   // -1 auto, 0 directory search, 2 combinadic rank
-  int opt_bitparallel = 1;  // 0: walk the groups one by one even when the bit-parallel test applies
-  int opt_gather = -1;      // row traversal kernel: -1 auto (k_gather when it applies), 0 always the queued k_pull
+  Options opt;
   // k_gather applicability (set at context creation from the row-traversal tables)
   bool gather_ok = false, gather_narrow = false, gather_uniform = false;
   // k_rows applicability (bases with permutation symmetries, trivial characters, real bit-parallel operator) and its
   // hash table over this context's representatives (see table_slot in dmv_device.cuh)
   bool rows_ok = false;
-  int opt_rows = -1;        // -1 auto (k_rows when it applies), 0 the queued k_pull
-  int opt_rows_ctas = 2;    // k_rows: resident CTAs per SM: 2 (122 registers, default) | 3 (80 registers) | 4 (64 registers)
-  int opt_gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
-                            // (measured slower), 2 per-lane walk from the bottom bit (round 1)
-  int opt_gather_split = -1;  // k_gather: lanes per row, -1 auto (choose_row_split), else 1 | 2 | 4 | 8 | 16 | 32
   DevBuf<unsigned char> d_table;
   DevBuf<unsigned char> d_mph_blocks, d_dense;   // dense index: perfect-hash blocks, dense table of (key, value) slots
   PerfectHash mph{};
   bool dense_index = false;
-  int opt_rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (kept for reference:
-                             // the dense table is still many times L2, so a look-up still costs a random sector)
   DevBuf<uint32_t> d_slot_of;
   uint32_t table_slots = 0;
-  // layout of the open-addressing table without the dense index: 0 hashed home (table_slot), 1 ordered by key prefix
-  // (ordered_block in dmv_device.cuh; its directory of at most 2^bits blocks lives in shared memory, so bits <= 14),
-  // complex128 with `buckets` one-slot buckets per state (float64: two-slot buckets, 2 per state, in both layouts).
-  // Ordered, 2^14 blocks and 8 buckets per state: on an H100 (700 W, L2 flushed) 6.6 % faster than hashed on the 6x6
-  // square, 3.4 % on chain_32_symm and 7.3 % on chain_36_symm (complex128), 1.7 / 0.3 / 5.5 % (float64).  With 4 or 2
-  // buckets per state the extra probes of linear probing (1.17 / 1.5 per look-up against 1.07) cost more than the
-  // smaller table saves: 5-15 % / 35-60 % slower (profiles/h100_rows_table_sweep*.log)
-  int opt_rows_table = 1;
-  int opt_rows_table_bits = 14;
-  int opt_rows_table_buckets = 8;
   DevBuf<uint32_t> d_table_dir;
   OrderedDir table_dir{};
   int table_elt = 0;        // element type the slots are laid out for (0: not built)
@@ -221,8 +232,6 @@ struct dmv_context {
   DevBuf<unsigned char> d_table_batch;
   DevBuf<uint32_t> d_slot_of_batch;
   uint32_t table_batch_slots = 0;
-  int opt_rows_batch_min = 2;   // doubles per state (vectors x element width) from which a batch goes through k_rows_batch
-  int opt_rows_batch = -1;  // -1 / 1: batched products of symmetric bases go through k_rows_batch | 0: vector by vector
   double gather_uni[2] = {0.0, 0.0};
   int index_mode = INDEX_DIRECTORY;
   DevBuf<uint32_t> d_binom, d_lin_a, d_lin_b;
@@ -252,7 +261,6 @@ struct dmv_context {
   int row_split = 1;                       // lanes per source state (chosen at plan time from the block size)
   bool peer_direct = false;                // records are stored straight into the peers' incoming buffers
   int ptr_width = 0;                       // record width the destination pointer table was built for
-  int opt_exchange = -1;                   // -1 auto (peer-direct when possible), 0 NCCL send/recv, 1 peer-direct
   std::vector<void *> peer_betas, peer_coeffs;   // IPC-mapped incoming buffers of the peers
   std::vector<int64_t> my_offset_in_peer;         // first slot of MY region in every peer's incoming buffer
   DevBuf<int> d_barrier;
@@ -290,7 +298,6 @@ struct dmv_context {
   // peer-direct all-gather of x (launch_push_block): the peers' gathered vectors (two buffers, alternating by epoch) and
   // flag words mapped with CUDA IPC
   bool peer_gather = false;
-  int opt_peer_gather = -1;                 // -1 auto, 0 NCCL all-gather
   std::vector<void *> peer_xcat, peer_flagmem;
   DevBuf<unsigned> d_flags, d_push_done;    // [num_ranks] epochs raised by the peers; CTA counter of k_push_block
   DevBuf<void *> d_peer_slot[2];            // [num_ranks] slot `rank` of every rank's buffer b
@@ -323,7 +330,6 @@ struct dmv_context {
     cudaEvent_t ev_begin = nullptr, ev_done = nullptr;
     int64_t terms = 0;
   } rounds;
-  int opt_rounds = -1;                        // -1 auto, 0 / 1 off (generate everything, fence, accumulate), R > 1
 
   // Lanczos work space (dmv_lanczos)
   DevBuf<double> lz_v[4];

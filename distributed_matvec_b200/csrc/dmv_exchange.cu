@@ -33,7 +33,7 @@ void setup_exchange(dmv_context *ctx) {
   ctx->d_barrier.alloc(1);
   CUDA_CHECK(cudaMemsetAsync(ctx->d_barrier.ptr, 0, sizeof(int), ctx->stream));
   ctx->peer_direct = false;
-  if (ctx->opt_exchange == 0 || P > 32) return;
+  if (ctx->opt.exchange == 0 || P > 32) return;
 
   // ---- try to map the peers' incoming buffers
   struct Handles { cudaIpcMemHandle_t betas, coeffs; int ok; int pad[15]; };
@@ -73,7 +73,7 @@ void setup_exchange(dmv_context *ctx) {
   if (!agree) {
     for (auto &q : ctx->peer_betas) if (q) { cudaIpcCloseMemHandle(q); q = nullptr; }
     for (auto &q : ctx->peer_coeffs) if (q) { cudaIpcCloseMemHandle(q); q = nullptr; }
-    if (ctx->opt_exchange == 1) throw std::runtime_error("peer-direct exchange requested but CUDA IPC mapping failed");
+    if (ctx->opt.exchange == 1) throw std::runtime_error("peer-direct exchange requested but CUDA IPC mapping failed");
     return;
   }
   // my region inside peer q's incoming buffer: after the regions of the ranks before me (q itself sends nothing)
@@ -123,15 +123,10 @@ void setup_replicated(dmv_context *ctx) {
     dmv_context *g = nullptr;
     if (dmv_context_create(&b, &o, ctx->device, 0, 1, &g) != 0) throw std::runtime_error(g_last_error);
     ctx->global = g;
-    g->opt_rows = ctx->opt_rows;
-    g->opt_gather_walk = ctx->opt_gather_walk;
-    g->opt_gather_split = ctx->opt_gather_split;
-    g->opt_rows_index = ctx->opt_rows_index;
-    g->opt_rows_table = ctx->opt_rows_table;
-    g->opt_rows_table_bits = ctx->opt_rows_table_bits;
-    g->opt_rows_table_buckets = ctx->opt_rows_table_buckets;
-    g->opt_rows_ctas = ctx->opt_rows_ctas;
-    if (ctx->opt_canon != g->opt_canon && g->proj == PROJ_GROUP) { g->opt_canon = ctx->opt_canon; upload_orbit(g); }
+    // every option of the rank; "index" takes effect in the basis build.  ("mode", "exchange", "rounds", "peer_gather"
+    // and "rows_batch*" steer single, collective and batched products, which nothing asks of the twin.)
+    g->opt = ctx->opt;
+    if (g->opt.canon != Options{}.canon && g->proj == PROJ_GROUP) upload_orbit(g);
     if (dmv_basis_build(g) != 0) throw std::runtime_error(g_last_error);
   }
   dmv_context *g = ctx->global;
@@ -205,7 +200,7 @@ void setup_rounds(dmv_context *ctx) {
   const int P = ctx->num_ranks;
   Q.tried = true;
   Q.ready = false;
-  int R = ctx->opt_rounds;
+  int R = ctx->opt.rounds;
   if (R < 0) R = ctx->n_states >= (1 << 18) ? 4 : 1;
   // every rank must use the same number of rounds
   ctx->d_barrier.alloc(1);
@@ -213,7 +208,7 @@ void setup_rounds(dmv_context *ctx) {
   NCCL_CHECK(N.AllReduce(ctx->d_barrier.ptr, ctx->d_barrier.ptr, 1, ncclInt32, ncclMin, ctx->comm, ctx->stream));
   CUDA_CHECK(cudaMemcpyAsync(&R, ctx->d_barrier.ptr, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
   CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  if (R <= 1 || P > 32 || ctx->opt_exchange == 0) return;
+  if (R <= 1 || P > 32 || ctx->opt.exchange == 0) return;
   Q.R = R;
   Q.row_split = 1;
   Q.row_begin.assign(R + 1, 0);
@@ -417,7 +412,7 @@ void setup_peer_gather(dmv_context *ctx) {
   struct Handles { cudaIpcMemHandle_t xcat, flags; int ok; int pad[15]; };
   static_assert(sizeof(Handles) % 8 == 0, "handle block");
   Handles mine{};
-  mine.ok = (ctx->opt_peer_gather != 0 && cudaIpcGetMemHandle(&mine.xcat, ctx->d_xcat.ptr) == cudaSuccess &&
+  mine.ok = (ctx->opt.peer_gather != 0 && cudaIpcGetMemHandle(&mine.xcat, ctx->d_xcat.ptr) == cudaSuccess &&
              cudaIpcGetMemHandle(&mine.flags, ctx->d_flags.ptr) == cudaSuccess) ? 1 : 0;
   cudaGetLastError();
   DevBuf<char> d_mine, d_handles;
@@ -486,7 +481,7 @@ void decide_exchange(dmv_context *ctx) {
   NcclApi &N = nccl();
   int ok = 0;
   std::string why;
-  const bool want = (ctx->opt_exchange == 2 || ctx->opt_exchange == -1) && ctx->opt_mode != 0;
+  const bool want = (ctx->opt.exchange == 2 || ctx->opt.exchange == -1) && ctx->opt.mode != 0;
   if (want && ctx->num_ranks <= 32) {
     try { setup_replicated(ctx); ok = 1; } catch (const std::exception &e) { why = e.what(); ok = 0; }
   } else {
@@ -504,7 +499,7 @@ void decide_exchange(dmv_context *ctx) {
   if (!ctx->replicated) {
     delete ctx->global; ctx->global = nullptr;
     ctx->d_pos.release(); ctx->d_xcat.release();
-    if (ctx->opt_exchange == 2)
+    if (ctx->opt.exchange == 2)
       throw std::runtime_error("replicated-x exchange requested but not possible on every rank: " + why);
   }
 }

@@ -235,7 +235,7 @@ class Operator:
         return out
 
     def set_option(self, name: str, value: int):
-        """Options of include/dmv_b200.h: "mode", "gather", "index", "bitparallel", "canon", "exchange"."""
+        """dmv_set_option: the options and their values are listed in include/dmv_b200.h."""
         nat.check(nat.lib().dmv_set_option(self._ctx, name.encode(), int(value)))
         return self
 

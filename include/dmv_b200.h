@@ -72,7 +72,9 @@ int dmv_context_destroy(dmv_context *ctx);
  * non-blocking stream when use_own_stream != 0 (the initial state) */
 int dmv_set_stream(dmv_context *ctx, void *cuda_stream, int use_own_stream);
 int dmv_synchronize(dmv_context *ctx);
-/* options: "mode"     = -1 auto (row traversal on one rank when a row kernel applies -- k_gather: bit-parallel operator on a
+/* options (a value outside those listed raises and leaves the option unchanged; every option also applies to the
+ * whole-basis context of the replicated-x product, whether set before or after that context exists):
+ *          "mode"     = -1 auto (row traversal on one rank when a row kernel applies -- k_gather: bit-parallel operator on a
  *                        basis without permutation symmetries; k_rows: real bit-parallel operator on a basis with
  *                        permutation symmetries and trivial characters -- else push) | 0 push: scatter with FP64
  *                        atomics, the reference's traversal (DMV:73-127) | 1 rows (k_gather / k_rows, else the queued
@@ -93,11 +95,10 @@ int dmv_synchronize(dmv_context *ctx);
  *                        state (six real / three complex vectors) through k_rows_batch | 0 vector by vector;
  *                        "rows_batch_min" = doubles per state (vectors x element width, default 2) from which it is used
  *          "gather_walk" = 0 every lane walks its emitting groups from the top bit | 1 group-major warp-uniform walk
- *                        (measured slower; only at row split 1, else walk 0) | 2 from the bottom bit (round 1); other
- *                        values raise
+ *                        (measured slower; only at row split 1, else walk 0) | 2 from the bottom bit (round 1)
  *          "gather_split" = -1 auto (more lanes per row of k_gather on bases of fewer than 16 warps of rows per SM, never
  *                        more lanes than flip-mask groups) | 1, 2, 4, 8, 16 or 32 lanes per row, each walking every
- *                        S-th group; other values raise.  Applies to the single, batched and replicated-x products
+ *                        S-th group.  Applies to the single, batched and replicated-x products
  *          "index"    = -1 auto (identity / Lin tables / directory) | 0 directory + binary search | 2 combinadic rank
  *                        | 3 Lin tables (full fixed-Hamming bases)
  *          "bitparallel" = 1 | 0 walk the flip-mask groups one by one
@@ -113,7 +114,8 @@ int dmv_synchronize(dmv_context *ctx);
  *               "canon_mode", "torus_mode", "peer_direct", "replicated", "replicated_block", "peer_gather", "rounds",
  *               "global_states", "complex_coefficients", "rows_tk" (side of the square-torus orbit minimum k_rows is
  *               compiled for with the current options: 4 | 6, 0 the generic walk), "gather_split" (lanes per row the next
- *               single-rank k_gather launch uses), ... (-1: unknown) */
+ *               single-rank k_gather launch uses), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
+ *               context of the replicated-x product (-1 while there is none) */
 int dmv_set_option(dmv_context *ctx, const char *name, int64_t value);
 int64_t dmv_get_info(const dmv_context *ctx, const char *name);
 
