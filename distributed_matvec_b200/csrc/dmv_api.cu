@@ -1125,6 +1125,8 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "n_buckets") return (int64_t)ctx->n_buckets;
   if (key == "expm_dot_vectors") return ctx->kr_dot_vectors;
   if (key == "expm_combine_vectors") return ctx->kr_combine_vectors;
+  if (key == "eigsh_block_vectors") return ctx->eg_block_vectors;
+  if (key == "eigsh_rotate_vectors") return ctx->eg_rotate_vectors;
   return -1;
 }
 

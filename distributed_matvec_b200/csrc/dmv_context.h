@@ -337,6 +337,9 @@ struct dmv_context {
   // Krylov work space (dmv_expm_multiply): one allocation of (krylov_dim + 1) vectors, kept and reused between calls
   DevBuf<double> kr_basis, kr_scal, kr_partials;
   int64_t kr_dot_vectors = 0, kr_combine_vectors = 0;   // vector passes of the last call's block kernels
+  // block Krylov-Schur (dmv_eigsh): the basis of (krylov_dim + block_size) vectors is kr_basis; scalars and partials
+  DevBuf<double> eg_scal, eg_partials;
+  int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;   // vectors read or written by the last call's block kernels
 
   ~dmv_context() {
     delete global;

@@ -208,6 +208,19 @@ void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J,
 // w), nrm2[0] = |out|^2
 void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
                           const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s);
+// Block kernels of dmv_eigsh: W = R <= kMaxBlockRhs vectors, w_stride elements apart; V and W are read once per call.
+constexpr int kMaxBlockRhs = 6;
+// doubles the `partials` buffer of launch_block_gram / launch_block_update must hold
+size_t block_gram_partials();
+// h[2 (k R + r) + {0, 1}] = <V_k, W_r> for k < J, h[2 (J R + r R + s) + {0, 1}] = <W_r, W_s> (real vectors: imaginary 0)
+void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
+                       int R, double *partials, double *h, cudaStream_t s);
+// W_r -= sum_{k < J} c_{kr} V_k (c[2 (k R + r) + {0, 1}] in device memory), nrm2[2 r] = |W_r|^2 after
+void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
+                         int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s);
+// in place V_j <- sum_{i < k} S_{ij} V_i for j < l <= k (S[2 (i l + j) + {0, 1}] in device memory); no second basis
+void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
+                         cudaStream_t s);
 int64_t launch_counter();
 int planned_grid(int64_t rows, int row_split);
 int choose_row_split(int64_t rows, int n_groups);

@@ -1,7 +1,9 @@
 // dmv_solver.cu -- vector kernels of the device-resident Lanczos iteration (the consumer of the hot path; the reference
 // drives its product from PRIMME's matvec callback, src/Diagonalize.chpl:134-225, src/PRIMME.chpl:267-373).
 // Everything stays in HBM between products: y = H v, alpha = <v, y>, y -= alpha v + beta v_prev, beta' = |y|.
-// Also the block kernels of dmv_expm_multiply (dmv_krylov.cu): h = V^H w and out = a w - V c over many stored vectors.
+// Also the block kernels of dmv_expm_multiply (dmv_krylov.cu): h = V^H w and out = a w - V c over many stored vectors,
+// and those of dmv_eigsh (dmv_eigsh.cu): V^H W and W^H W, W -= V C for a block W of up to six vectors, and the in-place
+// rotation V <- V S.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -251,6 +253,252 @@ __global__ void __launch_bounds__(kThreads) k_reduce_partials(int blocks, int wi
   }
 }
 
+// ---- block kernels of dmv_eigsh (block Krylov-Schur): R <= 6 right-hand vectors W_0 .. W_{R-1}, w_stride elements apart
+// (a block of the basis), against J stored vectors.  Deterministic like the kernels above.
+
+// Sums each of the NV values of a[] over the warp (NV a power of two, <= 32) in a fixed order with NV - 1 + 5 - log2(NV)
+// shuffles instead of 5 NV: each step hands half of the values to the partner lane.  On return, lane v << (5 - log2 NV)
+// holds the total of value v (the other lanes hold copies or partial sums).
+template <int N, int H, int OFF>
+__device__ __forceinline__ void reduce_scatter_steps(double (&a)[N], int lane) {   // the first H values -> H / 2
+  if constexpr (H > 1) {
+    constexpr int h = H / 2;
+    const bool hi = lane & OFF;
+#pragma unroll
+    for (int i = 0; i < h; ++i) {
+      const double send = hi ? a[i] : a[i + h];
+      const double keep = hi ? a[i + h] : a[i];
+      a[i] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);
+    }
+    reduce_scatter_steps<N, h, OFF / 2>(a, lane);
+  }
+}
+
+template <int NV>
+__device__ __forceinline__ double warp_reduce_scatter(double (&a)[NV]) {
+  static_assert(NV >= 1 && NV <= 32 && (NV & (NV - 1)) == 0, "NV must be a power of two <= 32");
+  reduce_scatter_steps<NV, NV, 16>(a, threadIdx.x & 31);
+  double v = a[0];
+#pragma unroll
+  for (int off = 16 / NV; off >= 1; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+  return v;
+}
+
+constexpr int log2_int(int v) { return v <= 1 ? 0 : 1 + log2_int(v / 2); }
+constexpr int pow2_ceil(int v) { return v <= 1 ? 1 : 2 * pow2_ceil((v + 1) / 2); }
+
+template <bool CE, int R> __host__ __device__ constexpr int gram_chunk() { return R >= 8 ? 1 : 8 / R; }
+// elements per thread and tile of k_block_gram: about 24 doubles of W in registers
+template <bool CE, int R> __host__ __device__ constexpr int gram_elems() {
+  return CE ? (R <= 3 ? 4 : 2) : (R <= 3 ? 8 : 4);
+}
+
+// partials[(blockIdx * width + t) * 2 + {0, 1}], width = J R + R R: this CTA's share of <V_k, W_r> (t = k R + r) and of
+// <W_r, W_s> (t = J R + r R + s).  Every warp accumulates into its own rows of dynamic shared memory.
+template <bool CE, int R>
+__global__ void __launch_bounds__(kThreads, 2) k_block_gram(int64_t n, VecList V, int J, const double *__restrict__ W,
+                                                         int64_t w_stride, double *__restrict__ partials) {
+  constexpr int E = gram_elems<CE, R>(), KC = gram_chunk<CE, R>(), C = CE ? 2 : 1;
+  constexpr int NV = KC * R * C, NVP = pow2_ceil(NV), SH = 5 - log2_int(NVP);
+  constexpr int NG = R * C, NGP = pow2_ceil(NG), SHG = 5 - log2_int(NGP);
+  extern __shared__ double s_gram[];   // [warps][width][C]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int width = J * R + R * R;
+  double *acc = s_gram + (size_t)warp * width * C;
+  for (int t = lane; t < width * C; t += 32) acc[t] = 0.0;
+  __syncwarp();
+  const int64_t tile = (int64_t)kThreads * E;
+  for (int64_t base = (int64_t)blockIdx.x * tile; base < n; base += (int64_t)gridDim.x * tile) {
+    double wr[R][E], wi[R][E];
+    unsigned in = 0;
+#pragma unroll
+    for (int e = 0; e < E; ++e) {   // W is read once per tile; the stored vectors stream past it KC at a time
+      const int64_t i = base + (int64_t)e * kThreads + threadIdx.x;
+      if (i < n) in |= 1u << e;
+#pragma unroll
+      for (int r = 0; r < R; ++r) {
+        wr[r][e] = wi[r][e] = 0.0;
+        if (i < n) {
+          if (CE) { const double2 t = reinterpret_cast<const double2 *>(W + 2 * r * w_stride)[i]; wr[r][e] = t.x; wi[r][e] = t.y; }
+          else wr[r][e] = W[r * w_stride + i];
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r) {   // row r of the Gram matrix: conj(W_r) W_s
+      double g[NGP];
+#pragma unroll
+      for (int v = 0; v < NGP; ++v) g[v] = 0.0;
+#pragma unroll
+      for (int s = 0; s < R; ++s)
+#pragma unroll
+        for (int e = 0; e < E; ++e) {
+          g[s * C] += wr[r][e] * wr[s][e] + wi[r][e] * wi[s][e];
+          if (CE) g[s * C + 1] += wr[r][e] * wi[s][e] - wi[r][e] * wr[s][e];
+        }
+      const double t = warp_reduce_scatter<NGP>(g);
+      if ((lane & ((1 << SHG) - 1)) == 0 && (lane >> SHG) < NG) acc[(J * R + r * R) * C + (lane >> SHG)] += t;
+    }
+    for (int k0 = 0; k0 < J; k0 += KC) {
+      double a[NVP];
+#pragma unroll
+      for (int v = 0; v < NVP; ++v) a[v] = 0.0;
+#pragma unroll
+      for (int kk = 0; kk < KC; ++kk) {
+        if (k0 + kk < J) {
+          const double *v = V.p[k0 + kk];
+#pragma unroll
+          for (int e = 0; e < E; ++e) {
+            if (!(in >> e & 1u)) continue;
+            const int64_t i = base + (int64_t)e * kThreads + threadIdx.x;
+            if (CE) {   // conj(v) * w
+              const double2 t = __ldg(reinterpret_cast<const double2 *>(v) + i);
+#pragma unroll
+              for (int r = 0; r < R; ++r) {
+                a[(kk * R + r) * 2] += t.x * wr[r][e] + t.y * wi[r][e];
+                a[(kk * R + r) * 2 + 1] += t.x * wi[r][e] - t.y * wr[r][e];
+              }
+            } else {
+              const double t = __ldg(v + i);
+#pragma unroll
+              for (int r = 0; r < R; ++r) a[kk * R + r] += t * wr[r][e];
+            }
+          }
+        }
+      }
+      const double t = warp_reduce_scatter<NVP>(a);
+      const int v = lane >> SH;
+      if ((lane & ((1 << SH) - 1)) == 0 && v < NV && k0 * R * C + v < J * R * C) acc[k0 * R * C + v] += t;
+    }
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < width; t += blockDim.x) {
+    double re = 0.0, im = 0.0;
+#pragma unroll
+    for (int q = 0; q < kThreads / 32; ++q) {
+      re += s_gram[((size_t)q * width + t) * C];
+      if (CE) im += s_gram[((size_t)q * width + t) * C + 1];
+    }
+    partials[((int64_t)blockIdx.x * width + t) * 2] = re;
+    partials[((int64_t)blockIdx.x * width + t) * 2 + 1] = im;
+  }
+}
+
+// W_r -= sum_{k < J} c_{k r} V_k with c[2 (k R + r) + {0, 1}] in device memory (real vectors use the real parts);
+// partials[(blockIdx * R + r) * 2] = this CTA's share of |W_r|^2 after the update
+template <bool CE, int R>
+__global__ void __launch_bounds__(kThreads) k_block_update(int64_t n, VecList V, int J, const double *__restrict__ coef,
+                                                           double *W, int64_t w_stride, double *__restrict__ partials) {
+  __shared__ double s_c[kMaxBlockVectors * R][2];
+  __shared__ double s[kThreads / 32][R];
+  for (int k = threadIdx.x; k < J * R; k += blockDim.x) { s_c[k][0] = coef[2 * k]; s_c[k][1] = coef[2 * k + 1]; }
+  __syncthreads();
+  double nrm[R];
+#pragma unroll
+  for (int r = 0; r < R; ++r) nrm[r] = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    double re[R], im[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (CE) { const double2 t = reinterpret_cast<const double2 *>(W + 2 * r * w_stride)[i]; re[r] = t.x; im[r] = t.y; }
+      else { re[r] = W[r * w_stride + i]; im[r] = 0.0; }
+    }
+    for (int k0 = 0; k0 < J; k0 += kDotChunk) {
+      double vr[kDotChunk], vi[kDotChunk];
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {   // issue the chunk's loads before the first use
+        vr[kk] = vi[kk] = 0.0;
+        if (k0 + kk < J) {
+          if (CE) { const double2 t = __ldg(reinterpret_cast<const double2 *>(V.p[k0 + kk]) + i); vr[kk] = t.x; vi[kk] = t.y; }
+          else vr[kk] = __ldg(V.p[k0 + kk] + i);
+        }
+      }
+#pragma unroll
+      for (int kk = 0; kk < kDotChunk; ++kk) {
+        if (k0 + kk >= J) break;
+#pragma unroll
+        for (int r = 0; r < R; ++r) {
+          const double cr = s_c[(k0 + kk) * R + r][0], ci = s_c[(k0 + kk) * R + r][1];
+          if (CE) { re[r] -= cr * vr[kk] - ci * vi[kk]; im[r] -= cr * vi[kk] + ci * vr[kk]; }
+          else re[r] -= cr * vr[kk];
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < R; ++r) {
+      if (CE) reinterpret_cast<double2 *>(W + 2 * r * w_stride)[i] = make_double2(re[r], im[r]);
+      else W[r * w_stride + i] = re[r];
+      nrm[r] += re[r] * re[r] + im[r] * im[r];
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const double t = warp_sum(nrm[r]);
+    if (lane == 0) s[warp][r] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x < R) {
+    double t = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) t += s[q][threadIdx.x];
+    partials[(blockIdx.x * R + threadIdx.x) * 2] = t;
+    partials[(blockIdx.x * R + threadIdx.x) * 2 + 1] = 0.0;
+  }
+}
+
+// In place V_j <- sum_{i < k} S_{ij} V_i for j < l <= k, S[2 (i l + j) + {0, 1}] in device memory (real vectors use the
+// real parts).  A CTA stages a tile of every one of the k inputs in shared memory before it writes any output over them,
+// so no second basis is needed; each output element is summed over i in ascending order.
+constexpr int kRotWords = 64;   // 8-byte words of every vector in a tile: 64 real or 32 complex elements
+constexpr int kRotOut = 4;      // outputs per thread and pass
+template <bool CE>
+__global__ void __launch_bounds__(kThreads) k_block_rotate(int64_t n, VecList V, int k, int l,
+                                                           const double *__restrict__ S) {
+  constexpr int TE = CE ? kRotWords / 2 : kRotWords;   // elements per tile
+  extern __shared__ double s_tile[];                   // [k][kRotWords]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const double2 *S2 = reinterpret_cast<const double2 *>(S);
+  for (int64_t base = (int64_t)blockIdx.x * TE; base < n; base += (int64_t)gridDim.x * TE) {
+    const int words = (int)(std::min<int64_t>(TE, n - base) * (CE ? 2 : 1));
+    const int64_t w0 = base * (CE ? 2 : 1);
+    for (int t = threadIdx.x; t < k * kRotWords; t += kThreads) {
+      const int i = t / kRotWords, e = t % kRotWords;
+      s_tile[t] = e < words ? V.p[i][w0 + e] : 0.0;
+    }
+    __syncthreads();
+    for (int j0 = warp * kRotOut; j0 < l; j0 += (kThreads / 32) * kRotOut) {
+      double ar[kRotOut][2], ai[kRotOut][2];   // [output][element of the lane: lane, lane + 32 (real only)]
+#pragma unroll
+      for (int jj = 0; jj < kRotOut; ++jj) ar[jj][0] = ar[jj][1] = ai[jj][0] = ai[jj][1] = 0.0;
+      for (int i = 0; i < k; ++i) {
+        double xr0, xi0 = 0.0, xr1 = 0.0;
+        if (CE) { const double2 t = reinterpret_cast<const double2 *>(s_tile + i * kRotWords)[lane]; xr0 = t.x; xi0 = t.y; }
+        else { xr0 = s_tile[i * kRotWords + lane]; xr1 = s_tile[i * kRotWords + 32 + lane]; }
+#pragma unroll
+        for (int jj = 0; jj < kRotOut; ++jj) {
+          if (j0 + jj < l) {
+            const double2 c = __ldg(S2 + (size_t)i * l + j0 + jj);
+            if (CE) { ar[jj][0] += xr0 * c.x - xi0 * c.y; ai[jj][0] += xr0 * c.y + xi0 * c.x; }
+            else { ar[jj][0] += xr0 * c.x; ar[jj][1] += xr1 * c.x; }
+          }
+        }
+      }
+#pragma unroll
+      for (int jj = 0; jj < kRotOut; ++jj) {
+        if (j0 + jj >= l) break;
+        double *out = const_cast<double *>(V.p[j0 + jj]) + w0;
+        if (CE) { if (2 * lane < words) reinterpret_cast<double2 *>(out)[lane] = make_double2(ar[jj][0], ai[jj][0]); }
+        else {
+          if (lane < words) out[lane] = ar[jj][0];
+          if (32 + lane < words) out[32 + lane] = ar[jj][1];
+        }
+      }
+    }
+    __syncthreads();   // the next tile overwrites s_tile
+  }
+}
+
 int sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
@@ -354,6 +602,111 @@ void launch_block_combine(int64_t n, bool complex_elements, double a, const doub
   check("k_block_combine");
   k_reduce_partials<<<1, kThreads, 0, s>>>(grid, 1, partials, nrm2);
   check("k_reduce_partials");
+}
+
+namespace {
+
+// one wave of CTAs of a kernel with `smem` bytes of dynamic shared memory (the opt-in above 48 KB is set here)
+template <typename K>
+int one_wave_smem(K kernel, int64_t work_items, size_t smem) {
+  if (smem > 48 * 1024)
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
+  if (per_sm < 1) per_sm = 1;
+  const int64_t b = std::min<int64_t>(std::max<int64_t>(work_items, 1), (int64_t)sm_count() * per_sm);
+  return (int)b;
+}
+
+template <bool CE, int R>
+void gram_r(int64_t n, const VecList &V, int J, const double *W, int64_t w_stride, double *partials, double *h,
+            cudaStream_t s) {
+  constexpr int E = gram_elems<CE, R>();
+  const int width = J * R + R * R;
+  const size_t smem = (size_t)(kThreads / 32) * width * (CE ? 2 : 1) * sizeof(double);
+  const int grid = one_wave_smem(k_block_gram<CE, R>, (std::max<int64_t>(n, 0) + (int64_t)kThreads * E - 1) /
+                                                          ((int64_t)kThreads * E), smem);
+  k_block_gram<CE, R><<<grid, kThreads, smem, s>>>(n, V, J, W, w_stride, partials);
+  check("k_block_gram");
+  k_reduce_partials<<<width, kThreads, 0, s>>>(grid, width, partials, h);
+  check("k_reduce_partials");
+}
+
+template <bool CE, int R>
+void update_r(int64_t n, const VecList &V, int J, const double *coef, double *W, int64_t w_stride, double *partials,
+              double *nrm2, cudaStream_t s) {
+  const int grid = one_wave_smem(k_block_update<CE, R>, (std::max<int64_t>(n, 0) + kThreads - 1) / kThreads, 0);
+  k_block_update<CE, R><<<grid, kThreads, 0, s>>>(n, V, J, coef, W, w_stride, partials);
+  check("k_block_update");
+  k_reduce_partials<<<R, kThreads, 0, s>>>(grid, R, partials, nrm2);
+  check("k_reduce_partials");
+}
+
+template <bool CE>
+void gram_dispatch(int R, int64_t n, const VecList &V, int J, const double *W, int64_t w_stride, double *partials,
+                   double *h, cudaStream_t s) {
+  switch (R) {
+    case 1: gram_r<CE, 1>(n, V, J, W, w_stride, partials, h, s); break;
+    case 2: gram_r<CE, 2>(n, V, J, W, w_stride, partials, h, s); break;
+    case 3: gram_r<CE, 3>(n, V, J, W, w_stride, partials, h, s); break;
+    case 4: gram_r<CE, 4>(n, V, J, W, w_stride, partials, h, s); break;
+    case 5: gram_r<CE, 5>(n, V, J, W, w_stride, partials, h, s); break;
+    default: gram_r<CE, 6>(n, V, J, W, w_stride, partials, h, s); break;
+  }
+}
+
+template <bool CE>
+void update_dispatch(int R, int64_t n, const VecList &V, int J, const double *coef, double *W, int64_t w_stride,
+                     double *partials, double *nrm2, cudaStream_t s) {
+  switch (R) {
+    case 1: update_r<CE, 1>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+    case 2: update_r<CE, 2>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+    case 3: update_r<CE, 3>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+    case 4: update_r<CE, 4>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+    case 5: update_r<CE, 5>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+    default: update_r<CE, 6>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
+  }
+}
+
+}  // namespace
+
+size_t block_gram_partials() {
+  // the most CTAs one wave can hold (8 of 256 threads per SM) times the widest output, J R + R R with J < 65, R = 6
+  return (size_t)sm_count() * 8 * (kMaxBlockVectors * kMaxBlockRhs + kMaxBlockRhs * kMaxBlockRhs) * 2;
+}
+
+void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
+                       int R, double *partials, double *h, cudaStream_t s) {
+  if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
+    throw std::runtime_error("k_block_gram: bad number of vectors");
+  if (complex_elements) gram_dispatch<true>(R, n, V, J, W, w_stride, partials, h, s);
+  else gram_dispatch<false>(R, n, V, J, W, w_stride, partials, h, s);
+}
+
+void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
+                         int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s) {
+  if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
+    throw std::runtime_error("k_block_update: bad number of vectors");
+  if (complex_elements) update_dispatch<true>(R, n, V, J, coef, W, w_stride, partials, nrm2, s);
+  else update_dispatch<false>(R, n, V, J, coef, W, w_stride, partials, nrm2, s);
+}
+
+void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
+                         cudaStream_t s) {
+  if (k < 1 || k > kMaxBlockVectors || l < 1 || l > k) throw std::runtime_error("k_block_rotate: bad shape");
+  if (n <= 0) return;
+  const size_t smem = (size_t)k * kRotWords * sizeof(double);
+  const int64_t tiles = (n + (complex_elements ? kRotWords / 2 : kRotWords) - 1) /
+                        (complex_elements ? kRotWords / 2 : kRotWords);
+  if (complex_elements) {
+    const int grid = one_wave_smem(k_block_rotate<true>, tiles, smem);
+    k_block_rotate<true><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
+  } else {
+    const int grid = one_wave_smem(k_block_rotate<false>, tiles, smem);
+    k_block_rotate<false><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
+  }
+  check("k_block_rotate");
 }
 
 }  // namespace dmv

@@ -325,6 +325,36 @@ class Operator:
                                               float(tol), C.byref(prods), C.byref(err)))
         return y, int(prods.value), float(err.value)
 
+    def eigsh(self, k, block_size: int = 0, krylov_dim: int = 0, tol: float = 1e-10, max_restarts: int = 1000,
+              seed: int = 42, complex_vectors: bool = False, eigenvectors=True):
+        """The k lowest eigenpairs by block Krylov-Schur on the device (dmv_eigsh).  eigenvectors: True -> a numpy array
+        (k, n); False -> none; or a C-contiguous torch CUDA tensor (k, n) of the vector type, filled in place on torch's
+        current stream.  Collective when num_ranks > 1.
+        -> (eigenvalues[k], vectors or None, residuals[k], converged, products, restarts)"""
+        elt = nat.DMV_C128 if complex_vectors else nat.DMV_F64
+        n = self.basis.numberStates()
+        k = int(k)
+        vec, ptr = None, None
+        if _is_torch(eigenvectors):
+            import torch
+            want = torch.complex128 if complex_vectors else torch.float64
+            if (tuple(eigenvectors.shape) != (k, n) or eigenvectors.dtype != want or not eigenvectors.is_cuda
+                    or not eigenvectors.is_contiguous()):
+                raise ValueError(f"eigenvectors must be a C-contiguous CUDA tensor of shape ({k}, {n}) and dtype {want}")
+            self.use_torch_stream()
+            vec, ptr = eigenvectors, _ptr(eigenvectors)
+        elif eigenvectors is True:
+            vec = np.zeros((max(k, 0), n), dtype=np.complex128 if complex_vectors else np.float64)
+            ptr = vec.ctypes.data
+        elif eigenvectors is not False and eigenvectors is not None:
+            raise TypeError("eigenvectors must be True, False or a torch CUDA tensor")
+        evals, res = np.zeros(max(k, 1)), np.zeros(max(k, 1))
+        conv, prods, rst = C.c_int(), C.c_int(), C.c_int()
+        nat.check(nat.lib().dmv_eigsh(self._ctx, elt, k, int(block_size), int(krylov_dim), float(tol),
+                                      int(max_restarts), int(seed), evals.ctypes.data, ptr, res.ctypes.data,
+                                      C.byref(conv), C.byref(prods), C.byref(rst)))
+        return evals[:k], vec, res[:k], int(conv.value), int(prods.value), int(rst.value)
+
     # -- replicated-x form of the distributed product (dmv_replicated_*), for hosts that own the all-gather -------
     def replicated_setup(self) -> int:
         """Build the whole basis and the slot table on this rank; returns the slot size (elements per rank)."""

@@ -251,6 +251,32 @@ int dmv_lanczos(dmv_context *ctx, int elt, int max_iters, double tol, uint64_t s
 int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const void *x, void *y,
                       int krylov_dim, double tol, int *products, double *error_estimate);
 
+/* ---- the nev lowest eigenpairs on the device (row f3: what src/Diagonalize.chpl asks PRIMME for) by block
+ * Krylov-Schur with full reorthogonalisation; the basis stays in HBM, the products run through dmv_matvec_batch, dot
+ * products are reduced over the ranks with NCCL and only small dense matrices visit the host.  Collective when
+ * num_ranks > 1 (needs dmv_comm_init), like dmv_lanczos.
+ * elt = DMV_C128 always; DMV_F64 only when info "complex_coefficients" == 0.  1 <= nev <= the global dimension.
+ * block_size: 0 = auto (min(nev, 4) for DMV_F64, min(nev, 3) for DMV_C128: the vectors one batched product shares), else
+ *   1..6, capped at the global dimension.  block_size 1 finds one copy of a degenerate eigenvalue at a time and can miss
+ *   its other copies; block_size >= the multiplicity finds them all.
+ * krylov_dim: basis size m; 0 = auto, min(65 - p, max(32, 2 nev + 4 p)) with p the block size; else nev + 2 p <= m and
+ *   m + p <= 65.  m is capped at the global dimension n_global; when the capped m is n_global, nev + 2 p <= m is waived
+ *   (the basis spans the whole space and every pair is exact after one Rayleigh-Ritz).  The basis is one context-owned
+ *   allocation of (m + p) * dmv_number_states elements, shared with dmv_expm_multiply and kept for later calls; the call
+ *   fails (naming the bytes needed) when it does not fit.
+ * tol > 0: pair i is converged when its Krylov-Schur residual estimate |H y_i - theta_i y_i| <= tol * max(1, |theta_i|).
+ * max_restarts >= 0: the call stops after that many restart cycles even if not every pair has converged (not an error).
+ * seed: the start block is a deterministic function of it (k_fill, as dmv_lanczos).
+ * eigenvalues (nev, ascending), residuals (nev, may be NULL): host memory.  eigenvectors (may be NULL): nev vectors of
+ * dmv_number_states elements of type elt one after the other ([nev, n], the layout of dmv_matvec_batch), this rank's
+ * hashed block, host or device memory; orthonormal over the ranks; within a degenerate eigenspace any orthonormal basis.
+ * converged: pairs of the nev that met the criterion; products: single-vector applications of H; restarts: restart
+ * cycles (each may be NULL).  dmv_get_info "eigsh_block_vectors" / "eigsh_rotate_vectors": vectors read or written by the
+ * Gram / update kernels and by the in-place rotation k_block_rotate in the last call (for bandwidth accounting). */
+int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim, double tol, int max_restarts,
+              uint64_t seed, double *eigenvalues, void *eigenvectors, double *residuals,
+              int *converged, int *products, int *restarts);
+
 /* ---- per-stage timings of the last product, in milliseconds (the reference's timing tree,
  * DMV:1028-1052).  names: see dmv_timing_name(i); returns the number of stages. */
 int dmv_last_timings(dmv_context *ctx, double *ms, int capacity);
@@ -314,6 +340,10 @@ int dmv_debug_tridiagonal_lowest(int k, const double *diag, const double *offdia
 /* dmv_debug_tridiagonal_expm: host half of dmv_expm_multiply, c = exp(z T) e_1 for the symmetric tridiagonal T
  *   (diag a[0..k), off-diag b[0..k-1)), c interleaved (re, im), 2k doubles */
 int dmv_debug_tridiagonal_expm(int k, const double *a, const double *b, double z_re, double z_im, double *c);
+/* dmv_debug_hermitian_eigen: host half of dmv_eigsh, the cyclic Jacobi eigensolver: a = k x k Hermitian matrix,
+ *   row-major, interleaved (re, im) (2 k^2 doubles); eigenvalues ascending (k doubles); eigenvectors (may be NULL):
+ *   2 k^2 doubles, component r of eigenvector i at [2 (r k + i)] */
+int dmv_debug_hermitian_eigen(int k, const double *a, double *eigenvalues, double *eigenvectors);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
