@@ -340,6 +340,8 @@ struct dmv_context {
   // block Krylov-Schur (dmv_eigsh): the basis of (krylov_dim + block_size) vectors is kr_basis; scalars and partials
   DevBuf<double> eg_scal, eg_partials;
   int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;   // vectors read or written by the last call's block kernels
+  // spin-spin correlations (dmv_zz_correlations): per-CTA partial Gram blocks and their sum
+  DevBuf<double> zz_partials, zz_gram;
 
   ~dmv_context() {
     delete global;

@@ -221,6 +221,16 @@ void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int
 // in place V_j <- sum_{i < k} S_{ij} V_i for j < l <= k (S[2 (i l + j) + {0, 1}] in device memory); no second basis
 void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
                          cudaStream_t s);
+// out[2k + {0, 1}] = sum over b < blocks of partials[(b * width + k) * 2 + {0, 1}], in a fixed order (k_reduce_partials)
+void launch_reduce_partials(int blocks, int width, const double *partials, double *out, cudaStream_t s);
+// Spin-spin Gram block of dmv_zz_correlations (dmv_observe.cu): gram[i * zz_gram_columns + j] = sum_b |x_b|^2 a_i s_j
+// with s_j = +-1 for bit j of reps[b] and a = (s, 1); zz_gram_size doubles (rows padded to 16, columns to 8).
+// `partials` must hold zz_gram_partials(n, n_sites) doubles.
+int zz_gram_columns(int n_sites);
+size_t zz_gram_size(int n_sites);
+size_t zz_gram_partials(int64_t n, int n_sites);
+void launch_zz_gram(int64_t n, bool complex_elements, int n_sites, const uint64_t *reps, const double *x,
+                    double *partials, double *gram, cudaStream_t s);
 int64_t launch_counter();
 int planned_grid(int64_t rows, int row_split);
 int choose_row_split(int64_t rows, int n_groups);

@@ -692,6 +692,11 @@ void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int
   else update_dispatch<false>(R, n, V, J, coef, W, w_stride, partials, nrm2, s);
 }
 
+void launch_reduce_partials(int blocks, int width, const double *partials, double *out, cudaStream_t s) {
+  k_reduce_partials<<<width, kThreads, 0, s>>>(blocks, width, partials, out);
+  check("k_reduce_partials");
+}
+
 void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
                          cudaStream_t s) {
   if (k < 1 || k > kMaxBlockVectors || l < 1 || l > k) throw std::runtime_error("k_block_rotate: bad shape");

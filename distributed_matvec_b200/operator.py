@@ -355,6 +355,24 @@ class Operator:
                                       C.byref(conv), C.byref(prods), C.byref(rst)))
         return evals[:k], vec, res[:k], int(conv.value), int(prods.value), int(rst.value)
 
+    def zz_correlations(self, x):
+        """Spin-spin correlations C[i, j] = <x|σᶻᵢσᶻⱼ|x> / <x|x> and magnetisation m[i] = <x|σᶻᵢ> / <x|x> on the device
+        (dmv_zz_correlations), with σᶻ = +1 on a set bit.  x: shape (n,) or (k, n), float64 or complex128, a numpy
+        array or a torch CUDA tensor (used in place on torch's current stream).  Collective when num_ranks > 1.
+        -> numpy (C, m) of shapes (N, N), (N,), or (k, N, N), (k, N) for a batch."""
+        elt = _elt_of(x)
+        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        if _is_torch(x):
+            self.use_torch_stream()
+        else:
+            x = np.ascontiguousarray(x)
+        C_out, m_out = np.zeros((k, N, N)), np.zeros((k, N))
+        nat.check(nat.lib().dmv_zz_correlations(self._ctx, elt, k, _ptr(x), C_out.ctypes.data, m_out.ctypes.data))
+        return (C_out[0], m_out[0]) if x.ndim == 1 else (C_out, m_out)
+
     # -- replicated-x form of the distributed product (dmv_replicated_*), for hosts that own the all-gather -------
     def replicated_setup(self) -> int:
         """Build the whole basis and the slot table on this rank; returns the slot size (elements per rank)."""

@@ -277,6 +277,17 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
               uint64_t seed, double *eigenvalues, void *eigenvectors, double *residuals,
               int *converged, int *products, int *restarts);
 
+/* ---- spin-spin correlations on the device (row f5; not in the reference): <x|σᶻᵢσᶻⱼ|x> / <x|x> and <x|σᶻᵢ> / <x|x>
+ * for num_vectors vectors ([num_vectors, n] layout of dmv_matvec_batch, n = dmv_number_states, this rank's hashed block),
+ * host or device x; σᶻ is +1 on a set bit.  x is a vector of the symmetry-adapted basis (the representatives and norms
+ * the products use); the answer is the expectation value in the state it represents on the full space.  One pass over
+ * x and the representatives per vector (k_zz_gram on the FP64 tensor cores) and an O(|G| N^2) group average on the
+ * host.  correlations: num_vectors * N * N doubles (vector, i, j), magnetization: num_vectors * N doubles (may be NULL),
+ * host or device.  Fails for a zero vector.  Collective when num_ranks > 1 (needs dmv_comm_init); every rank returns
+ * the same matrices.  A repeated call is bit-identical. */
+int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
+                        double *magnetization);
+
 /* ---- per-stage timings of the last product, in milliseconds (the reference's timing tree,
  * DMV:1028-1052).  names: see dmv_timing_name(i); returns the number of stages. */
 int dmv_last_timings(dmv_context *ctx, double *ms, int capacity);
@@ -344,6 +355,12 @@ int dmv_debug_tridiagonal_expm(int k, const double *a, const double *b, double z
  *   row-major, interleaved (re, im) (2 k^2 doubles); eigenvalues ascending (k doubles); eigenvectors (may be NULL):
  *   2 k^2 doubles, component r of eigenvector i at [2 (r k + i)] */
 int dmv_debug_hermitian_eigen(int k, const double *a, double *eigenvalues, double *eigenvectors);
+/* dmv_debug_zz_symmetrize: host half of dmv_zz_correlations, the group average of a Gram block: gram is (N + 1) x N,
+ *   row-major, gram[i][j] = sum_b |x_b|^2 s_i(r_b) s_j(r_b) for i < N and gram[N][j] = sum_b |x_b|^2 s_j(r_b)
+ *   (gram[0][0] = <x|x> must be positive); correlations N x N, magnetization N (may be NULL).  The group is that of
+ *   `basis`: its permutations and flips, {1, flip} for spin inversion alone, {1} without symmetries. */
+int dmv_debug_zz_symmetrize(const dmv_basis_desc *basis, const double *gram, double *correlations,
+                            double *magnetization);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,

@@ -1,0 +1,78 @@
+#!/usr/bin/env python3
+"""dmv_zz_correlations across ranks (one process per rank, NCCL inside libdmv_b200) against the one-rank result.
+With fewer GPUs than ranks, ranks share devices (round robin), as in tools/eigsh_check.py.
+
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 \
+        --master-port 29557 tools/zz_check.py [workload ...]
+
+A seeded random vector (float64, and complex128) in block order is cut into the ranks' chunks and moved to the hashed
+blocks (dmv_block_to_hashed); the collective call on the blocks must give the C and m of a one-rank context over the
+whole basis to 1e-13 on every rank, for one vector and for a batch of two.  Each line ends in OK or FAIL; used by
+tests/test_zz_correlations.py.
+"""
+import os
+import socket
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+import torch.distributed as dist  # noqa: E402
+
+from distributed_matvec_b200 import DistributedOperator, Operator  # noqa: E402
+from oracle import pyoracle as po  # noqa: E402
+from eigsh_check import load  # noqa: E402
+
+DEFAULT = ["heisenberg_chain_10", "heisenberg_square_4x4", "momentum_sector", "heisenberg_chain_24"]
+
+
+def main():
+    rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); local = int(os.environ["LOCAL_RANK"])
+    local %= torch.cuda.device_count()
+    if torch.cuda.device_count() < world:
+        os.environ["NCCL_HOSTID"] = f"{socket.gethostname()}-rank{rank}"
+        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
+        os.environ.setdefault("NCCL_IB_DISABLE", "1")
+    torch.cuda.set_device(local)
+    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    names = sys.argv[1:] or DEFAULT
+    failures = 0
+
+    def verdict(good, text):
+        nonlocal failures
+        flag = torch.tensor([0 if good else 1], device="cuda")
+        dist.all_reduce(flag)
+        if rank == 0:
+            print(f"{text} {'OK' if int(flag) == 0 else 'FAIL'}", flush=True)
+        failures += int(flag)
+
+    for name in names:
+        basis, matrix = load(name)
+        g = Operator(matrix, device=local)          # the whole sorted basis on one rank
+        g.basis.build()
+        n = g.basis.numberStates()
+        dop = DistributedOperator(matrix, device=local)
+        dop.basis.build()
+        masks = po.locale_idx_of(g.basis.representatives(), world)
+        bounds = np.linspace(0, n, world + 1).astype(int)
+        m_chunk = masks[bounds[rank]:bounds[rank + 1]]
+        rng = np.random.default_rng(23)
+        for dtype in (np.float64, np.complex128):
+            X = rng.normal(size=(2, n)) + (1j * rng.normal(size=(2, n)) if dtype == np.complex128 else 0)
+            C1, m1 = g.zz_correlations(X)
+            mine = np.stack([dop.op.block_to_hashed(np.ascontiguousarray(X[v, bounds[rank]:bounds[rank + 1]]),
+                                                    m_chunk) for v in range(2)])
+            C2, m2 = dop.op.zz_correlations(mine)                  # collective
+            Cs, ms = dop.op.zz_correlations(np.ascontiguousarray(mine[1]))
+            err = max(np.abs(C2 - C1).max(), np.abs(m2 - m1).max(), np.abs(Cs - C1[1]).max(), np.abs(ms - m1[1]).max())
+            verdict(err <= 1e-13, f"{name:26s} P={world} N={n} {np.dtype(dtype).name} C, m {err:.1e}")
+        dop.op.close()
+        g.close()
+    dist.barrier()
+    dist.destroy_process_group()
+    sys.exit(1 if failures else 0)
+
+
+if __name__ == "__main__":
+    main()
