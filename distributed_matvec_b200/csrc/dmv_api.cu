@@ -1127,6 +1127,7 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "expm_combine_vectors") return ctx->kr_combine_vectors;
   if (key == "eigsh_block_vectors") return ctx->eg_block_vectors;
   if (key == "eigsh_rotate_vectors") return ctx->eg_rotate_vectors;
+  if (key == "quadrature_group") return ctx->qd_group;
   return -1;
 }
 

@@ -342,6 +342,10 @@ struct dmv_context {
   int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;   // vectors read or written by the last call's block kernels
   // spin-spin correlations (dmv_zz_correlations): per-CTA partial Gram blocks and their sum
   DevBuf<double> zz_partials, zz_gram;
+  // finite-temperature Lanczos (dmv_lanczos_quadrature): 3 G vectors (r_{j-1}, r_j, H r_j of a group of G start vectors),
+  // the per-step scalars of a group, per-CTA partials; kept between calls
+  DevBuf<double> qd_vectors, qd_hist, qd_partials;
+  int qd_group = 0;   // G of the last call
 
   ~dmv_context() {
     delete global;

@@ -223,6 +223,24 @@ void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int
                          cudaStream_t s);
 // out[2k + {0, 1}] = sum over b < blocks of partials[(b * width + k) * 2 + {0, 1}], in a fixed order (k_reduce_partials)
 void launch_reduce_partials(int blocks, int width, const double *partials, double *out, cudaStream_t s);
+// Kernels of dmv_lanczos_quadrature (dmv_solver.cu): G <= kMaxBlockRhs recurrences, vector g at offset g n elements.
+// The recurrence of a vector breaks down at step t + 1 when beta_{t+1} = sqrt(b2_next) <= 1e-14 max(1, |alpha_t|) with
+// alpha_t = dot / b2 (b2 = |r_t|^2): one expression, evaluated alike by the device and the host.
+__host__ __device__ inline bool quad_breakdown(double b2_next, double dot, double b2) {
+  return sqrt(b2_next) <= 1e-14 * fmax(1.0, fabs(dot / b2));
+}
+// doubles the `partials` buffer of launch_quad_dot / launch_quad_update must hold for G vectors
+size_t quad_partials(int G);
+// x[g n + i] = seeded start value of vector first + g at representative reps[i], g < G
+void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
+                      double *x, cudaStream_t s);
+// out[2 g + {0, 1}] = <A_g, B_g> (A may equal B)
+void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
+                     double *out, cudaStream_t s);
+// step j: P <- r_{j+1} from P = r_{j-1}, Q = r_j, W = H r_j and the stored dot / b2 of steps j - 1 and j;
+// nrm2[2 g] = |r_{j+1}|^2
+void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
+                        const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s);
 // Spin-spin Gram block of dmv_zz_correlations (dmv_observe.cu): gram[i * zz_gram_columns + j] = sum_b |x_b|^2 a_i s_j
 // with s_j = +-1 for bit j of reps[b] and a = (s, 1); zz_gram_size doubles (rows padded to 16, columns to 8).
 // `partials` must hold zz_gram_partials(n, n_sites) doubles.

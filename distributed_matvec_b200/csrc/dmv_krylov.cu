@@ -6,86 +6,7 @@
 #include <complex>
 
 #include "dmv_context.h"
-
-namespace dmv { namespace host {
-
-using cplx = std::complex<double>;
-
-// Eigen-decomposition T = Q diag(lam) Q^T of the symmetric tridiagonal T (diagonal a[0..k), off-diagonal b[0..k-1)) by
-// the implicit QL method with Wilkinson shifts; q[r * k + i] = component r of eigenvector i.
-struct TridiagonalEigen {
-  int k = 0;
-  std::vector<double> lam, q;
-  TridiagonalEigen(const std::vector<double> &a, const std::vector<double> &b) {
-    k = (int)a.size();
-    lam = a;
-    std::vector<double> e(k, 0.0);
-    for (int i = 0; i + 1 < k; ++i) e[i] = b[i];
-    q.assign((size_t)k * k, 0.0);
-    for (int i = 0; i < k; ++i) q[(size_t)i * k + i] = 1.0;
-    std::vector<double> &d = lam;
-    for (int l = 0; l < k; ++l) {
-      for (int iter = 0;; ++iter) {
-        int m = l;
-        for (; m + 1 < k; ++m)   // the first negligible off-diagonal element at or below l splits the matrix
-          if (std::fabs(e[m]) <= DBL_EPSILON * (std::fabs(d[m]) + std::fabs(d[m + 1]))) break;
-        if (m == l) break;
-        if (iter == 200) throw std::runtime_error("tridiagonal eigensolver did not converge");
-        double g = (d[l + 1] - d[l]) / (2.0 * e[l]);   // Wilkinson shift from the leading 2 x 2 block
-        double r = std::hypot(g, 1.0);
-        g = d[m] - d[l] + e[l] / (g + std::copysign(r, g));
-        double s = 1.0, c = 1.0, p = 0.0;
-        bool underflow = false;
-        for (int i = m - 1; i >= l; --i) {   // chase the bulge up with plane rotations
-          double f = s * e[i];
-          const double bb = c * e[i];
-          r = std::hypot(f, g);
-          e[i + 1] = r;
-          if (r == 0.0) { d[i + 1] -= p; e[m] = 0.0; underflow = true; break; }
-          s = f / r;
-          c = g / r;
-          g = d[i + 1] - p;
-          r = (d[i] - g) * s + 2.0 * c * bb;
-          p = s * r;
-          d[i + 1] = g + p;
-          g = c * r - bb;
-          for (int t = 0; t < k; ++t) {
-            double *row = &q[(size_t)t * k];
-            f = row[i + 1];
-            row[i + 1] = s * row[i] + c * f;
-            row[i] = c * row[i] - s * f;
-          }
-        }
-        if (underflow) continue;
-        d[l] -= p;
-        e[l] = g;
-        e[m] = 0.0;
-      }
-    }
-  }
-  // c = exp(w T) e_1
-  void exp_e1(cplx w, std::vector<cplx> &c) const {
-    c.assign(k, cplx(0.0, 0.0));
-    for (int i = 0; i < k; ++i) {
-      const cplx f = std::exp(w * lam[i]) * q[i];   // q[0 * k + i]: first component of eigenvector i
-      for (int r = 0; r < k; ++r) c[r] += q[(size_t)r * k + i] * f;
-    }
-  }
-  // e_k^T phi_1(w T) e_1 with phi_1(x) = (e^x - 1) / x
-  cplx phi1_last(cplx w) const {
-    cplx s(0.0, 0.0);
-    for (int i = 0; i < k; ++i) s += q[(size_t)(k - 1) * k + i] * q[i] * phi1(w * lam[i]);
-    return s;
-  }
-  static cplx phi1(cplx x) {
-    if (std::abs(x) >= 0.5) return (std::exp(x) - 1.0) / x;
-    cplx s(1.0, 0.0);   // Taylor series sum_j x^j / (j + 1)!, Horner form; |x| < 0.5: the term j = 17 is < 1e-22
-    for (int j = 17; j >= 1; --j) s = 1.0 + s * x / (double)(j + 1);
-    return s;
-  }
-};
-
-} }  // namespace dmv::host
+#include "dmv_tridiagonal.h"
 
 extern "C" {
 

@@ -499,6 +499,138 @@ __global__ void __launch_bounds__(kThreads) k_block_rotate(int64_t n, VecList V,
   }
 }
 
+// ---- kernels of dmv_lanczos_quadrature (dmv_thermal.cu): G <= 6 independent three-term recurrences without a stored
+// basis, vector g of a group at offset g n elements.  Deterministic like the kernels above.
+
+// Seeded start vectors: entry s of vector first + g depends only on (seed, first + g, reps[s]), so every rank count
+// starts from the same vectors.  float64: +-1; complex128: e^{i phi}, phi uniform in [0, 2 pi).
+template <bool CE>
+__global__ void __launch_bounds__(kThreads) k_quad_fill(int64_t n, const uint64_t *__restrict__ reps, uint64_t seed,
+                                                        int first, int G, double *x) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int g = 0; g < G; ++g) {
+    const uint64_t key = hash64_01(seed + 0x9e3779b97f4a7c15ull * (uint64_t)(first + g + 1));
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+      const uint64_t h = hash64_01(reps[i] ^ key);
+      if (CE) {
+        double s, c;
+        sincos(6.283185307179586 * ((double)(h >> 11) * 0x1p-53), &s, &c);
+        reinterpret_cast<double2 *>(x)[(int64_t)g * n + i] = make_double2(c, s);
+      } else {
+        x[(int64_t)g * n + i] = (h >> 63) ? -1.0 : 1.0;
+      }
+    }
+  }
+}
+
+// partials[(blockIdx * G + g) * 2 + {0, 1}] = this CTA's share of <A_g, B_g>; A and B are read once
+template <bool CE, int G>
+__global__ void __launch_bounds__(kThreads) k_quad_dot(int64_t n, const double *__restrict__ A,
+                                                       const double *__restrict__ B, double *__restrict__ partials) {
+  double re[G], im[G];
+#pragma unroll
+  for (int g = 0; g < G; ++g) re[g] = im[g] = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      if (CE) {   // conj(a) * b
+        const double2 a = __ldg(reinterpret_cast<const double2 *>(A) + (int64_t)g * n + i);
+        const double2 b = __ldg(reinterpret_cast<const double2 *>(B) + (int64_t)g * n + i);
+        re[g] += a.x * b.x + a.y * b.y;
+        im[g] += a.x * b.y - a.y * b.x;
+      } else {
+        re[g] += __ldg(A + (int64_t)g * n + i) * __ldg(B + (int64_t)g * n + i);
+      }
+    }
+  }
+  __shared__ double s[kThreads / 32][G][2];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    const double r = warp_sum(re[g]);
+    const double t = CE ? warp_sum(im[g]) : 0.0;
+    if (lane == 0) { s[warp][g][0] = r; s[warp][g][1] = t; }
+  }
+  __syncthreads();
+  if (threadIdx.x < G) {
+    double r = 0.0, t = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) { r += s[q][threadIdx.x][0]; t += s[q][threadIdx.x][1]; }
+    partials[(blockIdx.x * G + threadIdx.x) * 2] = r;
+    partials[(blockIdx.x * G + threadIdx.x) * 2 + 1] = t;
+  }
+}
+
+// Step j of G recurrences r_{j+1} = W / beta_j - alpha_j r_j / beta_j - beta_j r_{j-1} / beta_{j-1}, written over
+// P = r_{j-1}; Q = r_j, W = H r_j.  The coefficients come from device memory: dot[2 (t G + g)] = <r_t, H r_t> and
+// b2[2 (t G + g)] = |r_t|^2 of step t.  A vector whose recurrence broke down at step j (quad_breakdown, or already zero)
+// gets r_{j+1} = r_j = 0.  partials[(blockIdx * G + g) * 2] = this CTA's share of |r_{j+1}|^2.
+template <bool CE, int G>
+__global__ void __launch_bounds__(kThreads) k_quad_update(int64_t n, double *P, double *Q, const double *__restrict__ W,
+                                                          const double *__restrict__ dot, const double *__restrict__ b2,
+                                                          int j, double *__restrict__ partials) {
+  __shared__ double s_c[G][3];   // 1 / beta_j, alpha_j / beta_j, beta_j / beta_{j-1}
+  __shared__ int s_dead[G];
+  __shared__ double s[kThreads / 32][G];
+  if (threadIdx.x < G) {
+    const int g = threadIdx.x;
+    const double bj2 = b2[2 * (j * G + g)];
+    bool dead = !(bj2 > 0.0);
+    double bp2 = 0.0;
+    if (!dead && j > 0) {
+      bp2 = b2[2 * ((j - 1) * G + g)];
+      dead = !(bp2 > 0.0) || quad_breakdown(bj2, dot[2 * ((j - 1) * G + g)], bp2);
+    }
+    const double beta = sqrt(bj2);
+    s_dead[g] = dead;
+    s_c[g][0] = dead ? 0.0 : 1.0 / beta;
+    s_c[g][1] = dead ? 0.0 : dot[2 * (j * G + g)] / bj2 / beta;
+    s_c[g][2] = dead || j == 0 ? 0.0 : beta / sqrt(bp2);
+  }
+  __syncthreads();
+  double nrm[G];
+#pragma unroll
+  for (int g = 0; g < G; ++g) nrm[g] = 0.0;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+#pragma unroll
+    for (int g = 0; g < G; ++g) {
+      const int64_t e = (int64_t)g * n + i;
+      if (s_dead[g]) {
+        if (CE) { reinterpret_cast<double2 *>(P)[e] = make_double2(0.0, 0.0); reinterpret_cast<double2 *>(Q)[e] = make_double2(0.0, 0.0); }
+        else { P[e] = 0.0; Q[e] = 0.0; }
+        continue;
+      }
+      const double cw = s_c[g][0], cq = s_c[g][1], cp = s_c[g][2];
+      if (CE) {
+        const double2 w = __ldg(reinterpret_cast<const double2 *>(W) + e), q = reinterpret_cast<const double2 *>(Q)[e];
+        const double2 p = j > 0 ? reinterpret_cast<const double2 *>(P)[e] : make_double2(0.0, 0.0);
+        const double rx = cw * w.x - cq * q.x - cp * p.x, ry = cw * w.y - cq * q.y - cp * p.y;
+        reinterpret_cast<double2 *>(P)[e] = make_double2(rx, ry);
+        nrm[g] += rx * rx + ry * ry;
+      } else {
+        const double p = j > 0 ? P[e] : 0.0;
+        const double r = cw * __ldg(W + e) - cq * Q[e] - cp * p;
+        P[e] = r;
+        nrm[g] += r * r;
+      }
+    }
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+    const double t = warp_sum(nrm[g]);
+    if (lane == 0) s[warp][g] = t;
+  }
+  __syncthreads();
+  if (threadIdx.x < G) {
+    double t = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) t += s[q][threadIdx.x];
+    partials[(blockIdx.x * G + threadIdx.x) * 2] = t;
+    partials[(blockIdx.x * G + threadIdx.x) * 2 + 1] = 0.0;
+  }
+}
+
 int sm_count() {
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
@@ -712,6 +844,82 @@ void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int
     k_block_rotate<false><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
   }
   check("k_block_rotate");
+}
+
+namespace {
+
+template <bool CE, int G>
+void quad_dot_g(int64_t n, const double *A, const double *B, double *partials, double *out, cudaStream_t s) {
+  const int grid = one_wave(k_quad_dot<CE, G>, n);
+  k_quad_dot<CE, G><<<grid, kThreads, 0, s>>>(n, A, B, partials);
+  check("k_quad_dot");
+  k_reduce_partials<<<G, kThreads, 0, s>>>(grid, G, partials, out);
+  check("k_reduce_partials");
+}
+
+template <bool CE, int G>
+void quad_update_g(int64_t n, double *P, double *Q, const double *W, const double *dot, const double *b2, int j,
+                   double *partials, double *nrm2, cudaStream_t s) {
+  const int grid = one_wave(k_quad_update<CE, G>, n);
+  k_quad_update<CE, G><<<grid, kThreads, 0, s>>>(n, P, Q, W, dot, b2, j, partials);
+  check("k_quad_update");
+  k_reduce_partials<<<G, kThreads, 0, s>>>(grid, G, partials, nrm2);
+  check("k_reduce_partials");
+}
+
+template <bool CE>
+void quad_dot_dispatch(int G, int64_t n, const double *A, const double *B, double *partials, double *out,
+                       cudaStream_t s) {
+  switch (G) {
+    case 1: quad_dot_g<CE, 1>(n, A, B, partials, out, s); break;
+    case 2: quad_dot_g<CE, 2>(n, A, B, partials, out, s); break;
+    case 3: quad_dot_g<CE, 3>(n, A, B, partials, out, s); break;
+    case 4: quad_dot_g<CE, 4>(n, A, B, partials, out, s); break;
+    case 5: quad_dot_g<CE, 5>(n, A, B, partials, out, s); break;
+    default: quad_dot_g<CE, 6>(n, A, B, partials, out, s); break;
+  }
+}
+
+template <bool CE>
+void quad_update_dispatch(int G, int64_t n, double *P, double *Q, const double *W, const double *dot, const double *b2,
+                          int j, double *partials, double *nrm2, cudaStream_t s) {
+  switch (G) {
+    case 1: quad_update_g<CE, 1>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+    case 2: quad_update_g<CE, 2>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+    case 3: quad_update_g<CE, 3>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+    case 4: quad_update_g<CE, 4>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+    case 5: quad_update_g<CE, 5>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+    default: quad_update_g<CE, 6>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
+  }
+}
+
+}  // namespace
+
+size_t quad_partials(int G) {
+  // the most CTAs one wave can hold (8 of 256 threads per SM) times G (re, im) pairs
+  return (size_t)sm_count() * 8 * G * 2;
+}
+
+void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
+                      double *x, cudaStream_t s) {
+  if (n <= 0) return;
+  if (complex_elements) k_quad_fill<true><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
+  else k_quad_fill<false><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
+  check("k_quad_fill");
+}
+
+void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
+                     double *out, cudaStream_t s) {
+  if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_dot: bad number of vectors");
+  if (complex_elements) quad_dot_dispatch<true>(G, n, A, B, partials, out, s);
+  else quad_dot_dispatch<false>(G, n, A, B, partials, out, s);
+}
+
+void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
+                        const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s) {
+  if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_update: bad number of vectors");
+  if (complex_elements) quad_update_dispatch<true>(G, n, P, Q, W, dot, b2, j, partials, nrm2, s);
+  else quad_update_dispatch<false>(G, n, P, Q, W, dot, b2, j, partials, nrm2, s);
 }
 
 }  // namespace dmv

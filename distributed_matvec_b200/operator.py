@@ -373,6 +373,36 @@ class Operator:
         nat.check(nat.lib().dmv_zz_correlations(self._ctx, elt, k, _ptr(x), C_out.ctypes.data, m_out.ctypes.data))
         return (C_out[0], m_out[0]) if x.ndim == 1 else (C_out, m_out)
 
+    def lanczos_quadrature(self, num_vectors: int, steps: int, seed: int = 42, start=None,
+                           complex_vectors: bool = False):
+        """Finite-temperature Lanczos (stochastic Lanczos quadrature) on the device (dmv_lanczos_quadrature): for each
+        start vector r, `steps` Lanczos steps give Gauss nodes and weights with <r|f(H)|r> ~ sum_k w_k f(theta_k).
+        start: None for the seeded vectors of `seed` (distributed_matvec_b200.thermal.seeded_start_vectors mirrors them),
+        else a numpy array or a torch CUDA tensor of shape (num_vectors, n), float64 or complex128 (then
+        complex_vectors follows its type).  Collective when num_ranks > 1.
+        -> numpy (nodes [R, steps], weights [R, steps], steps_done [R], products); slots past steps_done hold zeros."""
+        R, M = int(num_vectors), int(steps)
+        n = self.basis.numberStates()
+        ptr = None
+        if start is not None:
+            if _is_torch(start):
+                if not start.is_cuda:
+                    raise ValueError("a torch start must be a CUDA tensor")
+                self.use_torch_stream()
+                start = start.contiguous()
+            else:
+                start = np.ascontiguousarray(start)
+            complex_vectors = _elt_of(start) == nat.DMV_C128
+            if tuple(start.shape) != (R, n):
+                raise ValueError(f"start must have shape ({R}, {n})")
+            ptr = _ptr(start)
+        elt = nat.DMV_C128 if complex_vectors else nat.DMV_F64
+        nodes, weights = np.zeros((max(R, 1), max(M, 1))), np.zeros((max(R, 1), max(M, 1)))
+        done, prods = np.zeros(max(R, 1), dtype=np.int32), C.c_int()
+        nat.check(nat.lib().dmv_lanczos_quadrature(self._ctx, elt, R, M, int(seed), ptr, nodes.ctypes.data,
+                                                   weights.ctypes.data, done.ctypes.data, C.byref(prods)))
+        return nodes, weights, done.astype(np.int64), int(prods.value)
+
     # -- replicated-x form of the distributed product (dmv_replicated_*), for hosts that own the all-gather -------
     def replicated_setup(self) -> int:
         """Build the whole basis and the slot table on this rank; returns the slot size (elements per rank)."""

@@ -112,7 +112,7 @@ int dmv_synchronize(dmv_context *ctx);
  *                        (generate everything, fence, accumulate) | R <= 64 rounds
  * dmv_get_info: "index_mode", "pull", "gather", "rows", "rows_ok", "projection", "n_groups", "orbit_n_q", "orbit_n_t",
  *               "canon_mode", "torus_mode", "peer_direct", "replicated", "replicated_block", "peer_gather", "rounds",
- *               "global_states", "complex_coefficients", "rows_tk" (side of the square-torus orbit minimum k_rows is
+ *               "global_states", "complex_coefficients", "quadrature_group", "rows_tk" (side of the square-torus orbit minimum k_rows is
  *               compiled for with the current options: 4 | 6, 0 the generic walk), "gather_split" (lanes per row the next
  *               single-rank k_gather launch uses), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
  *               context of the replicated-x product (-1 while there is none) */
@@ -288,6 +288,34 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
 int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
                         double *magnetization);
 
+/* ---- finite-temperature Lanczos on the device (row f6; not in the reference): the random-vector quadrature of the
+ * finite-temperature Lanczos method (Jaklič & Prelovšek 1994), also called stochastic Lanczos quadrature.  For each of
+ * num_vectors start vectors r, `steps` steps of the three-term recurrence (no reorthogonalisation, no stored basis) give
+ * the tridiagonal T_M = Q diag(θ) Qᵀ and its Gauss quadrature: nodes θ_k and weights w_k = |r|² Q₀ₖ², so that
+ *     <r|f(H)|r> ≈ Σ_k w_k f(θ_k)   (exact for polynomials of degree below 2 M),
+ *     Tr_sector f(H) ≈ (1/R) Σ_r Σ_k w_rk f(θ_rk)   (unbiased when E[r r†] = 1).
+ * The quadrature stays correct after orthogonality is lost: spurious copies of converged Ritz values carry the right
+ * total weight.  Row r of nodes / weights (host memory, num_vectors * steps doubles each) holds vector r; Σ_k w_rk = |r|²
+ * (the norm over all ranks).  Slots past steps_done[r] hold node 0 and weight 0.
+ * steps: >= 1, capped at the global dimension.  A recurrence whose Krylov space is invariant (β_{j+1} <= 1e-14
+ *   max(1, |α_j|), decided from the reduced scalars, so every rank takes the same step) stops at j + 1 steps and its vector
+ *   is zeroed; steps_done[r] (may be NULL) says where.
+ * start: NULL for seeded vectors, else num_vectors vectors [num_vectors, n] of type elt (this rank's hashed block, host or
+ *   device memory; none may be zero).  Seeded entry s of vector r depends only on (seed, r, representative s), so one
+ *   rank and P ranks start from the same vectors:
+ *     h = hash64_01(s ^ hash64_01(seed + 0x9e3779b97f4a7c15 (r + 1)))   (arithmetic modulo 2^64)
+ *     DMV_F64: +1 if bit 63 of h is clear, else -1;  DMV_C128: e^{iφ} with φ = 2π (h >> 11) 2^-53.
+ *   Then |r|² = n_global (to rounding for DMV_C128) and E[r r†] = 1.
+ * elt = DMV_C128 always; DMV_F64 only when info "complex_coefficients" == 0.
+ * The recurrences run in groups of G start vectors that share one batched product per step (dmv_matvec_batch): G = 4 on
+ * k_gather, 6 real or 3 complex vectors on k_rows_batch, 1 otherwise (and at most num_vectors); dmv_get_info
+ * "quadrature_group" gives the G of the last call.  The 3 G vectors of a group are one context-owned allocation, kept for
+ * later calls; the call fails (naming the bytes needed) when it does not fit.  Every reduction has a fixed order: a
+ * repeated call on the same context gives bit-identical nodes and weights.  products (may be NULL): single-vector
+ * applications of H.  Collective when num_ranks > 1 (needs dmv_comm_init), like dmv_lanczos. */
+int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps, uint64_t seed, const void *start,
+                           double *nodes, double *weights, int *steps_done, int *products);
+
 /* ---- per-stage timings of the last product, in milliseconds (the reference's timing tree,
  * DMV:1028-1052).  names: see dmv_timing_name(i); returns the number of stages. */
 int dmv_last_timings(dmv_context *ctx, double *ms, int capacity);
@@ -355,6 +383,10 @@ int dmv_debug_tridiagonal_expm(int k, const double *a, const double *b, double z
  *   row-major, interleaved (re, im) (2 k^2 doubles); eigenvalues ascending (k doubles); eigenvectors (may be NULL):
  *   2 k^2 doubles, component r of eigenvector i at [2 (r k + i)] */
 int dmv_debug_hermitian_eigen(int k, const double *a, double *eigenvalues, double *eigenvectors);
+/* dmv_debug_tridiagonal_quadrature: host half of dmv_lanczos_quadrature, the Gauss quadrature of the symmetric
+ *   tridiagonal T (diag a[0..k), off-diag b[0..k-1)): nodes = its eigenvalues ascending, weights = the squared first
+ *   components of its eigenvectors (k doubles each; they sum to 1) */
+int dmv_debug_tridiagonal_quadrature(int k, const double *a, const double *b, double *nodes, double *weights);
 /* dmv_debug_zz_symmetrize: host half of dmv_zz_correlations, the group average of a Gram block: gram is (N + 1) x N,
  *   row-major, gram[i][j] = sum_b |x_b|^2 s_i(r_b) s_j(r_b) for i < N and gram[N][j] = sum_b |x_b|^2 s_j(r_b)
  *   (gram[0][0] = <x|x> must be positive); correlations N x N, magnetization N (may be NULL).  The group is that of
