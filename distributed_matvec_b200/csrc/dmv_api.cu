@@ -449,6 +449,14 @@ void upload_orbit(dmv_context *ctx) {
   if (ctx->opt.canon >= 0) { P.tor_mode = 0; P.chain_dihedral = 0; }   // 1: round-1 forms (coset chain / four run searches)
   if (ctx->opt.canon == 2) { P.canon_lut2 = nullptr; P.cc_n = 0; P.cc_stages = 0; }   // first version: single-block LUT, independent networks
   if (ctx->opt.canon == 0) P.canon_mode = 0;
+  // the row form of the square-torus minimum in k_rows: checked on the host against the single-state form for every flip
+  // mask of the operator; a disagreement leaves k_rows on the generic orbit walk
+  if (P.canon_mode != 0 && P.tor_mode == 2 && P.canon_k == P.canon_r && (P.canon_k == 4 || P.canon_k == 6)) {
+    std::vector<uint64_t> flips;
+    for (const LutGroup &g : ctx->h_pull.groups) flips.push_back(g.x);
+    for (const LutGroup &g : ctx->h_push.groups) flips.push_back(g.x);
+    P.tor_sq_rows = torus_sq_rows_check(H.view(), flips) ? 1 : 0;
+  }
   ctx->orbit = P;
 }
 
@@ -1578,6 +1586,34 @@ int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t 
     if (reps) reps[k] = r.rep;
     if (stab) stab[k] = r.stab;
   }
+  API_END
+}
+
+extern "C++" {
+template <int K>
+static void torus_sq_rows_eval(const OrbitProgram &P, int64_t count, const uint64_t *states, int64_t n_flips,
+                        const uint64_t *flips, uint64_t *rows, uint64_t *single) {
+  for (int64_t k = 0; k < count; ++k) {
+    const uint64_t s = states[k] & P.site_mask, st = torus_sq_columns<K>(s);
+    for (int64_t f = 0; f < n_flips; ++f) {
+      const uint64_t x = flips[f] & P.site_mask;
+      rows[k * n_flips + f] = orbit_min_torus_sq_t<K>(P, s ^ x, st ^ torus_sq_columns<K>(x));
+      single[k * n_flips + f] = orbit_min_torus_sq<K>(P, s ^ x);
+    }
+  }
+}
+}
+
+int dmv_debug_torus_sq_rows(const dmv_basis_desc *basis, int64_t count, const uint64_t *states, int64_t n_flips,
+                            const uint64_t *flips, uint64_t *rows, uint64_t *single) {
+  API_BEGIN
+  HostOrbitProgram H = compile_orbit_program(basis->number_sites, basis->group_order, basis->perms,
+                                             basis->flips, basis->characters);
+  const OrbitProgram P = H.view();
+  if (!(P.canon_mode != 0 && P.tor_mode == 2 && P.canon_k == P.canon_r && (P.canon_k == 4 || P.canon_k == 6)))
+    throw std::runtime_error("the group has no square-torus canonical form");
+  if (P.canon_k == 6) torus_sq_rows_eval<6>(P, count, states, n_flips, flips, rows, single);
+  else torus_sq_rows_eval<4>(P, count, states, n_flips, flips, rows, single);
   API_END
 }
 

@@ -131,6 +131,8 @@ struct OrbitProgram {
   int32_t tor_mode;            // 0: off; 1: rho and sigma (4 cosets of the block rotations); 2: and tau (8 cosets)
   int32_t tor_rho_n, tor_tau_n;   // delta-swap stages of rho / tau inside tor_net_*: rho first, then tau
   int32_t tor_div_r;           // floor(bit / R) = (bit * tor_div_r) >> 16 for bit < 32
+  int32_t tor_sq_rows;         // 1: k_rows evaluates the square form per row (orbit_min_torus_sq_t), self-checked against
+                               // orbit_min_torus_sq on the probe states x every flip mask of the operator
   const uint32_t *tor_lutm;    // [2^(2k)]
   const uint32_t *tor_luts;    // [2^(2k)]  (stays in global memory: read about once per state)
   const uint8_t *tor_frow;     // [4 k][2^k]: image of one row under F = flip^f rho^e rot_a, F = (2 f + e) k + a
@@ -749,58 +751,92 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus(const OrbitProgram 
   return best;
 }
 
-// The same for a K x K torus with the transposition in the group (tor_mode == 2), rows and columns in registers:
-// pass 1 is fully unrolled, 32-bit, with one shared-memory look-up per adjacent (row, row) / (column, column) pair,
-// which gives the pair's minimum in both orders (2K look-ups in all).
-// Column a of the lattice (= row a of the transposed image) comes out of one masked multiply:
+// The same for a K x K torus with the transposition in the group (tor_mode == 2), on the word w and its transpose
+// wt (the columns of w as rows): pass 1 is fully unrolled, 32-bit, with one shared-memory look-up per adjacent
+// (row, row) / (column, column) pair, which gives the pair's minimum in both orders (2K look-ups in all).
+// Both words are used with their rows repeated above bit n, uu = u | u << n (truncated to 64 bits), so that any K - 2
+// or fewer consecutive rows, cyclically, are one shift and one mask: the pair j = (row j, row j+1) is bits K j ..
+// K j + 2K - 1, i.e. the table index row(j+1) << K | row(j), whose entry holds
+//   low half:  row j+1 on top, the rows below descending (s = 0)      high half: row j on top, ascending (s = 1)
+// Candidate bit layout: bit t K + j for the low half of pair j of w (t = 0) or wt (t = 1), bit 16 + t K + j for the high.
+// Pass 2 builds the image of a candidate row by row from tor_frow[F][row] (F = flip^f rho^e rot_a on one row): its top
+// two rows are the minimal pair already, the other K - 2 are rows j+2, j+3, ..., j-1 (cyclically) in image order for
+// s = 0 and in reverse image order for s = 1, byte look-ups on a 32-bit word -- no 64-bit networks.
+// Column a of the lattice comes out of one masked multiply:
 //   t = (w >> a) & STRIDE has site (y, a) at bit K y; t * CMUL puts it at bit S + y (S = (K-1)^2; no two partial
 //   products meet, so there are no carries).
-// Pass 2 builds the image of a candidate row by row from tor_frow[F][row] (F = flip^f rho^e rot_a on one row): its top
-// two rows are the minimal pair already, the other K - 2 are byte look-ups on a 32-bit word -- no 64-bit networks.
-// Candidate bit layout here: (t, s = 0, y) -> t K + y, (t, s = 1, y) -> 16 + t K + y.
 template <int K>
-__host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgram &P, uint64_t w) {
-  constexpr int n = K * K;
+__host__ __device__ __forceinline__ uint32_t torus_sq_column(uint64_t w, int a) {
   constexpr uint32_t BM = (1u << K) - 1u;
   constexpr int S = (K - 1) * (K - 1);
-  constexpr int LOW = K * (K - 2);            // bits of the rows below the top pair
   uint32_t stride = 0, cmul = 0;
 #pragma unroll
   for (int y = 0; y < K; ++y) { stride |= 1u << (K * y); cmul |= 1u << ((K - 1) * (K - 1 - y)); }
-  uint32_t rows[2][K];
+  return ((((uint32_t)(w >> a) & stride) * cmul) >> S) & BM;
+}
+
+// The transposed lattice as a word: column a of w in bits K a .. K a + K - 1.  Transposition commutes with XOR, so the
+// transpose of b ^ x is transpose(b) ^ transpose(x): a row of the product computes transpose(b) once and every term of
+// the row only XORs in the transposed flip mask of its group (orbit_min_torus_sq_t).
+template <int K>
+__host__ __device__ __forceinline__ uint64_t torus_sq_columns(uint64_t w) {
+  uint64_t t = 0;
 #pragma unroll
-  for (int y = 0; y < K; ++y) rows[0][y] = (uint32_t)(w >> (K * y)) & BM;
-#pragma unroll
-  for (int a = 0; a < K; ++a) rows[1][a] = ((((uint32_t)(w >> a) & stride) * cmul) >> S) & BM;
+  for (int a = 0; a < K; ++a) t |= (uint64_t)torus_sq_column<K>(w, a) << (K * a);
+  return t;
+}
+
+// both 16-bit halves at once: the minimum of each half (VIMNMX.U16x2 on the device)
+__host__ __device__ __forceinline__ uint32_t min_u16x2(uint32_t a, uint32_t b) {
+#ifdef __CUDA_ARCH__
+  return __vminu2(a, b);
+#else
+  const uint32_t lo = (a & 0xffffu) < (b & 0xffffu) ? (a & 0xffffu) : (b & 0xffffu);
+  const uint32_t hi = (a >> 16) < (b >> 16) ? (a >> 16) : (b >> 16);
+  return lo | hi << 16;
+#endif
+}
+
+// min_g g(w) from w and its transpose wt = torus_sq_columns<K>(w) (layout above).  k_rows calls it per term: every term
+// of a row is w = b ^ x for the row's state b and a group's flip mask x, so wt = transpose(b) ^ transpose(x) costs one
+// XOR.  Exact for any flip mask x.  All 2K pairs are looked up, the unchanged ones too: the 32 lanes of a warp hold 32
+// different rows at 32 different terms, so the pairs one lane could skip are pairs another lane needs, and the warp would
+// issue every look-up anyway.
+// Pass 1 handles both halves of a table entry together, in packed 16-bit minima (VIMNMX.U16x2 on the device): mstar is
+// the minimum over every half, and with M1 = mstar + 1 in both halves, e_j = M1 - min(m2_j, M1) is 1 in a half equal to
+// mstar and 0 in any other (no half is below mstar, so no borrow crosses halves).  The candidate set is
+// sum_j e_j << j, taken as M1 sum_j 2^j - sum_j min(m2_j, M1) << j in 32-bit arithmetic: one packed minimum and one
+// multiply-add per pair.
+template <int K>
+__host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq_t(const OrbitProgram &P, uint64_t w, uint64_t wt) {
+  constexpr int n = K * K;
+  constexpr uint32_t BM = (1u << K) - 1u;
+  constexpr uint32_t PM = (1u << (2 * K)) - 1u;
+  constexpr int LOW = K * (K - 2);            // bits of the rows below the top pair
+  static_assert(K * (K - 1) + LOW <= 64, "the rows below the top pair must lie inside the repeated word");
+  const uint64_t uu0 = w | (w << n), uu1 = wt | (wt << n);
   const uint32_t *lutm = P.tor_lutm;
+  uint32_t m2[2][K];
+#pragma unroll
+  for (int j = 0; j < K; ++j) {
+    m2[0][j] = lutm[(uint32_t)(uu0 >> (K * j)) & PM];
+    m2[1][j] = lutm[(uint32_t)(uu1 >> (K * j)) & PM];
+  }
+  uint32_t mm = m2[0][0];
+#pragma unroll
+  for (int t = 0; t < 2; ++t)
+#pragma unroll
+    for (int j = 0; j < K; ++j)
+      if (t + j > 0) mm = min_u16x2(mm, m2[t][j]);
+  const uint32_t mstar = (mm & 0xffffu) < (mm >> 16) ? (mm & 0xffffu) : (mm >> 16);
+  const uint32_t M1 = (mstar + 1u) * 0x00010001u;   // mstar <= PM < 2^12: mstar + 1 fits a half
+  uint32_t cand = M1 * ((1u << (2 * K)) - 1u);
+#pragma unroll
+  for (int t = 0; t < 2; ++t)
+#pragma unroll
+    for (int j = 0; j < K; ++j) cand -= min_u16x2(m2[t][j], M1) << (t * K + j);
+  // pass 2
   const uint8_t *frow = P.tor_frow;
-  uint32_t md[2][K], mu[2][K];
-  uint32_t mstar = 0xffffffffu;
-#pragma unroll
-  for (int t = 0; t < 2; ++t) {
-#pragma unroll
-    for (int y = 0; y < K; ++y) {   // the pair (row y, row y+1): row y on top descending, row y+1 on top ascending
-      const uint32_t m2 = lutm[rows[t][y] << K | rows[t][(y + 1) % K]];
-      mu[t][y] = m2 & 0xffffu;
-      md[t][(y + 1) % K] = m2 >> 16;
-      mstar = mu[t][y] < mstar ? mu[t][y] : mstar;
-      mstar = md[t][(y + 1) % K] < mstar ? md[t][(y + 1) % K] : mstar;
-    }
-  }
-  uint32_t cand = 0;
-#pragma unroll
-  for (int t = 0; t < 2; ++t) {
-#pragma unroll
-    for (int y = 0; y < K; ++y) {
-      if (md[t][y] == mstar) cand |= 1u << (t * K + y);
-      if (mu[t][y] == mstar) cand |= 1u << (16 + t * K + y);
-    }
-  }
-  uint64_t u1 = 0;
-  if (cand & (((1u << K) - 1u) * 0x00010001u << K)) {   // a transposed image is among the candidates: assemble it
-#pragma unroll
-    for (int a = 0; a < K; ++a) u1 |= (uint64_t)rows[1][a] << (K * a);
-  }
   uint32_t best = 0xffffffffu;   // rows below the top pair of the best image (the top pair is mstar for every candidate)
   while (cand) {
 #ifdef __CUDA_ARCH__
@@ -810,21 +846,17 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgr
 #endif
     cand &= cand - 1;
     const int s = cb >> 4, ty = cb & 15;
-    const int t = ty >= K ? 1 : 0, y = ty - t * K;
-    const uint64_t u = t ? u1 : w;
-    const int yn = s ? (y + 1 == K ? 0 : y + 1) : (y == 0 ? K - 1 : y - 1);
-    const uint32_t idx = (((uint32_t)(u >> (K * y)) & BM) << K) | ((uint32_t)(u >> (K * yn)) & BM);
+    const int t = ty >= K ? 1 : 0, j = ty - t * K;
+    const uint64_t uu = t ? uu1 : uu0;
+    const uint32_t c = (uint32_t)(uu >> (K * j)) & PM;           // row j+1 << K | row j
+    const uint32_t idx = s ? ((c >> K) | ((c & BM) << K)) : c;   // top row << K | the row below it
 #ifdef __CUDA_ARCH__
     uint32_t Sset = __ldg(P.tor_luts + idx);
 #else
     uint32_t Sset = P.tor_luts[idx];
 #endif
-    // the K - 2 rows below the top pair, in image order (most significant first), as one LOW-bit word `below`:
-    //   s = 0: rows y-2, y-3, ...: rotate row y to the top, they are the low LOW bits, already in image order
-    //   s = 1: rows y+2, y+3, ...: rotate row y to block 0, they are blocks 2 .. K-1 in REVERSE image order
-    const int sh = s ? (K - y == K ? 0 : (K - y) * K) : (K - 1 - y) * K;   // left rotation by whole rows
-    const uint64_t ur = sh ? (((u << sh) | (u >> (n - sh))) & P.site_mask) : u;
-    const uint32_t below = s ? (uint32_t)(ur >> (2 * K)) : (uint32_t)ur & ((1u << LOW) - 1u);
+    const int jb = j + 2 >= K ? j + 2 - K : j + 2;
+    const uint32_t below = (uint32_t)(uu >> (K * jb)) & ((1u << LOW) - 1u);   // rows j+2, ..., j-1: row j+2 lowest
     while (Sset) {
 #ifdef __CUDA_ARCH__
       const int sb = __ffs((int)Sset) - 1;
@@ -843,6 +875,12 @@ __host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgr
     }
   }
   return ((uint64_t)mstar << LOW) | best;
+}
+
+// the same from w alone (the single-state entry point: self-checks, state_info, k_rows_batch)
+template <int K>
+__host__ __device__ __forceinline__ uint64_t orbit_min_torus_sq(const OrbitProgram &P, uint64_t w) {
+  return orbit_min_torus_sq_t<K>(P, w, torus_sq_columns<K>(w));
 }
 
 __host__ __device__ __forceinline__ uint64_t translation_canon(const OrbitProgram &P, uint64_t w) {

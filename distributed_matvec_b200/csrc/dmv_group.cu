@@ -513,19 +513,7 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
 
   // self-check against bit-by-bit application on random states
   OrbitProgram P = H.view();
-  std::mt19937_64 rng(12345);
-  // random states plus patterns with many tied rotations (uniform, alternating, repeated blocks, single bits)
-  std::vector<uint64_t> probes = {0ull, H.site_mask, 0x5555555555555555ull & H.site_mask,
-                                  0xaaaaaaaaaaaaaaaaull & H.site_mask, 1ull, H.site_mask >> 1,
-                                  0x3333333333333333ull & H.site_mask, 0x0f0f0f0f0f0f0f0full & H.site_mask,
-                                  0x249249249249249ull & H.site_mask, 0x1041041041041041ull & H.site_mask};
-  for (int trial = 0; trial < 256; ++trial) {
-    uint64_t v = rng() & H.site_mask;
-    if (trial & 1) v &= rng();            // sparse and dense words: long runs
-    if ((trial & 3) == 3) v = ~v & H.site_mask;
-    probes.push_back(v);
-  }
-  for (const uint64_t s : probes) {
+  for (const uint64_t s : orbit_probe_states(H.site_mask)) {
     uint64_t expect = ~0ull;
     int stab = 0;
     for (int i = 0; i < Gp; ++i) {
@@ -559,6 +547,43 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
   return H;
 }
 
+std::vector<uint64_t> orbit_probe_states(uint64_t site_mask) {
+  std::mt19937_64 rng(12345);
+  // random states plus patterns with many tied rotations (uniform, alternating, repeated blocks, single bits)
+  std::vector<uint64_t> probes = {0ull, site_mask, 0x5555555555555555ull & site_mask,
+                                  0xaaaaaaaaaaaaaaaaull & site_mask, 1ull, site_mask >> 1,
+                                  0x3333333333333333ull & site_mask, 0x0f0f0f0f0f0f0f0full & site_mask,
+                                  0x249249249249249ull & site_mask, 0x1041041041041041ull & site_mask};
+  for (int trial = 0; trial < 256; ++trial) {
+    uint64_t v = rng() & site_mask;
+    if (trial & 1) v &= rng();            // sparse and dense words: long runs
+    if ((trial & 3) == 3) v = ~v & site_mask;
+    probes.push_back(v);
+  }
+  return probes;
+}
+
+namespace {
+template <int K>
+bool torus_sq_rows_check_k(const OrbitProgram &P, const std::vector<uint64_t> &flips) {
+  for (const uint64_t s : orbit_probe_states(P.site_mask)) {
+    const uint64_t st = torus_sq_columns<K>(s);
+    for (const uint64_t x : flips) {
+      const uint64_t w = (s ^ x) & P.site_mask;
+      if (orbit_min_torus_sq_t<K>(P, w, st ^ torus_sq_columns<K>(x & P.site_mask)) != orbit_min_torus_sq<K>(P, w))
+        return false;
+    }
+  }
+  return true;
+}
+}  // namespace
+
+bool torus_sq_rows_check(const OrbitProgram &P, const std::vector<uint64_t> &flips) {
+  if (P.canon_k == 6) return torus_sq_rows_check_k<6>(P, flips);
+  if (P.canon_k == 4) return torus_sq_rows_check_k<4>(P, flips);
+  return false;
+}
+
 OrbitProgram HostOrbitProgram::view() const {
   OrbitProgram P;
   P.n_sites = n_sites;
@@ -586,6 +611,7 @@ OrbitProgram HostOrbitProgram::view() const {
   P.cc_mask = cc_mask.data();
   P.cc_delta = cc_delta.data();
   P.tor_mode = tor_mode; P.tor_rho_n = tor_rho_n; P.tor_tau_n = tor_tau_n; P.tor_div_r = tor_div_r;
+  P.tor_sq_rows = 0;
   P.tor_lutm = tor_lutm.data();
   P.tor_luts = tor_luts.data();
   P.tor_frow = tor_frow.data();

@@ -42,6 +42,11 @@ struct HostOrbitProgram {
 
 HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const int32_t *perms,
                                        const uint8_t *flips, const double *characters);
+// the states every orbit form is self-checked on: patterns with many tied images, then 256 seeded random words
+std::vector<uint64_t> orbit_probe_states(uint64_t site_mask);
+// orbit_min_torus_sq_t(s ^ x, transpose(s) ^ transpose(x)) == orbit_min_torus_sq(s ^ x) for every probe state s and
+// flip mask x (host pointers in P; square torus with K = 4 or 6 only)
+bool torus_sq_rows_check(const OrbitProgram &P, const std::vector<uint64_t> &flips);
 
 // projection mode of the basis: which branch of BatchedOperator.computeOffDiag applies
 // (reference src/BatchedOperator.chpl:89, 119, 163)

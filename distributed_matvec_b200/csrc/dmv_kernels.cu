@@ -893,6 +893,21 @@ __device__ __forceinline__ void bucket_load(const unsigned char *__restrict__ ta
 __device__ __forceinline__ void axpy(double &acc, double c, double v) { acc = fma(c, v, acc); }
 __device__ __forceinline__ void axpy(double2 &acc, double c, double2 v) { acc.x = fma(c, v.x, acc.x); acc.y = fma(c, v.y, acc.y); }
 
+// k_rows keeps two tables behind the staged ones: the directory of the ordered table (ORD) and, for the square-torus
+// form (TK > 0), the transposed flip mask of every group (torus_sq_columns), one 64-bit word per group
+struct RowsSmem { size_t dir, gxt, total; };
+__host__ __device__ inline RowsSmem rows_smem(const KernelParams &p, const SmemLayout &L, bool ord, int tk) {
+  RowsSmem R;
+  size_t off = align_up(L.total, 16);
+  R.dir = off;
+  if (ord) off += 4 * ((size_t)p.table_dir.last + 2);
+  off = align_up(off, 8);
+  R.gxt = off;
+  if (tk > 0) off += 8 * (size_t)p.n_groups;
+  R.total = (ord || tk > 0) ? off : L.total;
+  return R;
+}
+
 // two CTAs per SM: the pipeline state must stay in registers (a spilled request waits for its load at once), and the
 // latency is hidden inside the lane, not by occupancy
 // ORD: ordered table layout (see ordered_block); its directory is staged into shared memory behind the other tables, so
@@ -903,8 +918,12 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   extern __shared__ __align__(16) unsigned char smem[];
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
   const Tables<false> T = stage_tables<PROJ_GROUP, false>(p, smem, L);   // p.groups / p.lut: row-traversal tables
-  uint32_t *sdir = reinterpret_cast<uint32_t *>(smem + align_up(L.total, 16));
+  const RowsSmem RS = rows_smem(p, L, ORD, TK);
+  uint32_t *sdir = reinterpret_cast<uint32_t *>(smem + RS.dir);
   if constexpr (ORD) stage(sdir, p.table_dir.dir, (int)p.table_dir.last + 2);
+  uint64_t *sgxt = reinterpret_cast<uint64_t *>(smem + RS.gxt);
+  if constexpr (TK > 0)
+    for (int i = threadIdx.x; i < p.n_groups; i += blockDim.x) sgxt[i] = torus_sq_columns<TK>(p.groups[i].x);
   __syncthreads();
   const OrbitProgram &orbit = T.orbit;
   if constexpr (TK > 0) {
@@ -932,6 +951,7 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
     const int64_t i = p.row_begin + tile * 32 + lane;
     const bool valid = i < p.row_end;
     const uint64_t b = valid ? __ldg(row_states + i) : 0ull;
+    const uint64_t bt = TK > 0 ? torus_sq_columns<TK>(b) : 0ull;   // the row's transposed state: see orbit_min_torus_sq_t
     E acc = zero;
     int w = 0;
     RowTerms rt = row_terms<false>(T, 0, 0, min(64, p.n_groups), b);
@@ -998,9 +1018,10 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
         live0 = has;
         if (has) {
           uint64_t flip;
+          const uint64_t flip_t = TK > 0 ? sgxt[64 * w + __ffsll((long long)rt.mask) - 1] : 0ull;
           c0 = pop_term<false>(T, rt, 64 * w, b, any_s_out, flip);
           const uint64_t raw = b ^ flip;
-          if constexpr (TK > 0) want0 = orbit_min_torus_sq<TK>(orbit, raw);
+          if constexpr (TK > 0) want0 = orbit_min_torus_sq_t<TK>(orbit, raw, bt ^ flip_t);
           else want0 = orbit_representative(orbit, raw);
           uint32_t blk, bit, blk1 = 0, bit1 = 0;
           mph_position(want0, 0, H.n_blocks0, blk, bit);
@@ -1050,9 +1071,10 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
         live0 = true;
       } else if (has) {
         uint64_t flip;
+        const uint64_t flip_t = TK > 0 ? sgxt[64 * w + __ffsll((long long)rt.mask) - 1] : 0ull;
         c0 = pop_term<false>(T, rt, 64 * w, b, any_s_out, flip);
         const uint64_t raw = b ^ flip;
-        if constexpr (TK > 0) want0 = orbit_min_torus_sq<TK>(orbit, raw);
+        if constexpr (TK > 0) want0 = orbit_min_torus_sq_t<TK>(orbit, raw, bt ^ flip_t);
         else want0 = orbit_representative(orbit, raw);
         if constexpr (ORD) {
           const uint32_t blk = ordered_block(want0, p.table_dir.k_lo, p.table_dir.shift, p.table_dir.last);
@@ -1646,7 +1668,7 @@ namespace {
 template <bool CE, int TK, bool MPH, int CTAS = 2, bool ORD = false>
 void launch_rows_t(const KernelParams &p, cudaStream_t stream) {
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
-  const size_t smem_bytes = ORD ? align_up(L.total, 16) + 4 * ((size_t)p.table_dir.last + 2) : L.total;
+  const size_t smem_bytes = rows_smem(p, L, ORD, TK).total;
   auto kernel = k_rows<CE, TK, MPH, CTAS, ORD>;
   if (smem_bytes > 48 * 1024)
     DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
@@ -1705,6 +1727,7 @@ void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
 int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {
   const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
   if (k != 4 && k != 6) return 0;
+  if (!o.tor_sq_rows) return 0;   // the row form failed its self-check (upload_orbit): the generic walk
   if (k == 4 && !dense && rows_ctas == 4) return 0;   // no 4x4 build at 64 registers: the generic walk
   return k;
 }

@@ -371,6 +371,10 @@ void ls_chpl_enumerate_representatives(const void *ls_hs_basis_ptr, uint64_t low
  *   bit-by-bit permutation and evaluates the compiled program (the device functions themselves, compiled for the host)
  *   for `count` states: reps[k] = min_g g(s_k), stab[k] = |{g : g(s_k) = s_k}|.
  *   info[0..5] = {n_q, n_stages, n_t, n_left, n_right, has_flip}.
+ * dmv_debug_torus_sq_rows: for a basis whose group is the full space group of a K x K torus (K = 4 or 6), evaluates
+ *   the square-torus orbit minimum of s_k ^ x_f for every state k and flip mask f twice, with the device functions
+ *   compiled for the host: rows[k n_flips + f] through the row form k_rows runs (the transposed state XORed with the
+ *   transposed flip mask), single[...] through the single-state form.  Fails when the group has no square-torus form.
  * dmv_debug_ordered_table: builds the ordered layout of the k_rows table (complex128: one-slot buckets,
  *   `buckets_per_state` per state, at most 2^bits blocks) over the `n` ascending representatives `reps` with the device
  *   functions compiled for the host, inserts them in order and looks every one up again: block[k] = prefix block of
@@ -397,6 +401,8 @@ int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t 
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
                             uint32_t *home, uint32_t *probes);
+int dmv_debug_torus_sq_rows(const dmv_basis_desc *basis, int64_t count, const uint64_t *states, int64_t n_flips,
+                            const uint64_t *flips, uint64_t *rows, uint64_t *single);
 
 #ifdef __cplusplus
 }
