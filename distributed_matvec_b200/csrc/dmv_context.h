@@ -331,21 +331,11 @@ struct dmv_context {
     int64_t terms = 0;
   } rounds;
 
-  // Lanczos work space (dmv_lanczos)
-  DevBuf<double> lz_v[4];
-  DevBuf<double> lz_scal;
-  // Krylov work space (dmv_expm_multiply): one allocation of (krylov_dim + 1) vectors, kept and reused between calls
-  DevBuf<double> kr_basis, kr_scal, kr_partials;
-  int64_t kr_dot_vectors = 0, kr_combine_vectors = 0;   // vector passes of the last call's block kernels
-  // block Krylov-Schur (dmv_eigsh): the basis of (krylov_dim + block_size) vectors is kr_basis; scalars and partials
-  DevBuf<double> eg_scal, eg_partials;
-  int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;   // vectors read or written by the last call's block kernels
-  // spin-spin correlations (dmv_zz_correlations): per-CTA partial Gram blocks and their sum
-  DevBuf<double> zz_partials, zz_gram;
-  // finite-temperature Lanczos (dmv_lanczos_quadrature): 3 G vectors (r_{j-1}, r_j, H r_j of a group of G start vectors),
-  // the per-step scalars of a group, per-CTA partials; kept between calls
-  DevBuf<double> qd_vectors, qd_hist, qd_partials;
-  int qd_group = 0;   // G of the last call
+  // work space of the device solvers (dmv_solve.h): vectors, small scalar arrays, per-CTA partials; kept between calls
+  DevBuf<double> solver_vectors, solver_scalars, solver_partials;
+  int64_t kr_dot_vectors = 0, kr_combine_vectors = 0;   // vector passes of dmv_expm_multiply's last block kernels
+  int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;  // vectors read or written by dmv_eigsh's last block kernels
+  int qd_group = 0;   // G of the last dmv_lanczos_quadrature call
 
   ~dmv_context() {
     delete global;
@@ -455,6 +445,5 @@ void upload_peer_slots(dmv_context *ctx, int elt);
 void decide_exchange(dmv_context *ctx);
 void hashed_positions(dmv_context *ctx, int64_t count, const uint8_t *d_masks, int P, std::vector<int64_t> &counts, uint32_t *d_pos);
 std::vector<int64_t> all_gather_counts(dmv_context *ctx, const std::vector<int64_t> &mine);
-double tridiagonal_lowest(const std::vector<double> &a, const std::vector<double> &b, std::vector<double> &vec);
 
 } }  // namespace dmv::host

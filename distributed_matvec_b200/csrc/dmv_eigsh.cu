@@ -4,88 +4,9 @@
 // scalars visit the host, where the small dense Rayleigh-Ritz problem is solved by cyclic Jacobi.
 #include <cfloat>
 #include <complex>
-#include <numeric>
 
-#include "dmv_context.h"
-
-namespace dmv { namespace host {
-
-using cplx = std::complex<double>;
-
-// Eigen-decomposition A = Q diag(lam) Q^H of a Hermitian k x k matrix (row-major; (A + A^H) / 2 is used) by the cyclic
-// Jacobi method with complex rotations; lam ascending, q[r * k + i] = component r of eigenvector i.
-struct HermitianEigen {
-  int k = 0;
-  std::vector<double> lam;
-  std::vector<cplx> q;
-  HermitianEigen(int n, const std::vector<cplx> &a_in) : k(n) {
-    std::vector<cplx> a((size_t)n * n);
-    double frob = 0.0;
-    for (int i = 0; i < n; ++i)
-      for (int j = 0; j < n; ++j) {
-        a[(size_t)i * n + j] = 0.5 * (a_in[(size_t)i * n + j] + std::conj(a_in[(size_t)j * n + i]));
-        frob += std::norm(a[(size_t)i * n + j]);
-      }
-    for (int i = 0; i < n; ++i) a[(size_t)i * n + i] = a[(size_t)i * n + i].real();
-    frob = std::sqrt(frob);
-    std::vector<cplx> v((size_t)n * n, cplx(0.0, 0.0));
-    for (int i = 0; i < n; ++i) v[(size_t)i * n + i] = 1.0;
-    for (int sweep = 0;; ++sweep) {
-      double off = 0.0;
-      for (int p = 0; p < n; ++p)
-        for (int r = p + 1; r < n; ++r) off += std::norm(a[(size_t)p * n + r]);
-      if (off == 0.0 || std::sqrt(off) <= 1e-300 + 1e-22 * frob) break;
-      if (sweep == 100) throw std::runtime_error("Hermitian Jacobi eigensolver did not converge");
-      for (int p = 0; p < n; ++p)
-        for (int r = p + 1; r < n; ++r) {
-          const cplx apr = a[(size_t)p * n + r];
-          const double g = std::abs(apr);
-          if (g == 0.0) continue;
-          const double app = a[(size_t)p * n + p].real(), arr = a[(size_t)r * n + r].real();
-          if (sweep > 3 && std::fabs(app) + 100.0 * g == std::fabs(app) && std::fabs(arr) + 100.0 * g == std::fabs(arr)) {
-            a[(size_t)p * n + r] = a[(size_t)r * n + p] = 0.0;   // negligible next to both diagonal elements
-            continue;
-          }
-          // G = diag(1, conj(u)) * real rotation, u = a_pr / |a_pr|: G^H A G zeroes a_pr
-          const cplx u = apr / g, cu = std::conj(u);
-          const double theta = (arr - app) / (2.0 * g);
-          const double t = (theta >= 0.0 ? 1.0 : -1.0) / (std::fabs(theta) + std::hypot(theta, 1.0));
-          const double c = 1.0 / std::hypot(t, 1.0), s = t * c;
-          for (int i = 0; i < n; ++i) {   // columns p, r of A and of V: A G
-            cplx &x = a[(size_t)i * n + p], &y = a[(size_t)i * n + r];
-            const cplx xp = x, yp = y;
-            x = c * xp - s * cu * yp;
-            y = s * xp + c * cu * yp;
-            cplx &vx = v[(size_t)i * n + p], &vy = v[(size_t)i * n + r];
-            const cplx vxp = vx, vyp = vy;
-            vx = c * vxp - s * cu * vyp;
-            vy = s * vxp + c * cu * vyp;
-          }
-          for (int j = 0; j < n; ++j) {   // rows p, r: G^H (A G)
-            cplx &x = a[(size_t)p * n + j], &y = a[(size_t)r * n + j];
-            const cplx xp = x, yp = y;
-            x = c * xp - s * u * yp;
-            y = s * xp + c * u * yp;
-          }
-          a[(size_t)p * n + r] = a[(size_t)r * n + p] = 0.0;
-          a[(size_t)p * n + p] = a[(size_t)p * n + p].real();
-          a[(size_t)r * n + r] = a[(size_t)r * n + r].real();
-        }
-    }
-    std::vector<int> order(n);
-    std::iota(order.begin(), order.end(), 0);
-    std::stable_sort(order.begin(), order.end(),
-                     [&](int x, int y) { return a[(size_t)x * n + x].real() < a[(size_t)y * n + y].real(); });
-    lam.resize(n);
-    q.resize((size_t)n * n);
-    for (int i = 0; i < n; ++i) {
-      lam[i] = a[(size_t)order[i] * n + order[i]].real();
-      for (int r = 0; r < n; ++r) q[(size_t)r * n + i] = v[(size_t)r * n + order[i]];
-    }
-  }
-};
-
-} }  // namespace dmv::host
+#include "dmv_dense.h"
+#include "dmv_solve.h"
 
 extern "C" {
 
@@ -103,11 +24,7 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
   if (converged) *converged = 0;
   if (products) *products = 0;
   if (restarts) *restarts = 0;
-  use_device(ctx);
-  require_states(ctx);
-  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
-  if (elt == DMV_F64 && ctx->complex_coefficients)
-    throw std::runtime_error("the operator or its characters are complex: use complex vectors (DMV_C128)");
+  SolverRun run(ctx, elt, "dmv_eigsh", true);
   if (nev < 1) throw std::runtime_error("nev must be positive");
   if (!(tol > 0.0) || !std::isfinite(tol)) throw std::runtime_error("tol must be positive and finite");
   if (block_size < 0 || block_size > kMaxBlockRhs)
@@ -116,31 +33,16 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
     throw std::runtime_error("krylov_dim must be 0 (auto) or between 1 and " + std::to_string(kMaxBlockVectors - 1));
   if (max_restarts < 0) throw std::runtime_error("max_restarts must not be negative");
   if (!eigenvalues) throw std::runtime_error("eigenvalues must not be null");
-  const int P = ctx->num_ranks;
-  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_eigsh on several ranks needs dmv_comm_init");
-  const int64_t n = ctx->n_states;
-  const size_t words = (size_t)n * elt;
-  const bool ce = elt == DMV_C128;
-  cudaStream_t st = ctx->stream;
+  const int64_t n = run.n;
+  const size_t words = run.words;
+  const bool ce = run.ce;
+  cudaStream_t st = run.st;
   // scalars: [kH, kH + 2 * (65 * 6 + 36)) Gram results, [kN, kN + 12) norms of an update, [kC, ...) coefficients of an
   // update (J x R complex), [kS, ...) the coefficient matrix of a rotation (k x l complex)
   constexpr int kH = 0, kN = 1024, kC = 1040, kS = kC + 2 * kMaxBlockVectors * kMaxBlockRhs;
-  ctx->eg_scal.alloc(kS + 2 * kMaxBlockVectors * kMaxBlockVectors);
-  ctx->eg_partials.alloc(block_gram_partials());
-  double *scal = ctx->eg_scal.ptr, *partials = ctx->eg_partials.ptr;
-  auto all_reduce = [&](double *d, int count) {
-    if (P > 1) NCCL_CHECK(nccl().AllReduce(d, d, (size_t)count, ncclDouble, ncclSum, ctx->comm, st));
-  };
-  int64_t n_global = n;   // every rank takes its decisions from the GLOBAL dimension (as dmv_lanczos)
-  if (P > 1) {
-    const double mine = (double)n;
-    CUDA_CHECK(cudaMemcpyAsync(scal, &mine, sizeof(double), cudaMemcpyHostToDevice, st));
-    all_reduce(scal, 1);
-    double g = 0.0;
-    CUDA_CHECK(cudaMemcpyAsync(&g, scal, sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    n_global = (int64_t)std::llround(g);
-  }
+  double *scal = run.scalars(kS + 2 * kMaxBlockVectors * kMaxBlockVectors);
+  double *partials = run.partials(block_gram_partials());
+  const int64_t n_global = run.global_states();   // every rank takes its decisions from the GLOBAL dimension
   if (nev > n_global)
     throw std::runtime_error("nev = " + std::to_string(nev) + " exceeds the dimension of the space, " +
                              std::to_string(n_global));
@@ -155,22 +57,10 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
                              "block_size = " + std::to_string(nev + 2 * p) + " (and krylov_dim + block_size <= " +
                              std::to_string(kMaxBlockVectors) + ")");
   const int mp = m + p;
-  // the basis: one allocation of m + p vectors, kept for the next call (shared with dmv_expm_multiply); never shrunk
-  const size_t basis_words = (size_t)mp * std::max<size_t>(words, 1);
-  if (ctx->kr_basis.count < basis_words) {
-    ctx->kr_basis.release();
-    size_t free_b = 0, total_b = 0;
-    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-    const size_t need = basis_words * sizeof(double);
-    if (need > free_b)
-      throw std::runtime_error("dmv_eigsh: the Krylov basis of krylov_dim + block_size = " + std::to_string(mp) +
-                               " vectors of " + std::to_string(n) + " elements needs " + std::to_string(need) +
-                               " bytes, but only " + std::to_string(free_b) +
-                               " bytes are free on the device; use a smaller krylov_dim or block_size");
-    ctx->kr_basis.alloc(basis_words);
-  }
+  double *const basis = run.vectors(mp, "the Krylov basis of krylov_dim + block_size =",
+                                    "; use a smaller krylov_dim or block_size");
   ctx->eg_block_vectors = ctx->eg_rotate_vectors = 0;
-  auto slot = [&](int k) { return ctx->kr_basis.ptr + (size_t)k * words; };
+  auto slot = [&](int k) { return basis + (size_t)k * words; };
   auto list_of = [&](int first, int count) {
     VecList l{};
     for (int k = 0; k < count; ++k) l.p[k] = slot(first + k);
@@ -182,7 +72,7 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
     const int width = J * q + q * q;
     launch_block_gram(n, ce, list_of(0, J), J, slot(w), n, q, partials, scal + kH, st);
     ctx->eg_block_vectors += J + q;
-    all_reduce(scal + kH, 2 * width);
+    run.all_reduce(scal + kH, 2 * width);
     CUDA_CHECK(cudaMemcpyAsync(hbuf.data(), scal + kH, sizeof(double) * 2 * width, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     std::vector<cplx> h(width);
@@ -196,7 +86,7 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
     if (J) CUDA_CHECK(cudaMemcpyAsync(scal + kC, cd.data(), sizeof(double) * cd.size(), cudaMemcpyHostToDevice, st));
     launch_block_update(n, ce, list_of(0, J), J, scal + kC, slot(w), n, q, partials, scal + kN, st);
     ctx->eg_block_vectors += J + 2 * q;
-    all_reduce(scal + kN, 2 * q);
+    run.all_reduce(scal + kN, 2 * q);
     double nb[2 * kMaxBlockRhs];
     CUDA_CHECK(cudaMemcpyAsync(nb, scal + kN, sizeof(double) * 2 * q, cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
@@ -337,9 +227,7 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
     // expand: products of the block at [cur, cur + q) land at [cur + p, cur + p + q)
     while (cur < m) {
       const int q = std::min(p, m - cur), J = cur + p;
-      CUDA_CHECK(cudaMemsetAsync(slot(J), 0, (size_t)q * words * 8, st));   // products accumulate without a diagonal
-      const int rc = dmv_matvec_batch(ctx, elt, q, slot(cur), slot(J));
-      if (rc) throw std::runtime_error(g_last_error);
+      run.product(slot(cur), slot(J), q);
       prods += q;
       const std::vector<cplx> coef = orthonormalise(J, q);
       for (int r = 0; r < J + q; ++r)

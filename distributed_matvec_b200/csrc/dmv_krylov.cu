@@ -5,8 +5,8 @@
 #include <cfloat>
 #include <complex>
 
-#include "dmv_context.h"
-#include "dmv_tridiagonal.h"
+#include "dmv_dense.h"
+#include "dmv_solve.h"
 
 extern "C" {
 
@@ -20,84 +20,46 @@ int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const
   API_BEGIN
   if (products) *products = 0;
   if (error_estimate) *error_estimate = 0.0;
-  use_device(ctx);
-  require_states(ctx);
-  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  SolverRun run(ctx, elt, "dmv_expm_multiply", true);
   if (krylov_dim != 0 && (krylov_dim < 2 || krylov_dim > kMaxBlockVectors - 1))
     throw std::runtime_error("krylov_dim must be 0 (default 30) or between 2 and 64");
   if (!(tol > 0.0) || !std::isfinite(tol)) throw std::runtime_error("tol must be positive and finite");
   if (!std::isfinite(z_re) || !std::isfinite(z_im)) throw std::runtime_error("z must be finite");
   if (elt == DMV_F64 && z_im != 0.0)
     throw std::runtime_error("a complex z needs complex vectors (DMV_C128)");
-  if (elt == DMV_F64 && ctx->complex_coefficients)
-    throw std::runtime_error("the operator or its characters are complex: use complex vectors (DMV_C128)");
   if (!x || !y) throw std::runtime_error("x and y must not be null");
-  const int P = ctx->num_ranks;
-  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_expm_multiply on several ranks needs dmv_comm_init");
   const int m = krylov_dim == 0 ? 30 : krylov_dim;
-  const int64_t n = ctx->n_states;
-  const size_t words = (size_t)n * elt;
-  const bool ce = elt == DMV_C128;
+  const int64_t n = run.n;
+  const size_t words = run.words;
+  const bool ce = run.ce;
   const cplx z(z_re, z_im);
-  cudaStream_t st = ctx->stream;
+  cudaStream_t st = run.st;
   ctx->kr_dot_vectors = ctx->kr_combine_vectors = 0;
   if (z == cplx(0.0, 0.0)) {   // exp(0) = 1: x itself, bit for bit
     if (x != y && words) CUDA_CHECK(cudaMemcpyAsync(y, x, words * 8, cudaMemcpyDefault, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     return 0;
   }
-  // the basis: one allocation of m + 1 vectors, kept for the next call; never shrunk silently to what fits
-  const size_t basis_words = (size_t)(m + 1) * std::max<size_t>(words, 1);
-  if (ctx->kr_basis.count < basis_words) {
-    ctx->kr_basis.release();
-    size_t free_b = 0, total_b = 0;
-    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-    const size_t need = basis_words * sizeof(double);
-    if (need > free_b)
-      throw std::runtime_error("dmv_expm_multiply: the Krylov basis of krylov_dim + 1 = " + std::to_string(m + 1) +
-                               " vectors of " + std::to_string(n) + " elements needs " + std::to_string(need) +
-                               " bytes, but only " + std::to_string(free_b) +
-                               " bytes are free on the device; use a smaller krylov_dim");
-    ctx->kr_basis.alloc(basis_words);
-  }
+  double *const basis = run.vectors(m + 1, "the Krylov basis of krylov_dim + 1 =", "; use a smaller krylov_dim");
   // scalars: [0, 2 * 66) block dot results, [132, 134) |out|^2 of a combine, [136, 136 + 2 * 65) host coefficients
   constexpr int kNrm = 2 * (kMaxBlockVectors + 1), kCoef = kNrm + 4;
-  ctx->kr_scal.alloc(kCoef + 2 * kMaxBlockVectors);
-  ctx->kr_partials.alloc((size_t)block_partials_grid(n, ce) * (kMaxBlockVectors + 1) * 2);
-  double *scal = ctx->kr_scal.ptr, *partials = ctx->kr_partials.ptr;
+  double *scal = run.scalars(kCoef + 2 * kMaxBlockVectors);
+  double *partials = run.partials((size_t)block_partials_grid(n, ce) * (kMaxBlockVectors + 1) * 2);
   std::vector<double *> vp(m + 1);
-  for (int k = 0; k <= m; ++k) vp[k] = ctx->kr_basis.ptr + (size_t)k * words;
+  for (int k = 0; k <= m; ++k) vp[k] = basis + (size_t)k * words;
   VecList list{};
   auto set_list = [&](int J) { for (int k = 0; k < J; ++k) list.p[k] = vp[k]; };
-  // sum `count` scalars at `d` over the ranks (NCCL, on the device buffer)
-  auto all_reduce = [&](double *d, int count) {
-    if (P > 1) NCCL_CHECK(nccl().AllReduce(d, d, (size_t)count, ncclDouble, ncclSum, ctx->comm, st));
-  };
   auto fetch = [&](double *h, const double *d, int count) {
     CUDA_CHECK(cudaMemcpyAsync(h, d, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
   };
-  auto product = [&](const double *in, double *out) {
-    CUDA_CHECK(cudaMemsetAsync(out, 0, words * 8, st));   // operators without a diagonal accumulate into y (DMV:1062-1069)
-    const int rc = P == 1 ? dmv_local_matvec(ctx, elt, in, out) : dmv_matvec(ctx, elt, in, out);
-    if (rc) throw std::runtime_error(g_last_error);
-  };
   // Krylov space exhausted at the GLOBAL dimension: every rank takes the same decision (as dmv_lanczos)
-  int64_t n_global = n;
-  if (P > 1) {
-    const double mine = (double)n;
-    CUDA_CHECK(cudaMemcpyAsync(scal, &mine, sizeof(double), cudaMemcpyHostToDevice, st));
-    all_reduce(scal, 1);
-    double g = 0.0;
-    fetch(&g, scal, 1);
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    n_global = (int64_t)std::llround(g);
-  }
+  const int64_t n_global = run.global_states();
   // w = x (host or device; y may alias x: x is read in full before y is written)
   if (words) CUDA_CHECK(cudaMemcpyAsync(vp[0], x, words * 8, cudaMemcpyDefault, st));
   std::vector<double> hh(kNrm + 2), h2(kNrm + 2);
   launch_block_dot(n, ce, list, 0, vp[0], partials, scal, st);
   ctx->kr_dot_vectors += 1;
-  all_reduce(scal, 2);
+  run.all_reduce(scal, 2);
   fetch(hh.data(), scal, 2);
   CUDA_CHECK(cudaStreamSynchronize(st));
   double beta = std::sqrt(std::max(0.0, hh[0]));
@@ -114,15 +76,15 @@ int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const
     bool exact = false;
     for (int j = 0; j < m; ++j) {
       double *u = vp[j + 1];
-      product(vp[j], u);
+      run.product(vp[j], u);
       ++prods;
       const int J = j + 1;
       set_list(J);
       // h = V^H u (and |u|^2), reduced over the ranks on the device; u -= V h reads h from there: no host round trip
       launch_block_dot(n, ce, list, J, u, partials, scal, st);
-      all_reduce(scal, 2 * (J + 1));
+      run.all_reduce(scal, 2 * (J + 1));
       launch_block_combine(n, ce, 1.0, u, list, J, scal, u, partials, scal + kNrm, st);
-      all_reduce(scal + kNrm, 2);
+      run.all_reduce(scal + kNrm, 2);
       ctx->kr_dot_vectors += J + 1;
       ctx->kr_combine_vectors += J + 2;
       fetch(hh.data(), scal, 2 * (J + 1));
@@ -133,9 +95,9 @@ int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const
       double a_j = hh[2 * j];
       if (after < 0.7 * before) {   // DGKS: the pass cancelled most of u, so orthogonalise once more
         launch_block_dot(n, ce, list, J, u, partials, scal, st);
-        all_reduce(scal, 2 * (J + 1));
+        run.all_reduce(scal, 2 * (J + 1));
         launch_block_combine(n, ce, 1.0, u, list, J, scal, u, partials, scal + kNrm, st);
-        all_reduce(scal + kNrm, 2);
+        run.all_reduce(scal + kNrm, 2);
         ctx->kr_dot_vectors += J + 1;
         ctx->kr_combine_vectors += J + 2;
         fetch(h2.data(), scal, 2 * (J + 1));
@@ -172,7 +134,7 @@ int dmv_expm_multiply(dmv_context *ctx, int elt, double z_re, double z_im, const
     set_list(k);
     launch_block_combine(n, ce, 0.0, nullptr, list, k, scal + kCoef, vp[m], partials, scal + kNrm, st);
     ctx->kr_combine_vectors += k + 1;
-    all_reduce(scal + kNrm, 2);
+    run.all_reduce(scal + kNrm, 2);
     fetch(hh.data() + kNrm, scal + kNrm, 2);
     CUDA_CHECK(cudaStreamSynchronize(st));
     std::swap(vp[0], vp[m]);   // w = beta sum_j c_j V_j becomes the start of the next sub-step

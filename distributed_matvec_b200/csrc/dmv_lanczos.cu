@@ -1,90 +1,9 @@
 // dmv_lanczos.cu -- dmv_lanczos: ground state by Lanczos with all vectors resident in HBM (the consumer of the product;
 // the reference hands its product to PRIMME, src/Diagonalize.chpl:134-225).
-#include "dmv_context.h"
-
-namespace dmv { namespace host {
-
-
-// -------------------------------------------------------------------------------------------------
-// Lowest eigenpair of a symmetric tridiagonal matrix (diagonal a[0..k), off-diagonal b[0..k-1)): Sturm bisection for
-// the eigenvalue, inverse iteration for the vector.  Host side of dmv_lanczos; k is at most a few hundred.
-double tridiagonal_lowest(const std::vector<double> &a, const std::vector<double> &b, std::vector<double> &vec) {
-  const int k = (int)a.size();
-  double lo = a[0], hi = a[0];
-  for (int i = 0; i < k; ++i) {
-    const double r = (i > 0 ? std::fabs(b[i - 1]) : 0.0) + (i + 1 < k ? std::fabs(b[i]) : 0.0);
-    lo = std::min(lo, a[i] - r);
-    hi = std::max(hi, a[i] + r);
-  }
-  auto below = [&](double x) {   // number of eigenvalues < x
-    int count = 0;
-    double q = a[0] - x;
-    for (int i = 0;; ++i) {
-      if (q < 0.0) ++count;
-      if (i + 1 == k) break;
-      if (std::fabs(q) < 1e-300) q = q < 0 ? -1e-300 : 1e-300;
-      q = a[i + 1] - x - b[i] * b[i] / q;
-    }
-    return count;
-  };
-  for (int it = 0; it < 200 && hi - lo > 4e-16 * std::max(1.0, std::max(std::fabs(lo), std::fabs(hi))); ++it) {
-    const double mid = 0.5 * (lo + hi);
-    if (below(mid) >= 1) hi = mid; else lo = mid;
-  }
-  const double theta = 0.5 * (lo + hi);
-  // inverse iteration on (T - shift I): LU of a tridiagonal matrix with partial pivoting (the dgttrf / dgttrs scheme)
-  vec.assign(k, 1.0 / std::sqrt((double)k));
-  const double scale = std::max(1.0, std::max(std::fabs(lo), std::fabs(hi)));
-  const double shift = theta - 1e-13 * scale;
-  if (k > 1) {
-    std::vector<double> dl(k - 1), d(k), du(k - 1), du2(k > 2 ? k - 2 : 0, 0.0);
-    std::vector<int> piv(k - 1);
-    for (int i = 0; i < k; ++i) d[i] = a[i] - shift;
-    for (int i = 0; i + 1 < k; ++i) { dl[i] = b[i]; du[i] = b[i]; }
-    const double tiny = 1e-300;
-    for (int i = 0; i + 1 < k; ++i) {
-      if (std::fabs(d[i]) >= std::fabs(dl[i])) {
-        if (std::fabs(d[i]) < tiny) d[i] = tiny;
-        const double f = dl[i] / d[i];
-        dl[i] = f;
-        d[i + 1] -= f * du[i];
-        piv[i] = i;
-      } else {
-        const double f = d[i] / dl[i];
-        d[i] = dl[i];
-        dl[i] = f;
-        const double t = du[i];
-        du[i] = d[i + 1];
-        d[i + 1] = t - f * d[i + 1];
-        if (i + 2 < k) { du2[i] = du[i + 1]; du[i + 1] = -f * du[i + 1]; }
-        piv[i] = i + 1;
-      }
-    }
-    if (std::fabs(d[k - 1]) < tiny) d[k - 1] = tiny;
-    for (int rep = 0; rep < 4; ++rep) {
-      std::vector<double> x = vec;
-      for (int i = 0; i + 1 < k; ++i) {
-        if (piv[i] == i) x[i + 1] -= dl[i] * x[i];
-        else { const double t = x[i]; x[i] = x[i + 1]; x[i + 1] = t - dl[i] * x[i]; }
-      }
-      x[k - 1] /= d[k - 1];
-      if (k > 1) x[k - 2] = (x[k - 2] - du[k - 2] * x[k - 1]) / d[k - 2];
-      for (int i = k - 3; i >= 0; --i) x[i] = (x[i] - du[i] * x[i + 1] - du2[i] * x[i + 2]) / d[i];
-      double nrm = 0.0;
-      for (double v : x) nrm += v * v;
-      nrm = std::sqrt(nrm);
-      if (!(nrm > 0.0) || !std::isfinite(nrm)) break;
-      for (int i = 0; i < k; ++i) vec[i] = x[i] / nrm;
-    }
-  }
-  if (k == 1) vec[0] = 1.0;
-  return theta;
-}
-
-} }  // namespace dmv::host
+#include "dmv_dense.h"
+#include "dmv_solve.h"
 
 extern "C" {
-
 
 // ---- Lanczos ground-state solver on the device ("next" row f3): the consumer of the product.  The reference hands its
 // matvec to PRIMME (src/Diagonalize.chpl:134-225); here the three-term recurrence, its dot products (NCCL all-reduce
@@ -92,62 +11,47 @@ extern "C" {
 int dmv_lanczos(dmv_context *ctx, int elt, int max_iters, double tol, uint64_t seed, double *eigenvalue,
                 void *eigenvector, int *iterations, double *residual) {
   API_BEGIN
-  use_device(ctx);
-  require_states(ctx);
-  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  SolverRun run(ctx, elt, "dmv_lanczos", false);
   if (max_iters < 1) throw std::runtime_error("max_iters must be positive");
-  const int P = ctx->num_ranks;
-  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_lanczos on several ranks needs dmv_comm_init");
-  const int64_t n = ctx->n_states;
-  const size_t words = (size_t)n * elt;
-  const bool ce = elt == DMV_C128;
-  for (auto &b : ctx->lz_v) b.alloc(words);
-  ctx->lz_scal.alloc(8);
-  double *scal = ctx->lz_scal.ptr;
-  cudaStream_t st = ctx->stream;
-  auto reduce = [&](int count) {   // sum the first `count` scalars over the ranks, bring them to the host
-    if (P > 1) NCCL_CHECK(nccl().AllReduce(scal, scal, (size_t)count, ncclDouble, ncclSum, ctx->comm, st));
-    double h[4] = {0, 0, 0, 0};
-    CUDA_CHECK(cudaMemcpyAsync(h, scal, sizeof(double) * count, cudaMemcpyDeviceToHost, st));
+  const int64_t n = run.n;
+  const size_t words = run.words;
+  const bool ce = run.ce;
+  double *const vecs = run.vectors(4, "the work space of");   // v, v_prev, w and the Ritz vector
+  double *scal = run.scalars(8);
+  cudaStream_t st = run.st;
+  auto reduce = [&]() {   // sum scal[0] over the ranks, bring it to the host
+    run.all_reduce(scal, 1);
+    double h = 0.0;
+    CUDA_CHECK(cudaMemcpyAsync(&h, scal, sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
-    return std::vector<double>(h, h + count);
-  };
-  auto product = [&](const double *x, double *y) {
-    CUDA_CHECK(cudaMemsetAsync(y, 0, words * 8, st));   // operators without a diagonal accumulate into y (DMV:1062-1069)
-    const int rc = P == 1 ? dmv_local_matvec(ctx, elt, x, y) : dmv_matvec(ctx, elt, x, y);
-    if (rc) throw std::runtime_error(g_last_error);
+    return h;
   };
   auto start_vector = [&](double *v) {
     launch_fill((int64_t)words, seed, (uint64_t)ctx->rank << 40, v, st);
     CUDA_CHECK(cudaMemsetAsync(scal, 0, 8 * sizeof(double), st));
     launch_dot(n, ce, v, v, scal, st);
-    const double nrm = std::sqrt(reduce(1)[0]);
+    const double nrm = std::sqrt(reduce());
     if (!(nrm > 0.0)) throw std::runtime_error("empty basis");
     launch_scale((int64_t)words, 1.0 / nrm, v, v, false, st);
   };
   std::vector<double> alphas, betas, ritz;
   double theta = 0.0, res = 0.0;
   // every rank must take the same stopping decision: the Krylov space is exhausted at the GLOBAL dimension
-  int64_t n_global = n;
-  if (P > 1) {
-    const double mine = (double)n;
-    CUDA_CHECK(cudaMemcpyAsync(scal, &mine, sizeof(double), cudaMemcpyHostToDevice, st));
-    n_global = (int64_t)std::llround(reduce(1)[0]);
-  }
+  const int64_t n_global = run.global_states();
   {
-    double *v = ctx->lz_v[0].ptr, *u = ctx->lz_v[1].ptr, *w = ctx->lz_v[2].ptr;
+    double *v = vecs, *u = vecs + words, *w = vecs + 2 * words;
     start_vector(v);
     double beta_prev = 0.0;
     for (int j = 0; j < max_iters; ++j) {
-      product(v, w);
+      run.product(v, w);
       CUDA_CHECK(cudaMemsetAsync(scal, 0, 8 * sizeof(double), st));
       launch_dot(n, ce, v, w, scal, st);
-      const double alpha = reduce(1)[0];
+      const double alpha = reduce();
       const double coef[2] = {alpha, beta_prev};
       CUDA_CHECK(cudaMemcpyAsync(scal + 4, coef, sizeof(coef), cudaMemcpyHostToDevice, st));
       CUDA_CHECK(cudaMemsetAsync(scal, 0, sizeof(double), st));
       launch_lanczos_update(n, ce, w, v, j > 0 ? u : nullptr, scal + 4, scal, st);
-      const double beta = std::sqrt(std::max(0.0, reduce(1)[0]));
+      const double beta = std::sqrt(std::max(0.0, reduce()));
       alphas.push_back(alpha);
       theta = tridiagonal_lowest(alphas, betas, ritz);
       res = std::fabs(beta * ritz.back());
@@ -165,14 +69,14 @@ int dmv_lanczos(dmv_context *ctx, int elt, int max_iters, double tol, uint64_t s
   if (residual) *residual = res;
   if (eigenvector) {
     // second pass with the stored alpha / beta (no dot products): Ritz vector = sum_j s_j v_j
-    double *v = ctx->lz_v[0].ptr, *u = ctx->lz_v[1].ptr, *w = ctx->lz_v[2].ptr, *acc = ctx->lz_v[3].ptr;
+    double *v = vecs, *u = vecs + words, *w = vecs + 2 * words, *acc = vecs + 3 * words;
     start_vector(v);
     CUDA_CHECK(cudaMemsetAsync(acc, 0, words * 8, st));
     const int k = (int)alphas.size();
     for (int j = 0; j < k; ++j) {
       launch_scale((int64_t)words, ritz[j], v, acc, true, st);
       if (j + 1 == k) break;
-      product(v, w);
+      run.product(v, w);
       const double coef[2] = {alphas[j], j > 0 ? betas[j - 1] : 0.0};
       CUDA_CHECK(cudaMemcpyAsync(scal + 4, coef, sizeof(coef), cudaMemcpyHostToDevice, st));
       launch_lanczos_update(n, ce, w, v, j > 0 ? u : nullptr, scal + 4, scal, st);

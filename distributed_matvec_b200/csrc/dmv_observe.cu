@@ -11,11 +11,12 @@
 // diagonal is W and its last row the one-point sums.  The group average is O(|G| N^2) on the host.
 #include <cuda_runtime.h>
 
-#include "dmv_context.h"
+#include "dmv_solve.h"
 
 namespace dmv {
 
-void count_launch();
+int sm_count();                       // dmv_solver.cu
+void check_launch(const char *what);
 
 namespace {
 
@@ -119,13 +120,10 @@ int zz_run(bool launch, int64_t n, int n_sites, const uint64_t *reps, const doub
            cudaStream_t s) {
   const int rows = zz_row_tiles(n_sites), slices = zz_slices(n_sites), threads = 32 * rows * slices;
   const size_t smem = (size_t)16 * rows * 8 * CT * sizeof(double);
-  int per_sm = 0, dev = 0, sms = 0;
+  int per_sm = 0;
   cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_zz_gram<CE, CT>, threads, smem);
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t tiles = (std::max<int64_t>(n, 0) + kZzStates - 1) / kZzStates;
-  const int grid =
-      (int)std::min<int64_t>(std::max<int64_t>(tiles, 1), (int64_t)std::max(sms, 1) * std::max(per_sm, 1));
+  const int grid = (int)std::min<int64_t>(std::max<int64_t>(tiles, 1), (int64_t)sm_count() * std::max(per_sm, 1));
   if (launch) k_zz_gram<CE, CT><<<grid, threads, smem, s>>>(n, n_sites, rows, slices, reps, x, partials);
   return grid;
 }
@@ -145,12 +143,6 @@ int zz_dispatch(bool launch, int64_t n, int n_sites, const uint64_t *reps, const
   }
 }
 
-void check(const char *what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-  count_launch();
-}
-
 }  // namespace
 
 int zz_gram_columns(int n_sites) { return 8 * zz_col_tiles(n_sites); }
@@ -167,7 +159,7 @@ void launch_zz_gram(int64_t n, bool complex_elements, int n_sites, const uint64_
   if (n_sites < 1 || n_sites > 64) throw std::runtime_error("k_zz_gram: 1 to 64 sites");
   const int grid = complex_elements ? zz_dispatch<true>(true, n, n_sites, reps, x, partials, s)
                                     : zz_dispatch<false>(true, n, n_sites, reps, x, partials, s);
-  check("k_zz_gram");
+  check_launch("k_zz_gram");
   launch_reduce_partials(grid, (int)(zz_gram_size(n_sites) / 2), partials, gram, s);
 }
 
@@ -229,32 +221,26 @@ extern "C" {
 int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
                         double *magnetization) {
   API_BEGIN
-  use_device(ctx);
-  require_states(ctx);
-  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  SolverRun run(ctx, elt, "dmv_zz_correlations", false);
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
   if (!correlations) throw std::runtime_error("correlations must not be null");
-  const int P = ctx->num_ranks;
-  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_zz_correlations on several ranks needs dmv_comm_init");
   const int N = ctx->n_sites;
   const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
                              ctx->spin_inversion);
-  const int64_t n = ctx->n_states;
-  const size_t words = (size_t)n * elt;
-  cudaStream_t st = ctx->stream;
+  const int64_t n = run.n;
+  const size_t words = run.words;
+  cudaStream_t st = run.st;
   const size_t size = zz_gram_size(N);
-  ctx->zz_partials.alloc(zz_gram_partials(n, N));
-  ctx->zz_gram.alloc(size);
+  double *partials = run.partials(zz_gram_partials(n, N)), *d_gram = run.scalars(size);
   const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * words, st);
   std::vector<double> padded(size), gram((size_t)(N + 1) * N);
   std::vector<double> C((size_t)num_vectors * N * N), m((size_t)num_vectors * N);
   for (int v = 0; v < num_vectors; ++v) {
     // d_reps holds the states of every basis, the identity-index one included (dmv_basis_build enumerates them all)
-    launch_zz_gram(n, elt == DMV_C128, N, ctx->d_reps.ptr, xin.ptr + (size_t)v * words, ctx->zz_partials.ptr,
-                   ctx->zz_gram.ptr, st);
-    if (P > 1) NCCL_CHECK(nccl().AllReduce(ctx->zz_gram.ptr, ctx->zz_gram.ptr, size, ncclDouble, ncclSum, ctx->comm, st));
-    CUDA_CHECK(cudaMemcpyAsync(padded.data(), ctx->zz_gram.ptr, size * sizeof(double), cudaMemcpyDeviceToHost, st));
+    launch_zz_gram(n, run.ce, N, ctx->d_reps.ptr, xin.ptr + (size_t)v * words, partials, d_gram, st);
+    run.all_reduce(d_gram, size);
+    CUDA_CHECK(cudaMemcpyAsync(padded.data(), d_gram, size * sizeof(double), cudaMemcpyDeviceToHost, st));
     CUDA_CHECK(cudaStreamSynchronize(st));
     const int CP = zz_gram_columns(N);
     for (int i = 0; i <= N; ++i)

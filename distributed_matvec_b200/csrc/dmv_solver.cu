@@ -9,6 +9,7 @@
 #include <algorithm>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 
 #include "dmv_host.h"
 
@@ -24,6 +25,36 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int m = 16; m > 0; m >>= 1) v += __shfl_xor_sync(0xffffffffu, v, m);
   return v;
+}
+
+// The fixed-order epilogue of a CTA's reductions: value v of every thread (re[v], and im[v] when CX), summed inside the
+// warp by the xor butterfly and then over warps 0 .. 7 in order, lands in out[(blockIdx * NV + v) * 2 + {0, 1}]
+// (imaginary part 0 when !CX).  A repeated launch on the same grid writes the same bits.  The kernel declares `s` next
+// to its other shared arrays.
+template <int NV, bool CX>
+using CtaSums = double[kThreads / 32][NV][CX ? 2 : 1];
+template <int NV, bool CX>
+__device__ __forceinline__ void cta_partials(CtaSums<NV, CX> &s, const double *re, const double *im,
+                                             double *__restrict__ out) {
+#pragma unroll
+  for (int v = 0; v < NV; ++v) {
+    const double r = warp_sum(re[v]);
+    const double i = CX ? warp_sum(im[v]) : 0.0;
+    if ((threadIdx.x & 31) == 0) {
+      s[threadIdx.x >> 5][v][0] = r;
+      if constexpr (CX) s[threadIdx.x >> 5][v][1] = i;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < NV) {
+    double tr = 0.0, ti = 0.0;
+    for (int q = 0; q < kThreads / 32; ++q) {
+      tr += s[q][threadIdx.x][0];
+      if constexpr (CX) ti += s[q][threadIdx.x][1];
+    }
+    out[(blockIdx.x * NV + threadIdx.x) * 2] = tr;
+    out[(blockIdx.x * NV + threadIdx.x) * 2 + 1] = ti;
+  }
 }
 
 // out[0..1] += sum_i conj(a_i) b_i   (real vectors: out[1] untouched)
@@ -185,7 +216,7 @@ __global__ void __launch_bounds__(kThreads) k_block_combine(int64_t n, double a,
                                                             const double *__restrict__ coef, double *out,
                                                             double *__restrict__ partials) {
   __shared__ double s_c[kMaxBlockVectors][2];
-  __shared__ double s[kThreads / 32];
+  __shared__ CtaSums<1, false> s;
   for (int k = threadIdx.x; k < J; k += blockDim.x) { s_c[k][0] = coef[2 * k]; s_c[k][1] = coef[2 * k + 1]; }
   __syncthreads();
   double nrm = 0.0;
@@ -218,16 +249,7 @@ __global__ void __launch_bounds__(kThreads) k_block_combine(int64_t n, double a,
     else out[i] = re;
     nrm += re * re + im * im;
   }
-  nrm = warp_sum(nrm);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) s[warp] = nrm;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t = 0.0;
-    for (int q = 0; q < kThreads / 32; ++q) t += s[q];
-    partials[2 * blockIdx.x] = t;
-    partials[2 * blockIdx.x + 1] = 0.0;
-  }
+  cta_partials<1, false>(s, &nrm, nullptr, partials);
 }
 
 // out[2k + {0, 1}] = sum over the `blocks` CTAs of partials[(b * width + k) * 2 + {0, 1}], in a fixed order; one CTA per k
@@ -239,18 +261,8 @@ __global__ void __launch_bounds__(kThreads) k_reduce_partials(int blocks, int wi
     re += partials[((int64_t)b * width + k) * 2];
     im += partials[((int64_t)b * width + k) * 2 + 1];
   }
-  __shared__ double s_re[kThreads / 32], s_im[kThreads / 32];
-  re = warp_sum(re);
-  im = warp_sum(im);
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { s_re[warp] = re; s_im[warp] = im; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double r = 0.0, i = 0.0;
-    for (int q = 0; q < kThreads / 32; ++q) { r += s_re[q]; i += s_im[q]; }
-    out[2 * k] = r;
-    out[2 * k + 1] = i;
-  }
+  __shared__ CtaSums<1, true> s;
+  cta_partials<1, true>(s, &re, &im, out);
 }
 
 // ---- block kernels of dmv_eigsh (block Krylov-Schur): R <= 6 right-hand vectors W_0 .. W_{R-1}, w_stride elements apart
@@ -390,7 +402,7 @@ template <bool CE, int R>
 __global__ void __launch_bounds__(kThreads) k_block_update(int64_t n, VecList V, int J, const double *__restrict__ coef,
                                                            double *W, int64_t w_stride, double *__restrict__ partials) {
   __shared__ double s_c[kMaxBlockVectors * R][2];
-  __shared__ double s[kThreads / 32][R];
+  __shared__ CtaSums<R, false> s;
   for (int k = threadIdx.x; k < J * R; k += blockDim.x) { s_c[k][0] = coef[2 * k]; s_c[k][1] = coef[2 * k + 1]; }
   __syncthreads();
   double nrm[R];
@@ -432,19 +444,7 @@ __global__ void __launch_bounds__(kThreads) k_block_update(int64_t n, VecList V,
       nrm[r] += re[r] * re[r] + im[r] * im[r];
     }
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int r = 0; r < R; ++r) {
-    const double t = warp_sum(nrm[r]);
-    if (lane == 0) s[warp][r] = t;
-  }
-  __syncthreads();
-  if (threadIdx.x < R) {
-    double t = 0.0;
-    for (int q = 0; q < kThreads / 32; ++q) t += s[q][threadIdx.x];
-    partials[(blockIdx.x * R + threadIdx.x) * 2] = t;
-    partials[(blockIdx.x * R + threadIdx.x) * 2 + 1] = 0.0;
-  }
+  cta_partials<R, false>(s, nrm, nullptr, partials);
 }
 
 // In place V_j <- sum_{i < k} S_{ij} V_i for j < l <= k, S[2 (i l + j) + {0, 1}] in device memory (real vectors use the
@@ -544,21 +544,8 @@ __global__ void __launch_bounds__(kThreads) k_quad_dot(int64_t n, const double *
       }
     }
   }
-  __shared__ double s[kThreads / 32][G][2];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int g = 0; g < G; ++g) {
-    const double r = warp_sum(re[g]);
-    const double t = CE ? warp_sum(im[g]) : 0.0;
-    if (lane == 0) { s[warp][g][0] = r; s[warp][g][1] = t; }
-  }
-  __syncthreads();
-  if (threadIdx.x < G) {
-    double r = 0.0, t = 0.0;
-    for (int q = 0; q < kThreads / 32; ++q) { r += s[q][threadIdx.x][0]; t += s[q][threadIdx.x][1]; }
-    partials[(blockIdx.x * G + threadIdx.x) * 2] = r;
-    partials[(blockIdx.x * G + threadIdx.x) * 2 + 1] = t;
-  }
+  __shared__ CtaSums<G, true> s;   // real vectors too: their imaginary sums are zeros, as they always were
+  cta_partials<G, true>(s, re, im, partials);
 }
 
 // Step j of G recurrences r_{j+1} = W / beta_j - alpha_j r_j / beta_j - beta_j r_{j-1} / beta_{j-1}, written over
@@ -571,7 +558,7 @@ __global__ void __launch_bounds__(kThreads) k_quad_update(int64_t n, double *P, 
                                                           int j, double *__restrict__ partials) {
   __shared__ double s_c[G][3];   // 1 / beta_j, alpha_j / beta_j, beta_j / beta_{j-1}
   __shared__ int s_dead[G];
-  __shared__ double s[kThreads / 32][G];
+  __shared__ CtaSums<G, false> s;
   if (threadIdx.x < G) {
     const int g = threadIdx.x;
     const double bj2 = b2[2 * (j * G + g)];
@@ -616,20 +603,10 @@ __global__ void __launch_bounds__(kThreads) k_quad_update(int64_t n, double *P, 
       }
     }
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int g = 0; g < G; ++g) {
-    const double t = warp_sum(nrm[g]);
-    if (lane == 0) s[warp][g] = t;
-  }
-  __syncthreads();
-  if (threadIdx.x < G) {
-    double t = 0.0;
-    for (int q = 0; q < kThreads / 32; ++q) t += s[q][threadIdx.x];
-    partials[(blockIdx.x * G + threadIdx.x) * 2] = t;
-    partials[(blockIdx.x * G + threadIdx.x) * 2 + 1] = 0.0;
-  }
+  cta_partials<G, false>(s, nrm, nullptr, partials);
 }
+
+}  // namespace
 
 int sm_count() {
   int dev = 0, sms = 0;
@@ -638,170 +615,122 @@ int sm_count() {
   return sms > 0 ? sms : 132;
 }
 
-// one wave of resident CTAs (at least one, so that an empty block still writes its partials)
-template <typename K>
-int one_wave(K kernel, int64_t work_items) {
-  int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, 0);
-  if (per_sm < 1) per_sm = 1;
-  int64_t b = (work_items + kThreads - 1) / kThreads;
-  b = std::min<int64_t>(std::max<int64_t>(b, 1), (int64_t)sm_count() * per_sm);
-  return (int)b;
-}
-
-int blocks_for(int64_t n) {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  if (sms <= 0) sms = 132;
-  int64_t b = (n + kThreads - 1) / kThreads;
-  if (b < 1) b = 1;
-  if (b > (int64_t)sms * 8) b = (int64_t)sms * 8;
-  return (int)b;
-}
-
-void check(const char *what) {
+void check_launch(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
   count_launch();
+}
+
+namespace {
+
+constexpr int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
+
+// `ctas` CTAs' worth of work, at least one (so that an empty block still writes its partials), at most per_sm per SM
+int clamp_grid(int64_t ctas, int per_sm) {
+  return (int)std::min<int64_t>(std::max<int64_t>(ctas, 1), (int64_t)sm_count() * std::max(per_sm, 1));
+}
+
+// the vector kernels with atomic or no reductions: eight CTAs per SM at most
+int blocks_for(int64_t n) { return clamp_grid(ceil_div(n, kThreads), 8); }
+
+// one wave of resident CTAs of `kernel` (`threads` each, `smem` bytes of dynamic shared memory: the opt-in above 48 KB
+// is set here) over `ctas` CTAs' worth of work
+template <typename K>
+int one_wave(K kernel, int64_t ctas, size_t smem = 0, int threads = kThreads) {
+  if (smem > 48 * 1024)
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
+  int per_sm = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem);
+  return clamp_grid(ctas, per_sm);
+}
+
+// f(std::integral_constant<bool, CE>) for complex / real elements
+template <typename F>
+auto with_ce(bool complex_elements, F &&f) {
+  return complex_elements ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// f(std::integral_constant<int, W>) for the W = 1 .. kMaxBlockRhs vectors of a block or a group
+template <typename F>
+void with_width(int w, F &&f) {
+  switch (w) {
+    case 1: f(std::integral_constant<int, 1>{}); break;
+    case 2: f(std::integral_constant<int, 2>{}); break;
+    case 3: f(std::integral_constant<int, 3>{}); break;
+    case 4: f(std::integral_constant<int, 4>{}); break;
+    case 5: f(std::integral_constant<int, 5>{}); break;
+    default: f(std::integral_constant<int, 6>{}); break;
+  }
 }
 
 }  // namespace
 
 void launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s) {
   if (n <= 0) return;
-  if (complex_elements) k_dot<true><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2);
-  else k_dot<false><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2);
-  check("k_dot");
+  with_ce(complex_elements, [&](auto ce) { k_dot<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2); });
+  check_launch("k_dot");
 }
 
 void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
                            const double *coef2, double *out1, cudaStream_t s) {
   if (n <= 0) return;
-  if (complex_elements) k_lanczos_update<true><<<blocks_for(2 * n), kThreads, 0, s>>>(n, w, v, u, coef2, out1);
-  else k_lanczos_update<false><<<blocks_for(n), kThreads, 0, s>>>(n, w, v, u, coef2, out1);
-  check("k_lanczos_update");
+  with_ce(complex_elements, [&](auto ce) {
+    k_lanczos_update<ce()><<<blocks_for(ce() ? 2 * n : n), kThreads, 0, s>>>(n, w, v, u, coef2, out1);
+  });
+  check_launch("k_lanczos_update");
 }
 
 void launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s) {
   if (words <= 0) return;
   if (accumulate) k_scale<true><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y);
   else k_scale<false><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y);
-  check("k_scale");
+  check_launch("k_scale");
 }
 
 void launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s) {
   if (words <= 0) return;
   k_fill<<<blocks_for(words), kThreads, 0, s>>>(words, seed, offset, x);
-  check("k_fill");
+  check_launch("k_fill");
 }
 
+namespace {
+
+// CTAs of a k_block_dot / k_block_combine launch over n elements
+int block_dot_grid(int64_t n, bool complex_elements) {
+  return with_ce(complex_elements, [&](auto ce) {
+    return one_wave(k_block_dot<ce()>, ceil_div(ceil_div(std::max<int64_t>(n, 0), dot_elems<ce()>()), kThreads));
+  });
+}
+int block_combine_grid(int64_t n, bool complex_elements) {
+  return with_ce(complex_elements, [&](auto ce) { return one_wave(k_block_combine<ce()>, ceil_div(n, kThreads)); });
+}
+
+}  // namespace
+
 int block_partials_grid(int64_t n, bool complex_elements) {
-  const int64_t tiles = (std::max<int64_t>(n, 0) + (complex_elements ? 2 : 4) - 1) / (complex_elements ? 2 : 4);
-  const int a = complex_elements ? one_wave(k_block_dot<true>, tiles) : one_wave(k_block_dot<false>, tiles);
-  const int b = complex_elements ? one_wave(k_block_combine<true>, n) : one_wave(k_block_combine<false>, n);
-  return std::max(a, b);
+  return std::max(block_dot_grid(n, complex_elements), block_combine_grid(n, complex_elements));
 }
 
 void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
                       double *h, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_dot: bad number of vectors");
-  const int64_t tiles = (std::max<int64_t>(n, 0) + (complex_elements ? 2 : 4) - 1) / (complex_elements ? 2 : 4);
-  int grid;
-  if (complex_elements) {
-    grid = one_wave(k_block_dot<true>, tiles);
-    k_block_dot<true><<<grid, kThreads, 0, s>>>(n, V, J, w, partials);
-  } else {
-    grid = one_wave(k_block_dot<false>, tiles);
-    k_block_dot<false><<<grid, kThreads, 0, s>>>(n, V, J, w, partials);
-  }
-  check("k_block_dot");
-  k_reduce_partials<<<J + 1, kThreads, 0, s>>>(grid, J + 1, partials, h);
-  check("k_reduce_partials");
+  const int grid = block_dot_grid(n, complex_elements);
+  with_ce(complex_elements, [&](auto ce) { k_block_dot<ce()><<<grid, kThreads, 0, s>>>(n, V, J, w, partials); });
+  check_launch("k_block_dot");
+  launch_reduce_partials(grid, J + 1, partials, h, s);
 }
 
 void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
                           const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_combine: bad number of vectors");
-  int grid;
-  if (complex_elements) {
-    grid = one_wave(k_block_combine<true>, n);
-    k_block_combine<true><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
-  } else {
-    grid = one_wave(k_block_combine<false>, n);
-    k_block_combine<false><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
-  }
-  check("k_block_combine");
-  k_reduce_partials<<<1, kThreads, 0, s>>>(grid, 1, partials, nrm2);
-  check("k_reduce_partials");
+  const int grid = block_combine_grid(n, complex_elements);
+  with_ce(complex_elements, [&](auto ce) {
+    k_block_combine<ce()><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
+  });
+  check_launch("k_block_combine");
+  launch_reduce_partials(grid, 1, partials, nrm2, s);
 }
-
-namespace {
-
-// one wave of CTAs of a kernel with `smem` bytes of dynamic shared memory (the opt-in above 48 KB is set here)
-template <typename K>
-int one_wave_smem(K kernel, int64_t work_items, size_t smem) {
-  if (smem > 48 * 1024)
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-      throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
-  int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem);
-  if (per_sm < 1) per_sm = 1;
-  const int64_t b = std::min<int64_t>(std::max<int64_t>(work_items, 1), (int64_t)sm_count() * per_sm);
-  return (int)b;
-}
-
-template <bool CE, int R>
-void gram_r(int64_t n, const VecList &V, int J, const double *W, int64_t w_stride, double *partials, double *h,
-            cudaStream_t s) {
-  constexpr int E = gram_elems<CE, R>();
-  const int width = J * R + R * R;
-  const size_t smem = (size_t)(kThreads / 32) * width * (CE ? 2 : 1) * sizeof(double);
-  const int grid = one_wave_smem(k_block_gram<CE, R>, (std::max<int64_t>(n, 0) + (int64_t)kThreads * E - 1) /
-                                                          ((int64_t)kThreads * E), smem);
-  k_block_gram<CE, R><<<grid, kThreads, smem, s>>>(n, V, J, W, w_stride, partials);
-  check("k_block_gram");
-  k_reduce_partials<<<width, kThreads, 0, s>>>(grid, width, partials, h);
-  check("k_reduce_partials");
-}
-
-template <bool CE, int R>
-void update_r(int64_t n, const VecList &V, int J, const double *coef, double *W, int64_t w_stride, double *partials,
-              double *nrm2, cudaStream_t s) {
-  const int grid = one_wave_smem(k_block_update<CE, R>, (std::max<int64_t>(n, 0) + kThreads - 1) / kThreads, 0);
-  k_block_update<CE, R><<<grid, kThreads, 0, s>>>(n, V, J, coef, W, w_stride, partials);
-  check("k_block_update");
-  k_reduce_partials<<<R, kThreads, 0, s>>>(grid, R, partials, nrm2);
-  check("k_reduce_partials");
-}
-
-template <bool CE>
-void gram_dispatch(int R, int64_t n, const VecList &V, int J, const double *W, int64_t w_stride, double *partials,
-                   double *h, cudaStream_t s) {
-  switch (R) {
-    case 1: gram_r<CE, 1>(n, V, J, W, w_stride, partials, h, s); break;
-    case 2: gram_r<CE, 2>(n, V, J, W, w_stride, partials, h, s); break;
-    case 3: gram_r<CE, 3>(n, V, J, W, w_stride, partials, h, s); break;
-    case 4: gram_r<CE, 4>(n, V, J, W, w_stride, partials, h, s); break;
-    case 5: gram_r<CE, 5>(n, V, J, W, w_stride, partials, h, s); break;
-    default: gram_r<CE, 6>(n, V, J, W, w_stride, partials, h, s); break;
-  }
-}
-
-template <bool CE>
-void update_dispatch(int R, int64_t n, const VecList &V, int J, const double *coef, double *W, int64_t w_stride,
-                     double *partials, double *nrm2, cudaStream_t s) {
-  switch (R) {
-    case 1: update_r<CE, 1>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-    case 2: update_r<CE, 2>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-    case 3: update_r<CE, 3>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-    case 4: update_r<CE, 4>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-    case 5: update_r<CE, 5>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-    default: update_r<CE, 6>(n, V, J, coef, W, w_stride, partials, nrm2, s); break;
-  }
-}
-
-}  // namespace
 
 size_t block_gram_partials() {
   // the most CTAs one wave can hold (8 of 256 threads per SM) times the widest output, J R + R R with J < 65, R = 6
@@ -812,21 +741,37 @@ void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J
                        int R, double *partials, double *h, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_gram: bad number of vectors");
-  if (complex_elements) gram_dispatch<true>(R, n, V, J, W, w_stride, partials, h, s);
-  else gram_dispatch<false>(R, n, V, J, W, w_stride, partials, h, s);
+  const int width = J * R + R * R;
+  with_ce(complex_elements, [&](auto ce) {
+    with_width(R, [&](auto r) {
+      constexpr bool CE = ce();
+      constexpr int E = gram_elems<CE, r()>();
+      const size_t smem = (size_t)(kThreads / 32) * width * (CE ? 2 : 1) * sizeof(double);
+      const int grid = one_wave(k_block_gram<CE, r()>, ceil_div(std::max<int64_t>(n, 0), (int64_t)kThreads * E), smem);
+      k_block_gram<CE, r()><<<grid, kThreads, smem, s>>>(n, V, J, W, w_stride, partials);
+      check_launch("k_block_gram");
+      launch_reduce_partials(grid, width, partials, h, s);
+    });
+  });
 }
 
 void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
                          int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_update: bad number of vectors");
-  if (complex_elements) update_dispatch<true>(R, n, V, J, coef, W, w_stride, partials, nrm2, s);
-  else update_dispatch<false>(R, n, V, J, coef, W, w_stride, partials, nrm2, s);
+  with_ce(complex_elements, [&](auto ce) {
+    with_width(R, [&](auto r) {
+      const int grid = one_wave(k_block_update<ce(), r()>, ceil_div(std::max<int64_t>(n, 0), kThreads));
+      k_block_update<ce(), r()><<<grid, kThreads, 0, s>>>(n, V, J, coef, W, w_stride, partials);
+      check_launch("k_block_update");
+      launch_reduce_partials(grid, R, partials, nrm2, s);
+    });
+  });
 }
 
 void launch_reduce_partials(int blocks, int width, const double *partials, double *out, cudaStream_t s) {
   k_reduce_partials<<<width, kThreads, 0, s>>>(blocks, width, partials, out);
-  check("k_reduce_partials");
+  check_launch("k_reduce_partials");
 }
 
 void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
@@ -834,66 +779,12 @@ void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int
   if (k < 1 || k > kMaxBlockVectors || l < 1 || l > k) throw std::runtime_error("k_block_rotate: bad shape");
   if (n <= 0) return;
   const size_t smem = (size_t)k * kRotWords * sizeof(double);
-  const int64_t tiles = (n + (complex_elements ? kRotWords / 2 : kRotWords) - 1) /
-                        (complex_elements ? kRotWords / 2 : kRotWords);
-  if (complex_elements) {
-    const int grid = one_wave_smem(k_block_rotate<true>, tiles, smem);
-    k_block_rotate<true><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
-  } else {
-    const int grid = one_wave_smem(k_block_rotate<false>, tiles, smem);
-    k_block_rotate<false><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
-  }
-  check("k_block_rotate");
+  with_ce(complex_elements, [&](auto ce) {
+    const int grid = one_wave(k_block_rotate<ce()>, ceil_div(n, ce() ? kRotWords / 2 : kRotWords), smem);
+    k_block_rotate<ce()><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
+  });
+  check_launch("k_block_rotate");
 }
-
-namespace {
-
-template <bool CE, int G>
-void quad_dot_g(int64_t n, const double *A, const double *B, double *partials, double *out, cudaStream_t s) {
-  const int grid = one_wave(k_quad_dot<CE, G>, n);
-  k_quad_dot<CE, G><<<grid, kThreads, 0, s>>>(n, A, B, partials);
-  check("k_quad_dot");
-  k_reduce_partials<<<G, kThreads, 0, s>>>(grid, G, partials, out);
-  check("k_reduce_partials");
-}
-
-template <bool CE, int G>
-void quad_update_g(int64_t n, double *P, double *Q, const double *W, const double *dot, const double *b2, int j,
-                   double *partials, double *nrm2, cudaStream_t s) {
-  const int grid = one_wave(k_quad_update<CE, G>, n);
-  k_quad_update<CE, G><<<grid, kThreads, 0, s>>>(n, P, Q, W, dot, b2, j, partials);
-  check("k_quad_update");
-  k_reduce_partials<<<G, kThreads, 0, s>>>(grid, G, partials, nrm2);
-  check("k_reduce_partials");
-}
-
-template <bool CE>
-void quad_dot_dispatch(int G, int64_t n, const double *A, const double *B, double *partials, double *out,
-                       cudaStream_t s) {
-  switch (G) {
-    case 1: quad_dot_g<CE, 1>(n, A, B, partials, out, s); break;
-    case 2: quad_dot_g<CE, 2>(n, A, B, partials, out, s); break;
-    case 3: quad_dot_g<CE, 3>(n, A, B, partials, out, s); break;
-    case 4: quad_dot_g<CE, 4>(n, A, B, partials, out, s); break;
-    case 5: quad_dot_g<CE, 5>(n, A, B, partials, out, s); break;
-    default: quad_dot_g<CE, 6>(n, A, B, partials, out, s); break;
-  }
-}
-
-template <bool CE>
-void quad_update_dispatch(int G, int64_t n, double *P, double *Q, const double *W, const double *dot, const double *b2,
-                          int j, double *partials, double *nrm2, cudaStream_t s) {
-  switch (G) {
-    case 1: quad_update_g<CE, 1>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-    case 2: quad_update_g<CE, 2>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-    case 3: quad_update_g<CE, 3>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-    case 4: quad_update_g<CE, 4>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-    case 5: quad_update_g<CE, 5>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-    default: quad_update_g<CE, 6>(n, P, Q, W, dot, b2, j, partials, nrm2, s); break;
-  }
-}
-
-}  // namespace
 
 size_t quad_partials(int G) {
   // the most CTAs one wave can hold (8 of 256 threads per SM) times G (re, im) pairs
@@ -903,23 +794,36 @@ size_t quad_partials(int G) {
 void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
                       double *x, cudaStream_t s) {
   if (n <= 0) return;
-  if (complex_elements) k_quad_fill<true><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
-  else k_quad_fill<false><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
-  check("k_quad_fill");
+  with_ce(complex_elements, [&](auto ce) {
+    k_quad_fill<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
+  });
+  check_launch("k_quad_fill");
 }
 
 void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
                      double *out, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_dot: bad number of vectors");
-  if (complex_elements) quad_dot_dispatch<true>(G, n, A, B, partials, out, s);
-  else quad_dot_dispatch<false>(G, n, A, B, partials, out, s);
+  with_ce(complex_elements, [&](auto ce) {
+    with_width(G, [&](auto g) {
+      const int grid = one_wave(k_quad_dot<ce(), g()>, ceil_div(n, kThreads));
+      k_quad_dot<ce(), g()><<<grid, kThreads, 0, s>>>(n, A, B, partials);
+      check_launch("k_quad_dot");
+      launch_reduce_partials(grid, G, partials, out, s);
+    });
+  });
 }
 
 void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
                         const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_update: bad number of vectors");
-  if (complex_elements) quad_update_dispatch<true>(G, n, P, Q, W, dot, b2, j, partials, nrm2, s);
-  else quad_update_dispatch<false>(G, n, P, Q, W, dot, b2, j, partials, nrm2, s);
+  with_ce(complex_elements, [&](auto ce) {
+    with_width(G, [&](auto g) {
+      const int grid = one_wave(k_quad_update<ce(), g()>, ceil_div(n, kThreads));
+      k_quad_update<ce(), g()><<<grid, kThreads, 0, s>>>(n, P, Q, W, dot, b2, j, partials);
+      check_launch("k_quad_update");
+      launch_reduce_partials(grid, G, partials, nrm2, s);
+    });
+  });
 }
 
 }  // namespace dmv

@@ -3,8 +3,8 @@
 // T_M; its Gauss quadrature (nodes theta_k, weights |r|^2 Q_0k^2) estimates <r|f(H)|r> = sum_k w_k f(theta_k), exact for
 // polynomials of degree below 2M.  The recurrences of a group of G start vectors share one batched product per step;
 // their scalars stay on the device until the group is done, and only then visit the host, where each T_M is solved.
-#include "dmv_context.h"
-#include "dmv_tridiagonal.h"
+#include "dmv_dense.h"
+#include "dmv_solve.h"
 
 extern "C" {
 
@@ -15,63 +15,31 @@ int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps
                            double *nodes, double *weights, int *steps_done, int *products) {
   API_BEGIN
   if (products) *products = 0;
-  use_device(ctx);
-  require_states(ctx);
-  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
-  if (elt == DMV_F64 && ctx->complex_coefficients)
-    throw std::runtime_error("the operator or its characters are complex: use complex vectors (DMV_C128)");
+  SolverRun run(ctx, elt, "dmv_lanczos_quadrature", true);
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (steps < 1) throw std::runtime_error("steps must be positive");
   if (!nodes || !weights) throw std::runtime_error("nodes and weights must not be null");
-  const int P = ctx->num_ranks;
-  if (P > 1 && !ctx->comm) throw std::runtime_error("dmv_lanczos_quadrature on several ranks needs dmv_comm_init");
-  const int64_t n = ctx->n_states;
-  const size_t words = (size_t)n * elt;
-  const bool ce = elt == DMV_C128;
-  cudaStream_t st = ctx->stream;
-  auto all_reduce = [&](double *d, int count) {
-    if (P > 1) NCCL_CHECK(nccl().AllReduce(d, d, (size_t)count, ncclDouble, ncclSum, ctx->comm, st));
-  };
+  const int P = run.P;
+  const int64_t n = run.n;
+  const size_t words = run.words;
+  const bool ce = run.ce;
+  cudaStream_t st = run.st;
   // group width G: the vectors one batched product shares (dmv_matvec_batch): four on k_gather, six doubles per state
   // on k_rows_batch, else one
   int width = 1;
   if (P == 1 && use_pull(ctx) && use_gather(ctx)) width = 4;
   else if (P == 1 && use_pull(ctx) && use_rows(ctx) && ctx->opt.rows_batch != 0) width = kMaxBlockRhs / elt;
   const int G = std::min(width, num_vectors);
-  ctx->qd_partials.alloc(quad_partials(G));
-  ctx->qd_hist.alloc(2);
+  double *partials = run.partials(quad_partials(G));
   // steps cap at the GLOBAL dimension (every rank takes the same decision, as dmv_lanczos)
-  int64_t n_global = n;
-  if (P > 1) {
-    const double mine = (double)n;
-    CUDA_CHECK(cudaMemcpyAsync(ctx->qd_hist.ptr, &mine, sizeof(double), cudaMemcpyHostToDevice, st));
-    all_reduce(ctx->qd_hist.ptr, 1);
-    double g = 0.0;
-    CUDA_CHECK(cudaMemcpyAsync(&g, ctx->qd_hist.ptr, sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    n_global = (int64_t)std::llround(g);
-  }
+  const int64_t n_global = run.global_states();
   if (n_global < 1) throw std::runtime_error("the basis is empty");
   const int M = (int)std::min<int64_t>(steps, n_global);
   // per step t and vector g: dot[2 (t G + g)] = <r_t, H r_t>, b2[2 (t G + g)] = |r_t|^2 (odd slots: imaginary parts)
-  ctx->qd_hist.alloc((size_t)2 * G * (2 * (size_t)M + 1));
-  // the three vectors of every recurrence of a group: one allocation, kept for the next call; never shrunk silently
-  const size_t vec_words = (size_t)3 * G * std::max<size_t>(words, 1);
-  if (ctx->qd_vectors.count < vec_words) {
-    ctx->qd_vectors.release();
-    size_t free_b = 0, total_b = 0;
-    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
-    const size_t need = vec_words * sizeof(double);
-    if (need > free_b)
-      throw std::runtime_error("dmv_lanczos_quadrature: a group of " + std::to_string(G) + " recurrences keeps " +
-                               std::to_string(3 * G) + " vectors of " + std::to_string(n) + " elements, which needs " +
-                               std::to_string(need) + " bytes, but only " + std::to_string(free_b) +
-                               " bytes are free on the device");
-    ctx->qd_vectors.alloc(vec_words);
-  }
+  double *hist_dot = run.scalars((size_t)2 * G * (2 * (size_t)M + 1)), *hist_b2 = hist_dot + (size_t)2 * G * M;
+  // the three vectors of every recurrence of a group
+  double *const vecs = run.vectors(3 * G, "the work space of a group of " + std::to_string(G) + " recurrences, 3 G =");
   ctx->qd_group = G;
-  double *hist_dot = ctx->qd_hist.ptr, *hist_b2 = ctx->qd_hist.ptr + (size_t)2 * G * M;
-  double *partials = ctx->qd_partials.ptr;
   const char *start_bytes = static_cast<const char *>(start);
   std::fill(nodes, nodes + (size_t)num_vectors * steps, 0.0);
   std::fill(weights, weights + (size_t)num_vectors * steps, 0.0);
@@ -79,7 +47,7 @@ int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps
   int64_t prods = 0;
   for (int r0 = 0; r0 < num_vectors; r0 += G) {
     const int g = std::min(G, num_vectors - r0);   // this group's width: the step stride of the scalars too
-    double *Pb = ctx->qd_vectors.ptr, *Qb = Pb + (size_t)G * words, *Wb = Pb + (size_t)2 * G * words;
+    double *Pb = vecs, *Qb = Pb + (size_t)G * words, *Wb = Pb + (size_t)2 * G * words;
     auto dot_of = [&](int t) { return hist_dot + (size_t)2 * t * g; };
     auto b2_of = [&](int t) { return hist_b2 + (size_t)2 * t * g; };
     if (start) {
@@ -90,7 +58,7 @@ int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps
       launch_quad_fill(n, ce, ctx->d_reps.ptr, seed, r0, g, Qb, st);
     }
     launch_quad_dot(n, ce, g, Qb, Qb, partials, b2_of(0), st);
-    all_reduce(b2_of(0), 2 * g);
+    run.all_reduce(b2_of(0), 2 * g);
     if (start) {   // a zero start vector is an error: one synchronisation per group, before its recurrence
       hb2.resize((size_t)2 * g);
       CUDA_CHECK(cudaMemcpyAsync(hb2.data(), b2_of(0), sizeof(double) * 2 * g, cudaMemcpyDeviceToHost, st));
@@ -100,15 +68,12 @@ int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps
           throw std::runtime_error("start vector " + std::to_string(r0 + v) + " is a zero vector");
     }
     for (int j = 0; j < M; ++j) {
-      if (ctx->h_diag_kept == 0)   // operators without a diagonal accumulate into y (DMV:1062-1069)
-        CUDA_CHECK(cudaMemsetAsync(Wb, 0, (size_t)g * words * 8, st));
-      const int rc = dmv_matvec_batch(ctx, elt, g, Qb, Wb);
-      if (rc) throw std::runtime_error(g_last_error);
+      run.product(Qb, Wb, g);
       launch_quad_dot(n, ce, g, Qb, Wb, partials, dot_of(j), st);
-      all_reduce(dot_of(j), 2 * g);
+      run.all_reduce(dot_of(j), 2 * g);
       if (j + 1 == M) break;
       launch_quad_update(n, ce, g, Pb, Qb, Wb, hist_dot, hist_b2, j, partials, b2_of(j + 1), st);
-      all_reduce(b2_of(j + 1), 2 * g);
+      run.all_reduce(b2_of(j + 1), 2 * g);
       std::swap(Pb, Qb);
     }
     prods += (int64_t)g * M;

@@ -9,54 +9,24 @@ Every rank evolves its hashed block of x with the collective call, converts its 
 (dmv_hashed_to_block) and compares its chunk with y = exp(z H) x of a one-rank context over the whole basis.  Each line
 ends in OK or FAIL; used by tests/test_expm_multiply.py.
 """
-import os
-import socket
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.distributed as dist  # noqa: E402
+import numpy as np
+import torch
+import torch.distributed as dist
 
-from distributed_matvec_b200 import DistributedOperator, Operator, load_config_from_yaml  # noqa: E402
-from distributed_matvec_b200.config import basis_from_dict, operator_from_dict  # noqa: E402
-from oracle import pyoracle as po  # noqa: E402
+from rank_harness import Ranks, load
+from distributed_matvec_b200 import DistributedOperator, Operator
+from oracle import pyoracle as po
 
 DEFAULT = ["heisenberg_chain_10", "heisenberg_square_4x4", "heisenberg_chain_24_symm", "momentum_sector",
            "heisenberg_chain_24"]
 
 
-def load(name):
-    if name == "momentum_sector":   # translation symmetry with a complex character (momentum sector 1)
-        basis = basis_from_dict({"number_spins": 10, "hamming_weight": 5,
-                                 "symmetries": [{"permutation": [(i + 1) % 10 for i in range(10)], "sector": 1}]})
-        terms = [{"expression": f"σ{c}₀ σ{c}₁", "sites": [[i, (i + 1) % 10] for i in range(10)]} for c in "ˣʸᶻ"]
-        return basis, operator_from_dict({"terms": terms}, basis)
-    return load_config_from_yaml(os.path.join(ROOT, "data", name + ".yaml"))
-
-
 def main():
-    rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); local = int(os.environ["LOCAL_RANK"])
-    local %= torch.cuda.device_count()
-    if torch.cuda.device_count() < world:
-        os.environ["NCCL_HOSTID"] = f"{socket.gethostname()}-rank{rank}"
-        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
-        os.environ.setdefault("NCCL_IB_DISABLE", "1")
-    torch.cuda.set_device(local)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    names = sys.argv[1:] or DEFAULT
-    failures = 0
-
-    def verdict(good, text):
-        nonlocal failures
-        flag = torch.tensor([0 if good else 1], device="cuda")
-        dist.all_reduce(flag)
-        if rank == 0:
-            print(f"{text} {'OK' if int(flag) == 0 else 'FAIL'}", flush=True)
-        failures += int(flag)
-
-    for name in names:
+    ranks = Ranks()
+    rank, world, local, verdict = ranks.rank, ranks.world, ranks.local, ranks.verdict
+    for name in sys.argv[1:] or DEFAULT:
         basis, matrix = load(name)
         g = Operator(matrix, device=local)          # the whole sorted basis on one rank
         g.basis.build()
@@ -90,9 +60,7 @@ def main():
                     f"rel_diff={rel:.1e}")
         dop.op.close()
         g.close()
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(1 if failures else 0)
+    ranks.finish()
 
 
 if __name__ == "__main__":

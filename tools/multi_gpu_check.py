@@ -13,18 +13,15 @@ Also covered: the collective block <-> hashed redistribution, Lanczos across the
 tests/test_multi_gpu.py.
 """
 import os
-import socket
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.distributed as dist  # noqa: E402
+import numpy as np
+import torch
+import torch.distributed as dist
 
-from distributed_matvec_b200 import (DistributedOperator, HostExchangedProduct, HostReplicatedProduct, Operator,  # noqa: E402
-                                     load_config_from_yaml)
-from oracle import pyoracle as po  # noqa: E402
+from rank_harness import Ranks, load
+from distributed_matvec_b200 import DistributedOperator, HostExchangedProduct, HostReplicatedProduct, Operator
+from oracle import pyoracle as po
 
 DEFAULT = ["heisenberg_chain_10", "heisenberg_chain_16", "heisenberg_square_4x4", "heisenberg_chain_24_symm",
            "heisenberg_chain_24", "heisenberg_chain_32_symm", "heisenberg_square_6x6"]
@@ -44,30 +41,12 @@ def close(a, b):
 
 
 def main():
-    rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); local = int(os.environ["LOCAL_RANK"])
-    local %= torch.cuda.device_count()          # fewer GPUs than ranks: several ranks share a device
-    if torch.cuda.device_count() < world:
-        # NCCL refuses two ranks of one host on one device; as ranks of distinct hosts they talk over loopback sockets
-        # (the library's own NCCL communicator reads the same variables)
-        os.environ["NCCL_HOSTID"] = f"{socket.gethostname()}-rank{rank}"
-        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
-        os.environ.setdefault("NCCL_IB_DISABLE", "1")
-    torch.cuda.set_device(local)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    ranks = Ranks()
+    rank, world, local, verdict = ranks.rank, ranks.world, ranks.local, ranks.verdict
     po.set_num_threads(max(1, len(os.sched_getaffinity(0)) // world))
     names = sys.argv[1:] or DEFAULT
-    failures = 0
-
-    def verdict(good, text):
-        nonlocal failures
-        flag = torch.tensor([0 if good else 1], device="cuda")
-        dist.all_reduce(flag)
-        if rank == 0:
-            print(f"{text} {'OK' if int(flag) == 0 else 'FAIL'}", flush=True)
-        failures += int(flag)
-
     for name in names:
-        basis, matrix = load_config_from_yaml(os.path.join(ROOT, "data", name + ".yaml"))
+        basis, matrix = load(name)
         dop = DistributedOperator(matrix, device=local)
         dop.op.set_option("exchange", int(os.environ.get("DMV_EXCHANGE", "-1")))
         if os.environ.get("DMV_PEER_GATHER"):
@@ -147,9 +126,7 @@ def main():
                               f"{h.record_width(xd)}, replicated x)")
                 h.close()
         dop.op.close()
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(1 if failures else 0)
+    ranks.finish()
 
 
 if __name__ == "__main__":

@@ -10,44 +10,21 @@ blocks (dmv_block_to_hashed); the collective call on the blocks must give the C 
 whole basis to 1e-13 on every rank, for one vector and for a batch of two.  Each line ends in OK or FAIL; used by
 tests/test_zz_correlations.py.
 """
-import os
-import socket
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.distributed as dist  # noqa: E402
+import numpy as np
 
-from distributed_matvec_b200 import DistributedOperator, Operator  # noqa: E402
-from oracle import pyoracle as po  # noqa: E402
-from eigsh_check import load  # noqa: E402
+from rank_harness import Ranks, load
+from distributed_matvec_b200 import DistributedOperator, Operator
+from oracle import pyoracle as po
 
 DEFAULT = ["heisenberg_chain_10", "heisenberg_square_4x4", "momentum_sector", "heisenberg_chain_24"]
 
 
 def main():
-    rank = int(os.environ["RANK"]); world = int(os.environ["WORLD_SIZE"]); local = int(os.environ["LOCAL_RANK"])
-    local %= torch.cuda.device_count()
-    if torch.cuda.device_count() < world:
-        os.environ["NCCL_HOSTID"] = f"{socket.gethostname()}-rank{rank}"
-        os.environ.setdefault("NCCL_SOCKET_IFNAME", "lo")
-        os.environ.setdefault("NCCL_IB_DISABLE", "1")
-    torch.cuda.set_device(local)
-    dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    names = sys.argv[1:] or DEFAULT
-    failures = 0
-
-    def verdict(good, text):
-        nonlocal failures
-        flag = torch.tensor([0 if good else 1], device="cuda")
-        dist.all_reduce(flag)
-        if rank == 0:
-            print(f"{text} {'OK' if int(flag) == 0 else 'FAIL'}", flush=True)
-        failures += int(flag)
-
-    for name in names:
+    ranks = Ranks()
+    rank, world, local, verdict = ranks.rank, ranks.world, ranks.local, ranks.verdict
+    for name in sys.argv[1:] or DEFAULT:
         basis, matrix = load(name)
         g = Operator(matrix, device=local)          # the whole sorted basis on one rank
         g.basis.build()
@@ -69,9 +46,7 @@ def main():
             verdict(err <= 1e-13, f"{name:26s} P={world} N={n} {np.dtype(dtype).name} C, m {err:.1e}")
         dop.op.close()
         g.close()
-    dist.barrier()
-    dist.destroy_process_group()
-    sys.exit(1 if failures else 0)
+    ranks.finish()
 
 
 if __name__ == "__main__":
