@@ -437,6 +437,7 @@ struct OutArg {  // device view of an output array, copied back by finish()
 void setup_exchange(dmv_context *ctx);
 void setup_replicated(dmv_context *ctx);
 void replicated_rows(dmv_context *ctx, int elt, const void *x_cat, void *y_dev);
+const double *gather_x(dmv_context *ctx, int elt, const void *x);
 void setup_rounds(dmv_context *ctx);
 void upload_round_pointers(dmv_context *ctx, int width);
 void rounds_product(dmv_context *ctx, int elt, const void *x_dev, void *y_dev);

@@ -504,6 +504,40 @@ void decide_exchange(dmv_context *ctx) {
   }
 }
 
+// Collective, replicated-x form: this rank's block of x (host or device) into slot `rank` of every rank's gathered
+// vector; returns the gathered vector (slot r * repl_block holds rank r's block).  Peer-direct when set up, else NCCL.
+const double *gather_x(dmv_context *ctx, int elt, const void *x) {
+  const int P = ctx->num_ranks;
+  const size_t esz = (size_t)8 * elt, bytes = (size_t)ctx->n_states * esz;
+  if (ctx->peer_gather) {
+    // ---- peer-direct: my block goes straight into slot `rank` of every rank's buffer (epoch parity picks the buffer:
+    // a rank raises its flag for epoch e + 1 only after it has consumed buffer e, see DESIGN.md)
+    const void *x_dev = x;
+    if (!is_device_pointer(x)) {
+      ctx->d_x.alloc((size_t)ctx->n_states * elt);
+      CUDA_CHECK(cudaMemcpyAsync(ctx->d_x.ptr, x, bytes, cudaMemcpyHostToDevice, ctx->stream));
+      x_dev = ctx->d_x.ptr;
+    }
+    CUDA_CHECK(cudaEventRecord(ctx->ev[1], ctx->stream));
+    if (ctx->peer_slot_elt != elt) upload_peer_slots(ctx, elt);
+    const unsigned epoch = ++ctx->gather_epoch;
+    const int b = (int)(epoch & 1u);
+    const int64_t n_doubles = ctx->n_states * elt;
+    const bool wide = (n_doubles % 2 == 0) && (reinterpret_cast<uintptr_t>(x_dev) % 16 == 0) &&
+                      ((size_t)ctx->repl_block * elt) % 2 == 0;
+    launch_push_block(x_dev, n_doubles, P, ctx->d_peer_slot[b].ptr, ctx->d_push_done.ptr, ctx->d_peer_flags.ptr,
+                      ctx->rank, epoch, wide, ctx->stream);
+    launch_wait_flags(ctx->d_flags.ptr, P, epoch, ctx->d_status.ptr, ctx->stream);
+    return ctx->d_xcat.ptr + (size_t)b * ctx->repl_block * P * 2;
+  }
+  char *slot = reinterpret_cast<char *>(ctx->d_xcat.ptr) + (size_t)ctx->rank * ctx->repl_block * esz;
+  CUDA_CHECK(cudaMemcpyAsync(slot, x, bytes, cudaMemcpyDefault, ctx->stream));   // host or device x
+  CUDA_CHECK(cudaEventRecord(ctx->ev[1], ctx->stream));
+  NCCL_CHECK(nccl().AllGather(slot, ctx->d_xcat.ptr, (size_t)ctx->repl_block * elt, ncclDouble, ctx->comm,
+                              ctx->stream));
+  return ctx->d_xcat.ptr;
+}
+
 // -------------------------------------------------------------------------------------------------
 // Block <-> hashed redistribution of vectors (arrFromBlockToHashed, reference src/BlockToHashed.chpl:87-208;
 // arrFromHashedToBlock, src/HashedToBlock.chpl:67-153).  "Block" = the global array in sorted-state order cut into
@@ -598,33 +632,7 @@ int dmv_matvec(dmv_context *ctx, int elt, const void *x, void *y) {
       y_dev = ctx->d_y.ptr;
       if (ctx->h_diag_kept == 0) CUDA_CHECK(cudaMemcpyAsync(y_dev, y, bytes, cudaMemcpyHostToDevice, ctx->stream));
     }
-    const double *x_cat = ctx->d_xcat.ptr;
-    if (ctx->peer_gather) {
-      // ---- peer-direct: my block goes straight into slot `rank` of every rank's buffer (epoch parity picks the buffer:
-      // a rank raises its flag for epoch e + 1 only after it has consumed buffer e, see DESIGN.md)
-      const void *x_dev = x;
-      if (!is_device_pointer(x)) {
-        ctx->d_x.alloc((size_t)ctx->n_states * elt);
-        CUDA_CHECK(cudaMemcpyAsync(ctx->d_x.ptr, x, bytes, cudaMemcpyHostToDevice, ctx->stream));
-        x_dev = ctx->d_x.ptr;
-      }
-      CUDA_CHECK(cudaEventRecord(ctx->ev[1], ctx->stream));
-      if (ctx->peer_slot_elt != elt) upload_peer_slots(ctx, elt);
-      const unsigned epoch = ++ctx->gather_epoch;
-      const int b = (int)(epoch & 1u);
-      const int64_t n_doubles = ctx->n_states * elt;
-      const bool wide = (n_doubles % 2 == 0) && (reinterpret_cast<uintptr_t>(x_dev) % 16 == 0) &&
-                        ((size_t)ctx->repl_block * elt) % 2 == 0;
-      launch_push_block(x_dev, n_doubles, P, ctx->d_peer_slot[b].ptr, ctx->d_push_done.ptr, ctx->d_peer_flags.ptr,
-                        ctx->rank, epoch, wide, ctx->stream);
-      launch_wait_flags(ctx->d_flags.ptr, P, epoch, ctx->d_status.ptr, ctx->stream);
-      x_cat = ctx->d_xcat.ptr + (size_t)b * ctx->repl_block * P * 2;
-    } else {
-      char *slot = reinterpret_cast<char *>(ctx->d_xcat.ptr) + (size_t)ctx->rank * ctx->repl_block * esz;
-      CUDA_CHECK(cudaMemcpyAsync(slot, x, bytes, cudaMemcpyDefault, ctx->stream));   // host or device x
-      CUDA_CHECK(cudaEventRecord(ctx->ev[1], ctx->stream));
-      NCCL_CHECK(N.AllGather(slot, ctx->d_xcat.ptr, (size_t)ctx->repl_block * elt, ncclDouble, ctx->comm, ctx->stream));
-    }
+    const double *x_cat = gather_x(ctx, elt, x);
     CUDA_CHECK(cudaEventRecord(ctx->ev[6], ctx->stream));
     replicated_rows(ctx, elt, x_cat, y_dev);
     CUDA_CHECK(cudaEventRecord(ctx->ev[2], ctx->stream));

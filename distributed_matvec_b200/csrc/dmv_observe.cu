@@ -143,6 +143,236 @@ int zz_dispatch(bool launch, int64_t n, int n_sites, const uint64_t *reps, const
   }
 }
 
+// ---- flip-flop correlations (dmv_pm_correlations).  A row b and an antiparallel pair (i, j) with bit i of b set and
+// bit j clear give the term conj(x_b) / n_b chi (n x)[rep(b ^ (1 << i | 1 << j))] of the class of the ordered pair
+// (i, j); the host turns the class sums into <σ⁺ᵢσ⁻ⱼ>.  How the target's (n x) is found:
+enum PmLook {
+  PM_NONE = 0,        // no symmetry: the index of the basis
+  PM_INVERSION = 1,   // spin inversion alone: min(a, flip a), the character when flipped
+  PM_GROUP = 2,       // permutations: orbit minimum (orbit_scan and its character when they are not trivial), the index
+  PM_TABLE = 3,       // permutations, trivial characters: orbit minimum, then k_rows' hash table (x n in the slot)
+};
+
+struct PmArgs {
+  StateIndex index;          // the basis the targets are looked up in: this rank's, or the whole basis on several ranks
+  OrbitProgram orbit;
+  const double *norms;       // of index's states
+  const uint32_t *pos;       // several ranks: global index g lives at x[pos[g]]; null on one rank
+  const double *x;           // the vector (the gathered one on several ranks)
+  const uint64_t *rows;      // this rank's representatives and their norms
+  const double *row_norms;
+  int64_t n_rows, x_row_offset;
+  uint64_t site_mask;
+  double inversion_character;
+  const unsigned char *table;   // PM_TABLE: k_rows' table (table_slot / ordered layout), filled from x
+  uint32_t table_slots;
+  OrderedDir table_dir;
+  const int16_t *class_of;   // [N * N]: class of the ordered pair (i, j), -1 on the diagonal
+  const uint16_t *pairs;     // pair-major walk: the unordered pairs i | j << 8
+  int n_sites, n_pairs, c_lo, c_hi;   // classes [c_lo, c_hi) of this pass
+  double *partials;          // [grid][c_hi - c_lo][2]
+  unsigned long long *status;
+};
+
+template <bool CE>
+__device__ __forceinline__ double2 pm_load(const double *x, int64_t i) {
+  if constexpr (CE) return __ldg(reinterpret_cast<const double2 *>(x) + i);
+  else return make_double2(__ldg(x + i), 0.0);
+}
+
+// chi (n x)[rep(a)]; a target outside the basis is counted in bad / bad_state unless its projection vanishes (a
+// stabiliser sum of zero under non-trivial characters), which contributes nothing
+template <int LOOK, int TK, bool CE>
+__device__ __forceinline__ double2 pm_target(const PmArgs &A, uint64_t a, unsigned long long &bad, uint64_t &bad_state) {
+  double2 chi = make_double2(1.0, 0.0);
+  uint64_t key = a;
+  if constexpr (LOOK == PM_INVERSION) {
+    const uint64_t inv = a ^ A.site_mask;
+    if (inv < a) { key = inv; chi.x = A.inversion_character; }
+  } else if constexpr (LOOK == PM_GROUP || LOOK == PM_TABLE) {
+    if (LOOK == PM_TABLE || A.orbit.trivial_characters) {
+      if constexpr (TK > 0) key = orbit_min_torus_sq<TK>(A.orbit, a);
+      else key = orbit_representative(A.orbit, a);
+    } else {
+      const OrbitResult r = orbit_scan<false, false>(A.orbit, a);
+      key = r.rep;
+      chi = __ldg(A.orbit.characters + r.arg);   // chi(g), not conjugated: the convention of k_pull
+    }
+  }
+  if constexpr (LOOK == PM_TABLE) {
+    uint32_t bk = table_home(key, A.table_slots, A.table_dir);
+    for (;;) {
+      const ulonglong2 k = __ldg(reinterpret_cast<const ulonglong2 *>(A.table + (size_t)bk * 32));
+      const double2 v = __ldg(reinterpret_cast<const double2 *>(A.table + (size_t)bk * 32 + 16));
+      if (CE) {   // { key, spare, re, im }
+        if (k.x == key) return v;
+        if (k.x == kEmptyKey) break;
+      } else {    // { key0, key1, value0, value1 }
+        if (k.x == key) return make_double2(v.x, 0.0);
+        if (k.y == key) return make_double2(v.y, 0.0);
+        if (k.x == kEmptyKey || k.y == kEmptyKey) break;
+      }
+      bk = bk + 1 == A.table_slots ? 0 : bk + 1;
+    }
+    ++bad; bad_state = key;
+    return make_double2(0.0, 0.0);
+  } else {
+    const int64_t idx = locate(A.index, key);
+    if (idx < 0) {
+      if (LOOK != PM_GROUP || A.orbit.trivial_characters ||
+          orbit_stabiliser_sum(A.orbit, key) > 1e-12 * (double)A.orbit.group_order) { ++bad; bad_state = key; }
+      return make_double2(0.0, 0.0);
+    }
+    double2 v = pm_load<CE>(A.x, A.pos ? (int64_t)__ldg(A.pos + idx) : idx);
+    if constexpr (LOOK == PM_GROUP) {
+      const double nrm = __ldg(A.norms + idx);
+      v = make_double2(v.x * nrm, v.y * nrm);
+    }
+    return make_double2(chi.x * v.x - chi.y * v.y, chi.x * v.y + chi.y * v.x);
+  }
+}
+
+// conj(x_b) / n_b of row i
+template <int LOOK, bool CE>
+__device__ __forceinline__ double2 pm_row_factor(const PmArgs &A, int64_t i) {
+  const double2 v = pm_load<CE>(A.x, A.x_row_offset + i);
+  const double s = LOOK >= PM_GROUP ? 1.0 / __ldg(A.row_norms + i) : 1.0;
+  return make_double2(v.x * s, -v.y * s);
+}
+
+// Lane-major walk (bases with permutations: few classes).  One lane owns one row and walks all its antiparallel pairs
+// (w (N - w) at a fixed Hamming weight, the same for every lane).  Lane-private class slots in shared memory,
+// [class][thread] (real parts, then imaginary parts when CPLX), are summed in thread order = lane order, then warp order.
+template <int LOOK, int TK, bool CE, bool CPLX>
+__global__ void __launch_bounds__(256, 2) k_pm_rows(const PmArgs A) {
+  extern __shared__ double s_slot[];
+  const int T = blockDim.x, t = threadIdx.x, C = A.c_hi - A.c_lo, N = A.n_sites;
+  for (int c = 0; c < C * (CPLX ? 2 : 1); ++c) s_slot[c * T + t] = 0.0;
+  unsigned long long bad = 0;
+  uint64_t bad_state = 0;
+  for (int64_t i = (int64_t)blockIdx.x * T + t; i < A.n_rows; i += (int64_t)gridDim.x * T) {
+    const uint64_t b = __ldg(A.rows + i);
+    const double2 xb = pm_row_factor<LOOK, CE>(A, i);
+    for (uint64_t up = b & A.site_mask; up; up &= up - 1) {
+      const int si = __ffsll((long long)up) - 1;
+      const int16_t *cls = A.class_of + si * N;
+      for (uint64_t dn = ~b & A.site_mask; dn; dn &= dn - 1) {
+        const int sj = __ffsll((long long)dn) - 1;
+        const int c = (int)__ldg(cls + sj) - A.c_lo;
+        if ((unsigned)c >= (unsigned)C) continue;
+        const double2 v = pm_target<LOOK, TK, CE>(A, b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
+        s_slot[c * T + t] += xb.x * v.x - xb.y * v.y;
+        if constexpr (CPLX) s_slot[(C + c) * T + t] += xb.x * v.y + xb.y * v.x;
+      }
+    }
+  }
+  __syncthreads();
+  for (int c = t; c < C; c += T) {
+    double re = 0.0, im = 0.0;
+    for (int u = 0; u < T; ++u) {
+      re += s_slot[c * T + u];
+      if constexpr (CPLX) im += s_slot[(C + c) * T + u];
+    }
+    A.partials[((int64_t)blockIdx.x * C + c) * 2] = re;
+    A.partials[((int64_t)blockIdx.x * C + c) * 2 + 1] = im;
+  }
+  if (bad && atomicAdd(A.status, bad) == 0) A.status[1] = bad_state;
+}
+
+// Pair-major walk (bases without permutations: a class per ordered pair, or per {(i, j), (j, i)} with spin inversion).
+// The CTA's warps share a tile of 32 rows, one per lane; warp w takes the unordered pairs w, w + warps, ..., every lane
+// adds its row's term and the warp sums them by shuffles in a fixed order, one sum per direction of the pair.  The
+// classes of an unordered pair belong to one warp only, so lane 0 owns their slots in shared memory.
+template <int LOOK, bool CE>
+__global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
+  extern __shared__ double s_cls[];   // [classes] real parts, then imaginary parts
+  const int C = A.c_hi, N = A.n_sites, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+  for (int c = threadIdx.x; c < 2 * C; c += blockDim.x) s_cls[c] = 0.0;
+  __syncthreads();
+  unsigned long long bad = 0;
+  uint64_t bad_state = 0;
+  for (int64_t tile = blockIdx.x; tile * 32 < A.n_rows; tile += gridDim.x) {
+    const int64_t i = tile * 32 + lane;
+    const bool valid = i < A.n_rows;
+    const uint64_t b = valid ? __ldg(A.rows + i) : 0ull;
+    const double2 xb = valid ? pm_row_factor<LOOK, CE>(A, i) : make_double2(0.0, 0.0);
+    for (int p = warp; p < A.n_pairs; p += warps) {
+      const unsigned pr = __ldg(A.pairs + p), si = pr & 0xffu, sj = pr >> 8;
+      const bool bi = (b >> si) & 1ull, bj = (b >> sj) & 1ull;
+      double2 c = make_double2(0.0, 0.0);
+      if (valid && bi != bj) {
+        const double2 v = pm_target<LOOK, 0, CE>(A, b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
+        c = make_double2(xb.x * v.x - xb.y * v.y, xb.x * v.y + xb.y * v.x);
+      }
+      double s[4] = {bi ? c.x : 0.0, bi ? c.y : 0.0, bi ? 0.0 : c.x, bi ? 0.0 : c.y};   // (i, j), then (j, i)
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s[k] += __shfl_xor_sync(0xffffffffu, s[k], off);
+      if (lane == 0) {
+        const int cij = __ldg(A.class_of + si * N + sj), cji = __ldg(A.class_of + sj * N + si);
+        s_cls[cij] += s[0]; s_cls[C + cij] += s[1];
+        s_cls[cji] += s[2]; s_cls[C + cji] += s[3];
+      }
+    }
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    A.partials[((int64_t)blockIdx.x * C + c) * 2] = s_cls[c];
+    A.partials[((int64_t)blockIdx.x * C + c) * 2 + 1] = s_cls[C + c];
+  }
+  if (bad && atomicAdd(A.status, bad) == 0) A.status[1] = bad_state;
+}
+
+constexpr size_t kPmSmem = 96 * 1024;   // shared memory of one CTA: two CTAs per SM
+constexpr int kPmThreads = 256;
+
+template <typename K>
+int pm_grid(K kernel, int threads, size_t smem, int64_t work_blocks) {
+  CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 0;
+  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+  return (int)std::min<int64_t>(std::max<int64_t>(work_blocks, 1), (int64_t)sm_count() * std::max(per_sm, 1));
+}
+
+template <int LOOK, int TK, bool CE, bool CPLX>
+void pm_rows_run(bool launch, const PmArgs &A, int &grid, cudaStream_t s) {
+  const size_t smem = (size_t)kPmThreads * (A.c_hi - A.c_lo) * (CPLX ? 16 : 8);
+  grid = pm_grid(k_pm_rows<LOOK, TK, CE, CPLX>, kPmThreads, smem, (A.n_rows + kPmThreads - 1) / kPmThreads);
+  if (launch) k_pm_rows<LOOK, TK, CE, CPLX><<<grid, kPmThreads, smem, s>>>(A);
+}
+
+template <int LOOK, bool CE>
+void pm_pairs_run(bool launch, const PmArgs &A, int &grid, cudaStream_t s) {
+  const size_t smem = (size_t)A.c_hi * 16;
+  grid = pm_grid(k_pm_pairs<LOOK, CE>, kPmThreads, smem, (A.n_rows + 31) / 32);
+  if (launch) k_pm_pairs<LOOK, CE><<<grid, kPmThreads, smem, s>>>(A);
+}
+
+template <int LOOK, bool CE, bool CPLX>
+void pm_rows_tk(bool launch, int tk, const PmArgs &A, int &grid, cudaStream_t s) {
+  if (tk == 4) pm_rows_run<LOOK, 4, CE, CPLX>(launch, A, grid, s);
+  else if (tk == 6) pm_rows_run<LOOK, 6, CE, CPLX>(launch, A, grid, s);
+  else pm_rows_run<LOOK, 0, CE, CPLX>(launch, A, grid, s);
+}
+
+// one launch of the walk the basis asks for (launch == false: only the grid)
+void pm_dispatch(bool launch, int look, int tk, bool ce, bool cplx, const PmArgs &A, int &grid, cudaStream_t s) {
+  switch (look) {
+    case PM_NONE: return ce ? pm_pairs_run<PM_NONE, true>(launch, A, grid, s) : pm_pairs_run<PM_NONE, false>(launch, A, grid, s);
+    case PM_INVERSION:
+      return ce ? pm_pairs_run<PM_INVERSION, true>(launch, A, grid, s)
+                : pm_pairs_run<PM_INVERSION, false>(launch, A, grid, s);
+    case PM_GROUP:   // tk only with trivial characters
+      if (ce) return pm_rows_tk<PM_GROUP, true, true>(launch, tk, A, grid, s);
+      return cplx ? pm_rows_tk<PM_GROUP, false, true>(launch, tk, A, grid, s)
+                  : pm_rows_tk<PM_GROUP, false, false>(launch, tk, A, grid, s);
+    default:
+      return ce ? pm_rows_tk<PM_TABLE, true, true>(launch, tk, A, grid, s)
+                : pm_rows_tk<PM_TABLE, false, false>(launch, tk, A, grid, s);
+  }
+}
+
 }  // namespace
 
 int zz_gram_columns(int n_sites) { return 8 * zz_col_tiles(n_sites); }
@@ -212,6 +442,80 @@ void zz_symmetrize(int N, const ZzGroup &G, const double *gram, double *correlat
     for (int i = 0; i < N; ++i) magnetization[i] = m[i] * scale;
 }
 
+// W = <x|x> (the return value), C and m of one vector of this rank: k_zz_gram over this rank's rows, the block
+// all-reduced over the ranks, the group average on the host.  partials: zz_gram_partials doubles, d_gram: zz_gram_size.
+double zz_moments(SolverRun &run, const ZzGroup &G, const double *xv, double *partials, double *d_gram, double *C,
+                  double *m) {
+  const int N = run.ctx->n_sites;
+  const size_t size = zz_gram_size(N);
+  std::vector<double> padded(size), gram((size_t)(N + 1) * N);
+  // d_reps holds the states of every basis, the identity-index one included (dmv_basis_build enumerates them all)
+  launch_zz_gram(run.n, run.ce, N, run.ctx->d_reps.ptr, xv, partials, d_gram, run.st);
+  run.all_reduce(d_gram, size);
+  CUDA_CHECK(cudaMemcpyAsync(padded.data(), d_gram, size * sizeof(double), cudaMemcpyDeviceToHost, run.st));
+  CUDA_CHECK(cudaStreamSynchronize(run.st));
+  const int CP = zz_gram_columns(N);
+  for (int i = 0; i <= N; ++i)
+    for (int j = 0; j < N; ++j) gram[(size_t)i * N + j] = padded[(size_t)i * CP + j];
+  zz_symmetrize(N, G, gram.data(), C, m);
+  return gram[0];
+}
+
+// Classes of the ordered site pairs under the group: (p, no flip) sends (i, j) to (p(i), p(j)), (p, flip) to
+// (p(j), p(i)) (a global spin flip turns σ⁺σ⁻ into σ⁻σ⁺).  Numbered in the order of their first pair, row-major.
+struct PmClasses {
+  std::vector<int32_t> of;     // [N * N]: class of (i, j), -1 on the diagonal
+  std::vector<int32_t> size;   // [count]: pairs in the class
+};
+
+PmClasses pm_classes(int N, const ZzGroup &G) {
+  PmClasses K;
+  K.of.assign((size_t)N * N, -1);
+  for (int i = 0; i < N; ++i)
+    for (int j = 0; j < N; ++j) {
+      if (i == j || K.of[(size_t)i * N + j] >= 0) continue;
+      const int32_t id = (int32_t)K.size.size();
+      int32_t count = 0;
+      for (int64_t e = 0; e < G.order; ++e) {
+        const int32_t *p = G.perms.data() + e * N;
+        const int k = G.flips[e] ? p[j] : p[i], l = G.flips[e] ? p[i] : p[j];
+        if (K.of[(size_t)k * N + l] < 0) { K.of[(size_t)k * N + l] = id; ++count; }
+      }
+      K.size.push_back(count);
+    }
+  return K;
+}
+
+// pm[2 (i N + j) + {0, 1}] = <σ⁺ᵢσ⁻ⱼ> from the class sums (2 per class) for i != j, (1 + m_i) / 2 on the diagonal
+void pm_finish(int N, const PmClasses &K, const double *sums, double W, const double *m, double *pm) {
+  if (!(W > 0.0)) throw std::runtime_error("x is a zero vector: <x|x> = 0");
+  for (int i = 0; i < N; ++i)
+    for (int j = 0; j < N; ++j) {
+      double *out = pm + 2 * ((size_t)i * N + j);
+      if (i == j) { out[0] = 0.5 * (1.0 + m[i]); out[1] = 0.0; continue; }
+      const int32_t c = K.of[(size_t)i * N + j];
+      const double scale = 1.0 / (W * (double)K.size[c]);
+      out[0] = sums[2 * c] * scale;
+      out[1] = sums[2 * c + 1] * scale;
+    }
+}
+
+// sums[2 c + {0, 1}] = class sum c of the vector A.x over this rank's rows (classes < count).  The lane-major walk runs
+// once per group of classes whose slots fit in shared memory.
+void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, double *sums) {
+  const int per_pass = look <= PM_INVERSION ? count : (int)(kPmSmem / ((size_t)kPmThreads * (cplx ? 16 : 8)));
+  for (int c0 = 0; c0 < count; c0 += per_pass) {
+    A.c_lo = c0;
+    A.c_hi = std::min(count, c0 + per_pass);
+    int grid = 0;
+    pm_dispatch(false, look, tk, run.ce, cplx, A, grid, run.st);
+    A.partials = run.partials((size_t)grid * (A.c_hi - A.c_lo) * 2);
+    pm_dispatch(true, look, tk, run.ce, cplx, A, grid, run.st);
+    check_launch(look <= PM_INVERSION ? "k_pm_pairs" : "k_pm_rows");
+    launch_reduce_partials(grid, A.c_hi - A.c_lo, A.partials, sums + 2 * c0, run.st);
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -228,29 +532,127 @@ int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
   const int N = ctx->n_sites;
   const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
                              ctx->spin_inversion);
-  const int64_t n = run.n;
   const size_t words = run.words;
   cudaStream_t st = run.st;
-  const size_t size = zz_gram_size(N);
-  double *partials = run.partials(zz_gram_partials(n, N)), *d_gram = run.scalars(size);
+  double *partials = run.partials(zz_gram_partials(run.n, N)), *d_gram = run.scalars(zz_gram_size(N));
   const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * words, st);
-  std::vector<double> padded(size), gram((size_t)(N + 1) * N);
   std::vector<double> C((size_t)num_vectors * N * N), m((size_t)num_vectors * N);
-  for (int v = 0; v < num_vectors; ++v) {
-    // d_reps holds the states of every basis, the identity-index one included (dmv_basis_build enumerates them all)
-    launch_zz_gram(n, run.ce, N, ctx->d_reps.ptr, xin.ptr + (size_t)v * words, partials, d_gram, st);
-    run.all_reduce(d_gram, size);
-    CUDA_CHECK(cudaMemcpyAsync(padded.data(), d_gram, size * sizeof(double), cudaMemcpyDeviceToHost, st));
-    CUDA_CHECK(cudaStreamSynchronize(st));
-    const int CP = zz_gram_columns(N);
-    for (int i = 0; i <= N; ++i)
-      for (int j = 0; j < N; ++j) gram[(size_t)i * N + j] = padded[(size_t)i * CP + j];
-    zz_symmetrize(N, G, gram.data(), C.data() + (size_t)v * N * N, m.data() + (size_t)v * N);
-  }
+  for (int v = 0; v < num_vectors; ++v)
+    zz_moments(run, G, xin.ptr + (size_t)v * words, partials, d_gram, C.data() + (size_t)v * N * N,
+               m.data() + (size_t)v * N);
   CUDA_CHECK(cudaMemcpyAsync(correlations, C.data(), C.size() * sizeof(double), cudaMemcpyDefault, st));
   if (magnetization)
     CUDA_CHECK(cudaMemcpyAsync(magnetization, m.data(), m.size() * sizeof(double), cudaMemcpyDefault, st));
   CUDA_CHECK(cudaStreamSynchronize(st));
+  API_END
+}
+
+// ---- flip-flop correlations (DESIGN.md section 3, "dmv_pm_correlations"): per vector one k_zz_gram pass (W and the
+// magnetisation for the diagonal), one walk over this rank's rows and their antiparallel pairs (k_pm_rows with
+// permutations, k_pm_pairs without) into one sum per class of site pairs, all-reduced over the ranks, finished on the
+// host.  On several ranks the targets are looked up in the whole basis of the replicated-x form, against the gathered x.
+int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm) {
+  API_BEGIN
+  SolverRun run(ctx, elt, "dmv_pm_correlations", false);
+  if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
+  if (!x) throw std::runtime_error("x must not be null");
+  if (!pm) throw std::runtime_error("pm must not be null");
+  const int N = ctx->n_sites, P = run.P;
+  const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
+                             ctx->spin_inversion);
+  const PmClasses K = pm_classes(N, G);
+  const int count = (int)K.size.size();
+  cudaStream_t st = run.st;
+  dmv_context *basis = ctx;   // where the targets are looked up
+  if (P > 1) {
+    if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
+    if (!ctx->replicated)
+      throw std::runtime_error("dmv_pm_correlations on several ranks needs the whole basis on every rank (the "
+                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
+                               "fit in device memory");
+    basis = ctx->global;
+  }
+  const bool trivial = ctx->proj != PROJ_GROUP || ctx->orbit.trivial_characters;
+  const int look = ctx->proj == PROJ_NONE        ? PM_NONE
+                   : ctx->proj == PROJ_INVERSION ? PM_INVERSION
+                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
+                                                                     : PM_GROUP;
+  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
+                                                            basis->opt.rows_ctas) : 0;
+  const bool cplx = run.ce || !trivial;
+  std::vector<int16_t> class_of(K.of.begin(), K.of.end());
+  std::vector<uint16_t> pairs;
+  for (int i = 0; i < N; ++i)
+    for (int j = i + 1; j < N; ++j) pairs.push_back((uint16_t)(i | j << 8));
+  DevBuf<int16_t> d_class_of;
+  DevBuf<uint16_t> d_pairs;
+  d_class_of.upload(class_of, st);
+  d_pairs.upload(pairs, st);
+  PmArgs A{};
+  A.index = base_params(basis).index;
+  A.orbit = basis->orbit;
+  A.norms = basis->d_norms.ptr;
+  A.pos = P > 1 ? ctx->d_pos.ptr : nullptr;
+  A.rows = ctx->d_reps.ptr;
+  A.row_norms = ctx->d_norms.ptr;
+  A.n_rows = run.n;
+  A.x_row_offset = P > 1 ? (int64_t)ctx->rank * ctx->repl_block : 0;
+  A.site_mask = ctx->site_mask;
+  A.inversion_character = (double)ctx->spin_inversion;
+  A.class_of = d_class_of.ptr;
+  A.pairs = d_pairs.ptr;
+  A.n_sites = N;
+  A.n_pairs = (int)pairs.size();
+  A.status = ctx->d_status.ptr;
+  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
+    cudaStream_t keep = basis->stream;
+    basis->stream = st;
+    ensure_table(basis, elt);
+    basis->stream = keep;
+    A.table = basis->d_table.ptr;
+    A.table_slots = basis->table_slots;
+    A.table_dir = basis->table_dir;
+  }
+  const size_t gram_size = zz_gram_size(N);
+  double *d_gram = run.scalars(gram_size + 2 * (size_t)count), *d_sums = d_gram + gram_size;
+  const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
+  std::vector<double> out((size_t)num_vectors * N * N * 2), C((size_t)N * N), m((size_t)N), sums(2 * (size_t)count);
+  for (int v = 0; v < num_vectors; ++v) {
+    const double *xv = xin.ptr + (size_t)v * run.words;
+    const double W = zz_moments(run, G, xv, run.partials(zz_gram_partials(run.n, N)), d_gram, C.data(), m.data());
+    A.x = P > 1 ? gather_x(ctx, elt, xv) : xv;
+    if (look == PM_TABLE)
+      launch_table_fill(basis->n_states, run.ce, A.x, basis->d_norms.ptr, A.pos, basis->d_slot_of.ptr,
+                        basis->d_reps.ptr, basis->d_table.ptr, nullptr, st);
+    pm_sums(run, A, count, look, tk, cplx, d_sums);
+    run.all_reduce(d_sums, 2 * (size_t)count);
+    CUDA_CHECK(cudaMemcpyAsync(sums.data(), d_sums, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+    check_status(ctx);   // synchronises
+    pm_finish(N, K, sums.data(), W, m.data(), out.data() + (size_t)v * N * N * 2);
+  }
+  CUDA_CHECK(cudaMemcpyAsync(pm, out.data(), out.size() * sizeof(double), cudaMemcpyDefault, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  API_END
+}
+
+// host-only self-check entry for the host half of dmv_pm_correlations (no device needed)
+int dmv_debug_pm_classes(const dmv_basis_desc *basis, int32_t *class_of, int32_t *class_size, int32_t *num_classes,
+                         const double *sums, double W, const double *magnetization, double *pm) {
+  API_BEGIN
+  if (!basis || !class_of || !class_size || !num_classes)
+    throw std::runtime_error("basis, class_of, class_size and num_classes must not be null");
+  const int N = basis->number_sites;
+  if (N < 1 || N > 64) throw std::runtime_error("number_sites must be between 1 and 64");
+  const ZzGroup G = zz_group(N, basis->has_permutations != 0, basis->group_order, basis->perms, basis->flips,
+                             basis->spin_inversion);
+  const PmClasses K = pm_classes(N, G);
+  std::copy(K.of.begin(), K.of.end(), class_of);
+  std::copy(K.size.begin(), K.size.end(), class_size);
+  *num_classes = (int32_t)K.size.size();
+  if (sums) {
+    if (!magnetization || !pm) throw std::runtime_error("the finish needs magnetization and pm");
+    pm_finish(N, K, sums, W, magnetization, pm);
+  }
   API_END
 }
 

@@ -1,5 +1,5 @@
 // dmv_solve.h -- the host frame of the device solvers (dmv_lanczos, dmv_expm_multiply, dmv_eigsh, dmv_zz_correlations,
-// dmv_lanczos_quadrature): entry checks, reductions over the ranks, products and work space.  The rules every rank must
+// dmv_pm_correlations, dmv_lanczos_quadrature): entry checks, reductions over the ranks, products and work space.  The rules every rank must
 // follow live here once: decisions come from all-reduced scalars, a work space is never shrunk silently to what fits,
 // and a product's output is cleared first only when the operator has no diagonal (include/dmv_b200.h, dmv_local_matvec:
 // y = D x + O x with diagonal terms, else y += O x).

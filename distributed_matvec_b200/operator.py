@@ -373,6 +373,33 @@ class Operator:
         nat.check(nat.lib().dmv_zz_correlations(self._ctx, elt, k, _ptr(x), C_out.ctypes.data, m_out.ctypes.data))
         return (C_out[0], m_out[0]) if x.ndim == 1 else (C_out, m_out)
 
+    def pm_correlations(self, x):
+        """Flip-flop correlations T[i, j] = <x|σ⁺ᵢσ⁻ⱼ|x> / <x|x> on the device (dmv_pm_correlations), with σ⁺ turning a
+        0 bit into a 1 bit.  x as for zz_correlations.  -> numpy complex128 of shape (N, N), or (k, N, N) for a batch."""
+        elt = _elt_of(x)
+        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        if _is_torch(x):
+            self.use_torch_stream()
+        else:
+            x = np.ascontiguousarray(x)
+        out = np.zeros((k, N, N), dtype=np.complex128)
+        nat.check(nat.lib().dmv_pm_correlations(self._ctx, elt, k, _ptr(x), out.ctypes.data))
+        return out[0] if x.ndim == 1 else out
+
+    def spin_correlations(self, x):
+        """<σᵢ·σⱼ> = <σᶻᵢσᶻⱼ> + 4 Re <σ⁺ᵢσ⁻ⱼ> (3 on the diagonal) and the total spin <S²> = ¼ Σᵢⱼ <σᵢ·σⱼ>, from
+        zz_correlations and pm_correlations.  -> numpy (S [N, N], S2 float), or (S [k, N, N], S2 [k]) for a batch."""
+        Cz, _ = self.zz_correlations(x)
+        T = self.pm_correlations(x)
+        S = Cz + 4.0 * T.real
+        N = S.shape[-1]
+        S[..., np.arange(N), np.arange(N)] = 3.0
+        S2 = 0.25 * S.sum(axis=(-2, -1))
+        return (S, float(S2)) if S.ndim == 2 else (S, S2)
+
     def lanczos_quadrature(self, num_vectors: int, steps: int, seed: int = 42, start=None,
                            complex_vectors: bool = False):
         """Finite-temperature Lanczos (stochastic Lanczos quadrature) on the device (dmv_lanczos_quadrature): for each

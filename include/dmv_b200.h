@@ -288,6 +288,23 @@ int dmv_eigsh(dmv_context *ctx, int elt, int nev, int block_size, int krylov_dim
 int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
                         double *magnetization);
 
+/* ---- flip-flop correlations on the device (row f7; not in the reference): T_ij = <x|σ⁺ᵢσ⁻ⱼ|x> / <x|x> for num_vectors
+ * vectors (the layout, the basis and the meaning of x are those of dmv_zz_correlations), host or device x.  σ⁺ turns a
+ * 0 bit into a 1 bit (the convention of the operator expressions).  pm: num_vectors * N * N complex numbers (vector, i,
+ * j), interleaved (re, im), 2 num_vectors N^2 doubles, host or device.  T is Hermitian; T_ii = (1 + m_i) / 2 with m
+ * from dmv_zz_correlations.  For every basis, with or without a fixed Hamming weight, and i != j:
+ *     <σˣᵢσˣⱼ + σʸᵢσʸⱼ> = 2 (T_ij + T_ji) = 4 Re T_ij,    <σᵢ·σⱼ> = C_ij + 4 Re T_ij   (C: dmv_zz_correlations),
+ * and Im T_ij is the spin current of the bond (up to the sign convention of the current).
+ * Method: x lies in a one-dimensional irrep of the group G of the basis, so σ⁺ᵢσ⁻ⱼ may be replaced by its G-average,
+ * which the row formula of the product evaluates.  One walk over this rank's rows and their antiparallel pairs sums
+ * conj(x_b) / n_b chi (n x)[rep(r_b ^ (1 << i | 1 << j))] over the rows with bit i set and bit j clear into one sum per
+ * class (orbit under G) of ordered pairs; T_ij = S_c / (<x|x> |c|).  An element with a spin flip maps (i, j) to
+ * (p(j), p(i)).  elt = DMV_F64 or DMV_C128, also with complex characters.  Fails for a zero vector.  Collective when
+ * num_ranks > 1 (needs dmv_comm_init and the whole basis on every rank, as the replicated-x product); every rank
+ * returns the same matrices.  Every reduction has a fixed order and there are no floating-point atomics: a repeated
+ * call is bit-identical. */
+int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm);
+
 /* ---- finite-temperature Lanczos on the device (row f6; not in the reference): the random-vector quadrature of the
  * finite-temperature Lanczos method (Jaklič & Prelovšek 1994), also called stochastic Lanczos quadrature.  For each of
  * num_vectors start vectors r, `steps` steps of the three-term recurrence (no reorthogonalisation, no stored basis) give
@@ -397,6 +414,12 @@ int dmv_debug_tridiagonal_quadrature(int k, const double *a, const double *b, do
  *   `basis`: its permutations and flips, {1, flip} for spin inversion alone, {1} without symmetries. */
 int dmv_debug_zz_symmetrize(const dmv_basis_desc *basis, const double *gram, double *correlations,
                             double *magnetization);
+/* dmv_debug_pm_classes: host half of dmv_pm_correlations.  class_of (N * N): class of the ordered pair (i, j), -1 on the
+ *   diagonal, classes numbered in the row-major order of their first pair; class_size (room for N * N): pairs per class;
+ *   *num_classes.  With sums (2 per class, interleaved), W = <x|x> > 0 and magnetization (N): pm (2 N^2 doubles) as
+ *   dmv_pm_correlations finishes it.  The group is that of dmv_debug_zz_symmetrize. */
+int dmv_debug_pm_classes(const dmv_basis_desc *basis, int32_t *class_of, int32_t *class_size, int32_t *num_classes,
+                         const double *sums, double W, const double *magnetization, double *pm);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
