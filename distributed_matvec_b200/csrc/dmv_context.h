@@ -28,13 +28,6 @@ namespace dmv { namespace host {
 
 extern thread_local std::string g_last_error;   // defined in dmv_api.cu
 
-#define CUDA_CHECK(expr)                                                                        \
-  do {                                                                                          \
-    cudaError_t _e = (expr);                                                                    \
-    if (_e != cudaSuccess)                                                                      \
-      throw std::runtime_error(std::string(#expr) + ": " + cudaGetErrorString(_e));            \
-  } while (0)
-
 #define API_BEGIN try {
 #define API_END                                         \
   return 0;                                             \

@@ -24,8 +24,6 @@
 
 namespace dmv {
 
-void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -366,65 +364,6 @@ __global__ void k_owner_positions(const uint64_t *__restrict__ states, const uin
     }
 }
 
-int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
-template <bool INV, bool CV, bool CE, bool NARROW, bool LIN, bool UNI, int KB>
-void launch_t(const KernelParams &p, cudaStream_t stream) {
-  using V = typename Val<CV>::type;
-  const GatherLayout L = gather_layout(p, NARROW ? 4 : 8, sizeof(V), UNI);
-  auto kernel = k_gather<INV, CV, CE, NARROW, LIN, UNI, KB>;
-  if (L.total > 48 * 1024) {
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total) != cudaSuccess)
-      throw std::runtime_error("k_gather: operator tables do not fit in shared memory");
-  }
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, L.total) != cudaSuccess || per_sm < 1)
-    per_sm = 1;
-  const int rpt = 32 / (p.row_split > 1 ? p.row_split : 1);
-  const int64_t tiles = (p.row_end - p.row_begin + rpt - 1) / rpt;
-  int64_t blocks = (tiles + kThreads / 32 - 1) / (kThreads / 32);
-  const int64_t resident = (int64_t)sm_count() * per_sm;
-  if (blocks > resident) blocks = resident;   // whole waves of resident CTAs, grid-stride over the tiles
-  if (blocks < 1) blocks = 1;
-  kernel<<<(unsigned)blocks, kThreads, L.total, stream>>>(p);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_gather launch: ") + cudaGetErrorString(e));
-  count_launch();
-}
-
-template <bool INV, bool CV, bool CE, bool NARROW, bool LIN, bool UNI>
-void launch_k(const KernelParams &p, cudaStream_t s) {
-  if (p.batch == 4) launch_t<INV, CV, CE, NARROW, LIN, UNI, 4>(p, s);
-  else if (p.batch <= 1) launch_t<INV, CV, CE, NARROW, LIN, UNI, 1>(p, s);
-  else throw std::runtime_error("k_gather: vectors come one or four at a time");
-}
-template <bool INV, bool CV, bool CE, bool NARROW>
-void launch_n(const KernelParams &p, bool lin, bool uni, cudaStream_t s) {
-  if (lin) { if (uni) launch_k<INV, CV, CE, NARROW, true, true>(p, s); else launch_k<INV, CV, CE, NARROW, true, false>(p, s); }
-  else { if (uni) launch_k<INV, CV, CE, NARROW, false, true>(p, s); else launch_k<INV, CV, CE, NARROW, false, false>(p, s); }
-}
-template <bool INV, bool CV, bool CE>
-void launch_w(const KernelParams &p, bool narrow, bool lin, bool uni, cudaStream_t s) {
-  if (narrow) launch_n<INV, CV, CE, true>(p, lin, uni, s);
-  else launch_n<INV, CV, CE, false>(p, lin, uni, s);
-}
-template <bool INV>
-void launch_v(const KernelParams &p, bool cv, bool ce, bool narrow, bool lin, bool uni, cudaStream_t s) {
-  if (!cv && !ce) launch_w<INV, false, false>(p, narrow, lin, uni, s);
-  else if (!cv && ce) launch_w<INV, false, true>(p, narrow, lin, uni, s);
-  else if (cv && ce) launch_w<INV, true, true>(p, narrow, lin, uni, s);
-  else launch_w<INV, true, false>(p, narrow, lin, uni, s);
-}
-
 // out[pos[i]] = in[i] (scatter) or out[i] = in[pos[i]] (gather) for 8- or 16-byte elements
 template <typename T, bool GATHER>
 __global__ void k_permute(int64_t n, const uint32_t *__restrict__ pos, const T *__restrict__ in, T *__restrict__ out) {
@@ -439,17 +378,14 @@ __global__ void k_permute(int64_t n, const uint32_t *__restrict__ pos, const T *
 
 void launch_permute(int64_t n, int elt, const uint32_t *pos, const void *in, void *out, bool gather, cudaStream_t stream) {
   if (n <= 0) return;
-  const unsigned blocks = (unsigned)std::min<int64_t>((n + 255) / 256, (int64_t)sm_count() * 16);
-  if (elt == 1) {
-    if (gather) k_permute<double, true><<<blocks, 256, 0, stream>>>(n, pos, (const double *)in, (double *)out);
-    else k_permute<double, false><<<blocks, 256, 0, stream>>>(n, pos, (const double *)in, (double *)out);
-  } else {
-    if (gather) k_permute<double2, true><<<blocks, 256, 0, stream>>>(n, pos, (const double2 *)in, (double2 *)out);
-    else k_permute<double2, false><<<blocks, 256, 0, stream>>>(n, pos, (const double2 *)in, (double2 *)out);
-  }
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_permute launch: ") + cudaGetErrorString(e));
-  count_launch();
+  const int blocks = capped_grid((n + 255) / 256, (int64_t)sm_count() * 16);
+  with_bool(elt != 1, [&](auto wide) {
+    using T = std::conditional_t<wide(), double2, double>;
+    with_bool(gather, [&](auto g) {
+      k_permute<T, g()><<<blocks, 256, 0, stream>>>(n, pos, (const T *)in, (T *)out);
+    });
+  });
+  check_launch("k_permute");
 }
 
 void launch_owner_positions(const uint64_t *states, const uint8_t *masks, int64_t n, int num_ranks, int64_t chunk,
@@ -459,11 +395,11 @@ void launch_owner_positions(const uint64_t *states, const uint8_t *masks, int64_
   if (num_ranks > 32) throw std::runtime_error("replicated-x product supports at most 32 ranks");
   const int64_t n_chunks = (n + chunk - 1) / chunk;
   const unsigned blocks = (unsigned)((n_chunks + 127) / 128);
-  if (write_pass) k_owner_positions<true><<<blocks, 128, 0, stream>>>(states, masks, n, num_ranks, chunk, chunk_counts, chunk_base, block, pos);
-  else k_owner_positions<false><<<blocks, 128, 0, stream>>>(states, masks, n, num_ranks, chunk, chunk_counts, chunk_base, block, pos);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_owner_positions launch: ") + cudaGetErrorString(e));
-  count_launch();
+  with_bool(write_pass, [&](auto write) {
+    k_owner_positions<write()><<<blocks, 128, 0, stream>>>(states, masks, n, num_ranks, chunk, chunk_counts, chunk_base,
+                                                           block, pos);
+  });
+  check_launch("k_owner_positions");
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -526,37 +462,27 @@ __global__ void k_raise_flags(unsigned *const *__restrict__ peer_flags, int num_
 
 void launch_raise_flags(unsigned *const *peer_flags, int num_ranks, int rank, unsigned value, cudaStream_t stream) {
   k_raise_flags<<<1, 32, 0, stream>>>(peer_flags, num_ranks, rank, value);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_raise_flags launch: ") + cudaGetErrorString(e));
-  count_launch();
+  check_launch("k_raise_flags");
 }
 
 void launch_push_block(const void *x, int64_t n_doubles, int num_ranks, void *const *peer_slot, unsigned *done,
                        unsigned *const *peer_flags, int rank, unsigned epoch, bool wide, cudaStream_t stream) {
   // wide: 16-byte words (x and every slot 16-byte aligned, even number of doubles)
   const int64_t words = wide ? n_doubles / 2 : n_doubles;
-  int64_t blocks = (words + 4 * 256 - 1) / (4 * 256);   // a few words per thread: fewer CTAs to fence and count
-  if (blocks > (int64_t)sm_count() * 4) blocks = (int64_t)sm_count() * 4;
-  if (blocks < 1) blocks = 1;
-  if (wide)
-    k_push_block<double2><<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const double2 *>(x), words, num_ranks,
-                                                               reinterpret_cast<double2 *const *>(peer_slot), done,
-                                                               peer_flags, rank, epoch);
-  else
-    k_push_block<double><<<(unsigned)blocks, 256, 0, stream>>>(reinterpret_cast<const double *>(x), words, num_ranks,
-                                                             reinterpret_cast<double *const *>(peer_slot), done,
-                                                             peer_flags, rank, epoch);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_push_block launch: ") + cudaGetErrorString(e));
-  count_launch();
+  // a few words per thread: fewer CTAs to fence and count
+  const int blocks = capped_grid((words + 4 * 256 - 1) / (4 * 256), (int64_t)sm_count() * 4);
+  with_bool(wide, [&](auto w) {
+    using T = std::conditional_t<w(), double2, double>;
+    k_push_block<T><<<blocks, 256, 0, stream>>>(reinterpret_cast<const T *>(x), words, num_ranks,
+                                                reinterpret_cast<T *const *>(peer_slot), done, peer_flags, rank, epoch);
+  });
+  check_launch("k_push_block");
 }
 
 void launch_wait_flags(const unsigned *flags, int num_ranks, unsigned epoch, unsigned long long *status,
                        cudaStream_t stream) {
   k_wait_flags<<<1, 32, 0, stream>>>(flags, num_ranks, epoch, status);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string("k_wait_flags launch: ") + cudaGetErrorString(e));
-  count_launch();
+  check_launch("k_wait_flags");
 }
 
 // p.groups / p.lut / p.bp must point at the ROW-traversal tables (see k_pull); complex_values says whether the
@@ -564,8 +490,23 @@ void launch_wait_flags(const unsigned *flags, int num_ranks, unsigned epoch, uns
 void launch_gather(const KernelParams &p, bool inversion, bool complex_values, bool complex_elements,
                    bool narrow, bool lin, bool uniform, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  if (inversion) launch_v<true>(p, complex_values, complex_elements, narrow, lin, uniform, stream);
-  else launch_v<false>(p, complex_values, complex_elements, narrow, lin, uniform, stream);
+  if (p.batch > 1 && p.batch != 4) throw std::runtime_error("k_gather: vectors come one or four at a time");
+  const int rpt = 32 / (p.row_split > 1 ? p.row_split : 1);
+  const int64_t tiles = (p.row_end - p.row_begin + rpt - 1) / rpt;
+  with_bool(inversion, [&](auto inv) {
+  with_bool(complex_values, [&](auto cv) {
+  with_bool(complex_elements, [&](auto ce) {
+  with_bool(narrow, [&](auto nw) {
+  with_bool(lin, [&](auto ln) {
+  with_bool(uniform, [&](auto uni) {
+  with_choice<1, 4>(p.batch == 4 ? 4 : 1, [&](auto kb) {
+    auto kernel = k_gather<inv(), cv(), ce(), nw(), ln(), uni(), kb()>;
+    const size_t smem = gather_layout(p, nw() ? 4 : 8, sizeof(typename Val<cv()>::type), uni()).total;
+    // whole waves of resident CTAs, grid-stride over the tiles
+    const int grid = one_wave(kernel, (tiles + kThreads / 32 - 1) / (kThreads / 32), smem);
+    kernel<<<grid, kThreads, smem, stream>>>(p);
+    check_launch("k_gather");
+  }); }); }); }); }); }); });
 }
 
 }  // namespace dmv

@@ -3,7 +3,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+#include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "dmv_device.cuh"
@@ -123,7 +126,6 @@ struct KernelParams {
 };
 
 // launchers (dmv_kernels.cu)
-struct LaunchConfig { int blocks; int threads; size_t smem; };
 void launch_generate(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements,
                      bool count_only, cudaStream_t stream);
 void launch_pull(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements,
@@ -258,5 +260,55 @@ int64_t launch_counter();
 int planned_grid(int64_t rows, int row_split);
 int choose_row_split(int64_t rows, int n_groups);
 constexpr int kWarpsPerCta = 8;
+
+// ---- launch helpers of every launcher (dmv_kernels.cu defines sm_count and check_launch) ----------------------------
+#define CUDA_CHECK(expr)                                                                        \
+  do {                                                                                          \
+    cudaError_t _e = (expr);                                                                    \
+    if (_e != cudaSuccess)                                                                      \
+      throw std::runtime_error(std::string(#expr) + ": " + cudaGetErrorString(_e));            \
+  } while (0)
+
+// streaming multiprocessors of the current device (queried once per device ordinal)
+int sm_count();
+// after every launch: a launch error names the kernel, and the launch is counted once (launch_counter)
+void check_launch(const char *what);
+
+// `work_ctas` CTAs' worth of work, at least one (so that an empty launch still writes its partials), at most max_ctas
+inline int capped_grid(int64_t work_ctas, int64_t max_ctas) {
+  return (int)std::min<int64_t>(std::max<int64_t>(work_ctas, 1), max_ctas);
+}
+
+// let `kernel` have `smem` bytes of dynamic shared memory: launches above 48 KB need the opt-in
+template <typename K>
+void opt_in_smem(K kernel, size_t smem) {
+  if (smem > 48 * 1024)
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+      throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
+}
+
+// one wave of resident CTAs of `kernel` (`threads` each, `smem` bytes of dynamic shared memory) over `ctas` CTAs' worth
+// of work
+template <typename K>
+int one_wave(K kernel, int64_t ctas, size_t smem = 0, int threads = 32 * kWarpsPerCta) {
+  opt_in_smem(kernel, smem);
+  int per_sm = 0;
+  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+  return capped_grid(ctas, (int64_t)sm_count() * std::max(per_sm, 1));
+}
+
+// f(std::integral_constant<bool, B>) for the runtime flag b
+template <typename F>
+auto with_bool(bool b, F &&f) {
+  return b ? f(std::true_type{}) : f(std::false_type{});
+}
+
+// f(std::integral_constant<int, V>) for the V of the list equal to v; a value outside the list has no kernel instance
+template <int V, int... Rest, typename F>
+auto with_choice(int v, F &&f) {
+  if (v == V) return f(std::integral_constant<int, V>{});
+  if constexpr (sizeof...(Rest) > 0) return with_choice<Rest...>(v, f);
+  else throw std::runtime_error("no kernel instance for the value " + std::to_string(v));
+}
 
 }  // namespace dmv

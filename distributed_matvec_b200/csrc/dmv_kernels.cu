@@ -26,14 +26,28 @@ namespace dmv {
 
 static std::atomic<int64_t> g_launches{0};
 int64_t launch_counter() { return g_launches.load(); }
-void count_launch() { g_launches++; }
+static void count_launch() { g_launches++; }
 
-#define DMV_CUDA_CHECK(expr)                                                                    \
-  do {                                                                                          \
-    cudaError_t _e = (expr);                                                                    \
-    if (_e != cudaSuccess)                                                                      \
-      throw std::runtime_error(std::string(#expr) + ": " + cudaGetErrorString(_e));            \
-  } while (0)
+void check_launch(const char *what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
+  count_launch();
+}
+
+// each process or thread of a multi-GPU run asks for its own device, so the count is kept per device ordinal
+int sm_count() {
+  constexpr int kDevices = 64;
+  static std::atomic<int> cached[kDevices];
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const bool cacheable = dev >= 0 && dev < kDevices;
+  int n = cacheable ? cached[dev].load(std::memory_order_relaxed) : 0;
+  if (n > 0) return n;
+  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  if (n <= 0) n = 132;
+  if (cacheable) cached[dev].store(n, std::memory_order_relaxed);
+  return n;
+}
 
 namespace {
 
@@ -1547,182 +1561,64 @@ __global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed
   if (!WRITE) chunk_count[c] = n;
 }
 
-int grid_for(int64_t work_items, int per_block, int max_blocks) {
-  int64_t b = (work_items + per_block - 1) / per_block;
-  if (b < 1) b = 1;
-  if (b > max_blocks) b = max_blocks;
-  return (int)b;
+// f(PROJ, CV, CE) as integral constants for the value kinds k_generate, k_pull and k_accumulate are built for: real
+// values and vectors, complex values with real or complex vectors
+template <typename F>
+void with_values(Projection proj, bool complex_values, bool complex_elements, F &&f) {
+  if (complex_elements && !complex_values) throw std::runtime_error("complex vectors need complex values");
+  with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
+    with_bool(complex_values, [&](auto cv) {
+      with_bool(complex_elements, [&](auto ce) {
+        if constexpr (cv() || !ce()) f(pj, cv, ce);
+      });
+    });
+  });
 }
 
 }  // namespace
+
 // lanes per source state: enough warps to fill the machine (>= 8 per SM) on small bases, never more than the
 // number of flip-mask groups
 int choose_row_split(int64_t rows, int n_groups) {
-  int dev = 0, n = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  if (n <= 0) n = 132;
+  const int n = sm_count();
   int s = 1;
   while (s < 32 && 2 * s <= n_groups && (rows * s) / 32 < (int64_t)n * 16) s *= 2;
   return s;
 }
 
 int planned_grid(int64_t rows, int row_split) {   // grid of the planned launches: fixed, not occupancy-derived
-  int dev = 0, n = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-  if (n <= 0) n = 132;
   const int rows_per_tile = 32 / (row_split > 1 ? row_split : 1);
-  int64_t b = ((rows + rows_per_tile - 1) / rows_per_tile + kWarps - 1) / kWarps;
-  if (b < 1) b = 1;
-  if (b > (int64_t)n * 4) b = (int64_t)n * 4;
-  return (int)b;
-}
-namespace {
-
-int sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
+  return capped_grid(((rows + rows_per_tile - 1) / rows_per_tile + kWarps - 1) / kWarps, (int64_t)sm_count() * 4);
 }
 
-template <int PROJ, bool CV, bool CE, bool COUNT_ONLY>
-void launch_generate_t(const KernelParams &p, cudaStream_t stream) {
-  using V = typename ValT<CV>::type;
-  const SmemLayout L = smem_layout(p, PROJ, sizeof(V));
-  auto kernel = k_generate<PROJ, CV, CE, COUNT_ONLY>;
-  if (L.total > 48 * 1024)
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-  if (L.total > 40 * 1024)   // let several CTAs with large tables share the SM
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  int per_sm = 0;
-  DMV_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, L.total));
-  if (per_sm < 1) per_sm = 1;
-  const int rpt = 32 / (p.row_split > 1 ? p.row_split : 1);
-  const int64_t tiles = (p.row_end - p.row_begin + rpt - 1) / rpt;
-  // grid = a whole number of waves of resident CTAs (SMs x per_sm), or fewer when the work is small
-  const int blocks = p.grid_blocks > 0 ? p.grid_blocks : grid_for(tiles, kWarps, sm_count() * per_sm);
-  kernel<<<blocks, kThreads, L.total, stream>>>(p);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-
-template <int PROJ, bool CV, bool CE>
-void launch_generate_c(const KernelParams &p, bool count_only, cudaStream_t s) {
-  if (count_only) launch_generate_t<PROJ, CV, CE, true>(p, s);
-  else launch_generate_t<PROJ, CV, CE, false>(p, s);
-}
-template <int PROJ>
-void launch_generate_p(const KernelParams &p, bool cv, bool ce, bool count_only, cudaStream_t s) {
-  if (!cv && !ce) launch_generate_c<PROJ, false, false>(p, count_only, s);
-  else if (cv && ce) launch_generate_c<PROJ, true, true>(p, count_only, s);
-  else if (cv && !ce) launch_generate_c<PROJ, true, false>(p, count_only, s);
-  else throw std::runtime_error("complex vectors need complex values");
-}
-
-
-template <int PROJ, bool CV, bool CE>
-void launch_pull_t(const KernelParams &p, cudaStream_t stream) {
-  using V = typename ValT<CV>::type;
-  const SmemLayout L = smem_layout(p, PROJ, sizeof(V));
-  auto kernel = k_pull<PROJ, CV, CE>;
-  if (L.total > 48 * 1024)
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-  int per_sm = 0;
-  DMV_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, L.total));
-  if (per_sm < 1) per_sm = 1;
-  const int64_t tiles = (p.row_end - p.row_begin + 31) / 32;
-  const int blocks = grid_for(tiles, kWarps, sm_count() * per_sm);
-  kernel<<<blocks, kThreads, L.total, stream>>>(p);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-template <int PROJ>
-void launch_pull_p(const KernelParams &p, bool cv, bool ce, cudaStream_t s) {
-  if (!cv && !ce) launch_pull_t<PROJ, false, false>(p, s);
-  else if (cv && ce) launch_pull_t<PROJ, true, true>(p, s);
-  else if (cv && !ce) launch_pull_t<PROJ, true, false>(p, s);
-  else throw std::runtime_error("complex vectors need complex values");
-}
-
-template <int PROJ>
-void launch_accumulate_p(const KernelParams &p, bool cv, bool ce, int64_t count, const uint64_t *b,
-                         const double *c, cudaStream_t s) {
-  const int blocks = grid_for((count + 1) / 2, kThreads, sm_count() * 8);
-  if (!cv && !ce) k_accumulate<PROJ, false, false><<<blocks, kThreads, 0, s>>>(p, count, b, c);
-  else if (cv && ce) k_accumulate<PROJ, true, true><<<blocks, kThreads, 0, s>>>(p, count, b, c);
-  else if (cv && !ce) k_accumulate<PROJ, true, false><<<blocks, kThreads, 0, s>>>(p, count, b, c);
-  else throw std::runtime_error("complex vectors need complex values");
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-
-}  // namespace
-
-namespace {
-template <bool CE, int TK, bool MPH, int CTAS = 2, bool ORD = false>
-void launch_rows_t(const KernelParams &p, cudaStream_t stream) {
-  const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
-  const size_t smem_bytes = rows_smem(p, L, ORD, TK).total;
-  auto kernel = k_rows<CE, TK, MPH, CTAS, ORD>;
-  if (smem_bytes > 48 * 1024)
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-  int per_sm = 0;
-  DMV_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem_bytes));
-  if (per_sm < 1) per_sm = 1;
-  const int64_t tiles = (p.row_end - p.row_begin + 31) / 32;
-  const int blocks = grid_for(tiles, kWarps, sm_count() * per_sm);
-  kernel<<<blocks, kThreads, smem_bytes, stream>>>(p);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-template <bool CE>
-void launch_rows_e(const KernelParams &p, cudaStream_t stream) {
+// k_rows: two CTAs per SM by default (122 registers, nothing spills), three (80 registers, a few words of the pipeline
+// state spill) or four (64 registers) on request.  On an H100 (400 W, L2 flushed between products) three CTAs tie on the
+// 6x6 square (31.1 / 31.5 ms against 31.5 ms, complex128) and lose on chain_36_symm (79.4 ms against 71.3)
+void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream) {
+  if (p.row_end <= p.row_begin) return;
   const int k = rows_torus_k(p.orbit, p.dense != nullptr, p.rows_ctas);
-  if (p.dense != nullptr) {   // dense index (perfect hash)
-    if (k == 6) launch_rows_t<CE, 6, true>(p, stream);
-    else if (k == 4) launch_rows_t<CE, 4, true>(p, stream);
-    else launch_rows_t<CE, 0, true>(p, stream);
-    return;
-  }
-  if (p.table_dir.dir != nullptr) {   // ordered table layout
-    if (p.rows_ctas == 3) {
-      if (k == 6) launch_rows_t<CE, 6, false, 3, true>(p, stream);
-      else if (k == 4) launch_rows_t<CE, 4, false, 3, true>(p, stream);
-      else launch_rows_t<CE, 0, false, 3, true>(p, stream);
-    } else if (p.rows_ctas == 4) {
-      if (k == 6) launch_rows_t<CE, 6, false, 4, true>(p, stream);
-      else launch_rows_t<CE, 0, false, 4, true>(p, stream);
-    } else {
-      if (k == 6) launch_rows_t<CE, 6, false, 2, true>(p, stream);
-      else if (k == 4) launch_rows_t<CE, 4, false, 2, true>(p, stream);
-      else launch_rows_t<CE, 0, false, 2, true>(p, stream);
-    }
-    return;
-  }
-  if (p.rows_ctas == 3) {   // three CTAs per SM: 80 registers, a few words of the pipeline state spill
-    if (k == 6) launch_rows_t<CE, 6, false, 3>(p, stream);
-    else if (k == 4) launch_rows_t<CE, 4, false, 3>(p, stream);
-    else launch_rows_t<CE, 0, false, 3>(p, stream);
-    return;
-  }
-  if (p.rows_ctas == 4) {   // four CTAs per SM: 64 registers
-    if (k == 6) launch_rows_t<CE, 6, false, 4>(p, stream);
-    else launch_rows_t<CE, 0, false, 4>(p, stream);
-    return;
-  }
-  // default: two CTAs per SM (122 registers, nothing spills).  On an H100 (400 W, L2 flushed between products) three CTAs
-  // tie on the 6x6 square (31.1 / 31.5 ms against 31.5 ms, complex128) and lose on chain_36_symm (79.4 ms against 71.3)
-  if (k == 6) launch_rows_t<CE, 6, false>(p, stream);
-  else if (k == 4) launch_rows_t<CE, 4, false>(p, stream);
-  else launch_rows_t<CE, 0, false>(p, stream);
+  const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
+  auto launch = [&](auto kernel, bool ord, int tk) {
+    const size_t smem = rows_smem(p, L, ord, tk).total;
+    const int grid = one_wave(kernel, ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps, smem);
+    kernel<<<grid, kThreads, smem, stream>>>(p);
+    check_launch("k_rows");
+  };
+  with_bool(complex_elements, [&](auto ce) {
+    with_choice<6, 4, 0>(k, [&](auto tk) {
+      if (p.dense != nullptr) {   // the dense index (perfect hash) is built for two CTAs per SM and the hashed layout only
+        launch(k_rows<ce(), tk(), true, 2, false>, false, tk());
+        return;
+      }
+      with_choice<2, 3, 4>(p.rows_ctas, [&](auto ctas) {
+        with_bool(p.table_dir.dir != nullptr, [&](auto ord) {   // the ordered table layout
+          constexpr int TK = ctas() == 4 && tk() == 4 ? 0 : tk();   // no 4x4 build at 64 registers (see rows_torus_k)
+          launch(k_rows<ce(), TK, false, ctas(), ord()>, ord(), TK);
+        });
+      });
+    });
+  });
 }
-}  // namespace
 
 int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {
   const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
@@ -1732,25 +1628,6 @@ int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {
   return k;
 }
 
-namespace {
-template <int TK, int CTAS>
-void launch_rows_batch_t(const KernelParams &p, cudaStream_t stream) {
-  const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
-  const size_t smem_bytes = L.total;
-  auto kernel = k_rows_batch<TK, CTAS>;
-  if (smem_bytes > 48 * 1024)
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_bytes));
-  int per_sm = 0;
-  DMV_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, kThreads, smem_bytes));
-  if (per_sm < 1) per_sm = 1;
-  const int64_t tiles = (p.row_end - p.row_begin + 31) / 32;
-  const int blocks = grid_for(tiles, kWarps, sm_count() * per_sm);
-  kernel<<<blocks, kThreads, smem_bytes, stream>>>(p);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-}  // namespace
-
 // p.batch vectors of p.batch_elt doubles per element (p.batch * p.batch_elt <= 6), p.table = the 64-byte-bucket table
 void launch_rows_batch(const KernelParams &p, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
@@ -1758,27 +1635,24 @@ void launch_rows_batch(const KernelParams &p, cudaStream_t stream) {
     throw std::runtime_error("k_rows_batch: at most six doubles per state");
   const OrbitProgram &o = p.orbit;
   const int k = (o.canon_mode != 0 && o.tor_mode == 2 && o.canon_k == o.canon_r) ? o.canon_k : 0;
+  const size_t smem = smem_layout(p, PROJ_GROUP, sizeof(double), false).total;
   // two CTAs per SM (120-128 registers: the eight words of the request stay in registers; at 80 registers part of them
   // spills)
-  if (k == 6) launch_rows_batch_t<6, 2>(p, stream);
-  else if (k == 4) launch_rows_batch_t<4, 2>(p, stream);
-  else launch_rows_batch_t<0, 2>(p, stream);
+  with_choice<6, 4, 0>(k == 6 || k == 4 ? k : 0, [&](auto tk) {
+    auto kernel = k_rows_batch<tk(), 2>;
+    const int grid = one_wave(kernel, ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps, smem);
+    kernel<<<grid, kThreads, smem, stream>>>(p);
+    check_launch("k_rows_batch");
+  });
 }
 
 void launch_table_fill_batch(int64_t n, int num_vectors, int elt, const void *x, int64_t stride, const double *norms,
                              const uint32_t *slot_of, const uint64_t *reps, void *table, cudaStream_t stream) {
   if (n <= 0) return;
-  const int blocks = grid_for(n, 256, sm_count() * 16);
+  const int blocks = capped_grid((n + 255) / 256, (int64_t)sm_count() * 16);
   k_table_fill_batch<<<blocks, 256, 0, stream>>>(n, num_vectors * elt, elt, reinterpret_cast<const double *>(x), stride, norms,
                                                  slot_of, reps, reinterpret_cast<unsigned char *>(table));
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
-}
-
-void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream) {
-  if (p.row_end <= p.row_begin) return;
-  if (complex_elements) launch_rows_e<true>(p, stream);
-  else launch_rows_e<false>(p, stream);
+  check_launch("k_table_fill_batch");
 }
 
 void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t n_buckets, int slots_per_bucket,
@@ -1786,140 +1660,134 @@ void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t 
   if (n <= 0) return;
   k_table_insert<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(reps, n, reinterpret_cast<unsigned char *>(table),
                                                                  n_buckets, slots_per_bucket, slot_of, bucket_bytes, ord);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_table_insert");
 }
 
 void launch_ordered_dir(const uint64_t *reps, int64_t n, OrderedDir ord, uint32_t buckets_per_state, cudaStream_t stream) {
   const int64_t entries = (int64_t)ord.last + 2;
   k_ordered_dir<<<(unsigned)((entries + 255) / 256), 256, 0, stream>>>(reps, n, ord, buckets_per_state,
                                                                         const_cast<uint32_t *>(ord.dir));
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_ordered_dir");
 }
 
 void launch_table_fill(int64_t n, bool complex_elements, const void *x, const double *norms, const uint32_t *pos,
                        const uint32_t *slot_of, const uint64_t *reps, void *table, void *dense, cudaStream_t stream) {
   if (n <= 0) return;
-  const int blocks = grid_for(n, 256, sm_count() * 16);
+  const int blocks = capped_grid((n + 255) / 256, (int64_t)sm_count() * 16);
   unsigned char *t = reinterpret_cast<unsigned char *>(table), *d = reinterpret_cast<unsigned char *>(dense);
-  if (complex_elements) k_table_fill<true><<<blocks, 256, 0, stream>>>(n, x, norms, pos, slot_of, reps, t, d);
-  else k_table_fill<false><<<blocks, 256, 0, stream>>>(n, x, norms, pos, slot_of, reps, t, d);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  with_bool(complex_elements, [&](auto ce) {
+    k_table_fill<ce()><<<blocks, 256, 0, stream>>>(n, x, norms, pos, slot_of, reps, t, d);
+  });
+  check_launch("k_table_fill");
 }
 
 void launch_mph_mark(const uint64_t *keys, int64_t n, int level, uint32_t n_blocks, unsigned long long *seen,
                      unsigned long long *collide, cudaStream_t stream) {
   if (n <= 0) return;
   k_mph_mark<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(keys, n, level, n_blocks, seen, collide);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_mph_mark");
 }
 void launch_mph_compact(const uint64_t *keys, int64_t n, int level, uint32_t n_blocks, const unsigned long long *collide,
                         uint64_t *next, unsigned long long *next_count, cudaStream_t stream) {
   if (n <= 0) return;
   k_mph_compact<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(keys, n, level, n_blocks, collide, next, next_count);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_mph_compact");
 }
 void launch_mph_slots(const uint64_t *keys, int64_t n, PerfectHash mph, const void *table, uint32_t n_buckets,
                       int slots_per_bucket, uint32_t *slot_of, unsigned long long *status, cudaStream_t stream) {
   if (n <= 0) return;
   k_mph_slots<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(keys, n, mph, reinterpret_cast<const unsigned char *>(table),
                                                               n_buckets, slots_per_bucket, slot_of, status);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_mph_slots");
 }
 
-void launch_generate(const KernelParams &p, Projection proj, bool cv, bool ce, bool count_only,
+void launch_generate(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements, bool count_only,
                      cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  switch (proj) {
-    case PROJ_NONE: launch_generate_p<PROJ_NONE>(p, cv, ce, count_only, stream); break;
-    case PROJ_INVERSION: launch_generate_p<PROJ_INVERSION>(p, cv, ce, count_only, stream); break;
-    case PROJ_GROUP: launch_generate_p<PROJ_GROUP>(p, cv, ce, count_only, stream); break;
-  }
+  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
+    with_bool(count_only, [&](auto co) {
+      auto kernel = k_generate<pj(), cv(), ce(), co()>;
+      const SmemLayout L = smem_layout(p, pj(), sizeof(typename ValT<cv()>::type));
+      if (L.total > 40 * 1024)   // let several CTAs with large tables share the SM
+        CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      const int rpt = 32 / (p.row_split > 1 ? p.row_split : 1);
+      const int64_t tiles = (p.row_end - p.row_begin + rpt - 1) / rpt;
+      // grid = a whole number of waves of resident CTAs (SMs x per_sm), or fewer when the work is small
+      const int wave = one_wave(kernel, (tiles + kWarps - 1) / kWarps, L.total);
+      kernel<<<p.grid_blocks > 0 ? p.grid_blocks : wave, kThreads, L.total, stream>>>(p);
+      check_launch("k_generate");
+    });
+  });
 }
 
-void launch_pull(const KernelParams &p, Projection proj, bool cv, bool ce, cudaStream_t stream) {
+void launch_pull(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  switch (proj) {
-    case PROJ_NONE: launch_pull_p<PROJ_NONE>(p, cv, ce, stream); break;
-    case PROJ_INVERSION: launch_pull_p<PROJ_INVERSION>(p, cv, ce, stream); break;
-    case PROJ_GROUP: launch_pull_p<PROJ_GROUP>(p, cv, ce, stream); break;
-  }
+  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
+    auto kernel = k_pull<pj(), cv(), ce()>;
+    const SmemLayout L = smem_layout(p, pj(), sizeof(typename ValT<cv()>::type));
+    const int grid = one_wave(kernel, ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps, L.total);
+    kernel<<<grid, kThreads, L.total, stream>>>(p);
+    check_launch("k_pull");
+  });
 }
 
-void launch_accumulate(const KernelParams &p, Projection proj, bool cv, bool ce, int64_t count,
+void launch_accumulate(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements, int64_t count,
                        const uint64_t *betas, const double *coeffs, cudaStream_t stream) {
   if (count <= 0) return;
-  switch (proj) {
-    case PROJ_NONE: launch_accumulate_p<PROJ_NONE>(p, cv, ce, count, betas, coeffs, stream); break;
-    case PROJ_INVERSION: launch_accumulate_p<PROJ_INVERSION>(p, cv, ce, count, betas, coeffs, stream); break;
-    case PROJ_GROUP: launch_accumulate_p<PROJ_GROUP>(p, cv, ce, count, betas, coeffs, stream); break;
-  }
+  const int blocks = capped_grid(((count + 1) / 2 + kThreads - 1) / kThreads, (int64_t)sm_count() * 8);
+  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
+    k_accumulate<pj(), cv(), ce()><<<blocks, kThreads, 0, stream>>>(p, count, betas, coeffs);
+    check_launch("k_accumulate");
+  });
 }
 
 void launch_apply_diag(const KernelParams &p, int64_t count, const uint64_t *alphas, double *coeffs,
                        cudaStream_t stream) {
   if (count <= 0) return;
   const SmemLayout L = smem_layout(p, PROJ_NONE, sizeof(double2));
-  if (L.total > 48 * 1024)
-    DMV_CUDA_CHECK(cudaFuncSetAttribute(k_apply_diag, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-  k_apply_diag<<<grid_for(count, kThreads, sm_count() * 4), kThreads, L.total, stream>>>(p, count, alphas, coeffs);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  opt_in_smem(k_apply_diag, L.total);
+  const int blocks = capped_grid((count + kThreads - 1) / kThreads, (int64_t)sm_count() * 4);
+  k_apply_diag<<<blocks, kThreads, L.total, stream>>>(p, count, alphas, coeffs);
+  check_launch("k_apply_diag");
 }
 
 void launch_apply_off_diag(const KernelParams &p, int64_t count, const uint64_t *alphas, const int64_t *offsets,
                            int64_t *counts, uint64_t *betas, double *coeffs, bool write_pass, cudaStream_t stream) {
   if (count <= 0) return;
   const SmemLayout L = smem_layout(p, PROJ_NONE, sizeof(double2));
-  const int blocks = grid_for(count, kThreads, sm_count() * 4);
-  if (write_pass) {
-    if (L.total > 48 * 1024)
-      DMV_CUDA_CHECK(cudaFuncSetAttribute(k_apply_off_diag<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-    k_apply_off_diag<true><<<blocks, kThreads, L.total, stream>>>(p, count, alphas, offsets, counts, betas,
-                                                                   reinterpret_cast<double2 *>(coeffs));
-  } else {
-    if (L.total > 48 * 1024)
-      DMV_CUDA_CHECK(cudaFuncSetAttribute(k_apply_off_diag<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L.total));
-    k_apply_off_diag<false><<<blocks, kThreads, L.total, stream>>>(p, count, alphas, offsets, counts, betas,
-                                                                    reinterpret_cast<double2 *>(coeffs));
-  }
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  const int blocks = capped_grid((count + kThreads - 1) / kThreads, (int64_t)sm_count() * 4);
+  with_bool(write_pass, [&](auto write) {
+    opt_in_smem(k_apply_off_diag<write()>, L.total);
+    k_apply_off_diag<write()><<<blocks, kThreads, L.total, stream>>>(p, count, alphas, offsets, counts, betas,
+                                                                      reinterpret_cast<double2 *>(coeffs));
+  });
+  check_launch("k_apply_off_diag");
 }
 
 void launch_build_directory(const uint64_t *reps, int64_t n, uint32_t *dir, uint64_t n_buckets, int shift,
                             cudaStream_t stream) {
   const int64_t items = 2 * (int64_t)n_buckets;
   k_build_directory<<<(unsigned)((items + 255) / 256), 256, 0, stream>>>(reps, n, dir, n_buckets, shift);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_build_directory");
 }
 
 void launch_state_index(const StateIndex &ix, int64_t count, const uint64_t *spins, int64_t *indices,
                         cudaStream_t stream) {
   if (count <= 0) return;
   k_state_index<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(ix, count, spins, indices);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_state_index");
 }
 
 void launch_verify_rank(const StateIndex &ix, unsigned long long *status, cudaStream_t stream) {
   if (ix.n <= 0) return;
   k_verify_rank<<<(unsigned)((ix.n + 255) / 256), 256, 0, stream>>>(ix, status);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_verify_rank");
 }
 
 void launch_locale_idx(int64_t count, const uint64_t *states, int num_ranks, uint8_t *keys, cudaStream_t stream) {
   if (count <= 0) return;
   k_locale_idx<<<(unsigned)((count + 255) / 256), 256, 0, stream>>>(count, states, num_ranks, keys);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_locale_idx");
 }
 
 void launch_state_info(const OrbitProgram &P, Projection proj, uint64_t site_mask, double inv_char,
@@ -1928,21 +1796,17 @@ void launch_state_info(const OrbitProgram &P, Projection proj, uint64_t site_mas
   if (count <= 0) return;
   const unsigned blocks = (unsigned)((count + 127) / 128);
   double2 *ch = reinterpret_cast<double2 *>(characters);
-  switch (proj) {
-    case PROJ_NONE: k_state_info<PROJ_NONE><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms); break;
-    case PROJ_INVERSION: k_state_info<PROJ_INVERSION><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms); break;
-    case PROJ_GROUP: k_state_info<PROJ_GROUP><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms); break;
-  }
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
+    k_state_info<pj()><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms);
+  });
+  check_launch("k_state_info");
 }
 
 void launch_compute_norms(const OrbitProgram &P, int64_t count, const uint64_t *reps, double *norms,
                           cudaStream_t stream) {
   if (count <= 0) return;
   k_compute_norms<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(P, count, reps, norms);
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  check_launch("k_compute_norms");
 }
 
 void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask, bool fixed_hamming,
@@ -1952,23 +1816,14 @@ void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask
                       bool write_pass, cudaStream_t stream) {
   if (n_chunks <= 0) return;
   const unsigned blocks = (unsigned)((n_chunks + 127) / 128);
-#define DMV_ENUM(PR)                                                                                      \
-  if (write_pass)                                                                                         \
-    k_enumerate<PR, true><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, rank, num_ranks,       \
-                                                      n_chunks, chunk_first, chunk_last, chunk_count,     \
-                                                      chunk_offset, out, out_norms);                      \
-  else                                                                                                    \
-    k_enumerate<PR, false><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, rank, num_ranks,      \
-                                                       n_chunks, chunk_first, chunk_last, chunk_count,    \
-                                                       chunk_offset, out, out_norms)
-  switch (proj) {
-    case PROJ_NONE: DMV_ENUM(PROJ_NONE); break;
-    case PROJ_INVERSION: DMV_ENUM(PROJ_INVERSION); break;
-    case PROJ_GROUP: DMV_ENUM(PROJ_GROUP); break;
-  }
-#undef DMV_ENUM
-  DMV_CUDA_CHECK(cudaGetLastError());
-  g_launches++;
+  with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
+    with_bool(write_pass, [&](auto write) {
+      k_enumerate<pj(), write()><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, rank, num_ranks, n_chunks,
+                                                             chunk_first, chunk_last, chunk_count, chunk_offset, out,
+                                                             out_norms);
+    });
+  });
+  check_launch("k_enumerate");
 }
 
 }  // namespace dmv

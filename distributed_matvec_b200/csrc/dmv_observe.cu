@@ -15,9 +15,6 @@
 
 namespace dmv {
 
-int sm_count();                       // dmv_solver.cu
-void check_launch(const char *what);
-
 namespace {
 
 constexpr int kZzStates = 512;     // states staged in shared memory per tile
@@ -113,34 +110,23 @@ __global__ void __launch_bounds__(256, 1) k_zz_gram(int64_t n, int n_sites, int 
   for (int t = threadIdx.x; t < size; t += blockDim.x) partials[(int64_t)blockIdx.x * size + t] = s_block[t];
 }
 
-// one wave of resident CTAs over the tiles of states (at least one, so that an empty block still writes its partials);
-// launch == true also launches
-template <bool CE, int CT>
-int zz_run(bool launch, int64_t n, int n_sites, const uint64_t *reps, const double *x, double *partials,
-           cudaStream_t s) {
-  const int rows = zz_row_tiles(n_sites), slices = zz_slices(n_sites), threads = 32 * rows * slices;
-  const size_t smem = (size_t)16 * rows * 8 * CT * sizeof(double);
-  int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_zz_gram<CE, CT>, threads, smem);
-  const int64_t tiles = (std::max<int64_t>(n, 0) + kZzStates - 1) / kZzStates;
-  const int grid = (int)std::min<int64_t>(std::max<int64_t>(tiles, 1), (int64_t)sm_count() * std::max(per_sm, 1));
-  if (launch) k_zz_gram<CE, CT><<<grid, threads, smem, s>>>(n, n_sites, rows, slices, reps, x, partials);
-  return grid;
+// a k_zz_gram CTA: a warp per row tile and slice, the CTA's block of the Gram matrix in shared memory
+int zz_threads(int n_sites) { return 32 * zz_row_tiles(n_sites) * zz_slices(n_sites); }
+size_t zz_smem(int n_sites) { return (size_t)16 * zz_row_tiles(n_sites) * 8 * zz_col_tiles(n_sites) * sizeof(double); }
+
+// one wave of resident CTAs of `kernel` over the tiles of n states (at least one, so that an empty block still writes
+// its partials)
+template <typename K>
+int zz_grid(K kernel, int64_t n, int n_sites) {
+  return one_wave(kernel, (std::max<int64_t>(n, 0) + kZzStates - 1) / kZzStates, zz_smem(n_sites), zz_threads(n_sites));
 }
 
-template <bool CE>
-int zz_dispatch(bool launch, int64_t n, int n_sites, const uint64_t *reps, const double *x, double *partials,
-                cudaStream_t s) {
-  switch (zz_col_tiles(n_sites)) {
-    case 1: return zz_run<CE, 1>(launch, n, n_sites, reps, x, partials, s);
-    case 2: return zz_run<CE, 2>(launch, n, n_sites, reps, x, partials, s);
-    case 3: return zz_run<CE, 3>(launch, n, n_sites, reps, x, partials, s);
-    case 4: return zz_run<CE, 4>(launch, n, n_sites, reps, x, partials, s);
-    case 5: return zz_run<CE, 5>(launch, n, n_sites, reps, x, partials, s);
-    case 6: return zz_run<CE, 6>(launch, n, n_sites, reps, x, partials, s);
-    case 7: return zz_run<CE, 7>(launch, n, n_sites, reps, x, partials, s);
-    default: return zz_run<CE, 8>(launch, n, n_sites, reps, x, partials, s);
-  }
+// f(k_zz_gram<CE, CT>) for the column tiles CT of n_sites
+template <typename F>
+auto with_zz_gram(bool complex_elements, int n_sites, F &&f) {
+  return with_bool(complex_elements, [&](auto ce) {
+    return with_choice<1, 2, 3, 4, 5, 6, 7, 8>(zz_col_tiles(n_sites), [&](auto ct) { return f(k_zz_gram<ce(), ct()>); });
+  });
 }
 
 // ---- flip-flop correlations (dmv_pm_correlations).  A row b and an antiparallel pair (i, j) with bit i of b set and
@@ -327,50 +313,25 @@ __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
 constexpr size_t kPmSmem = 96 * 1024;   // shared memory of one CTA: two CTAs per SM
 constexpr int kPmThreads = 256;
 
-template <typename K>
-int pm_grid(K kernel, int threads, size_t smem, int64_t work_blocks) {
-  CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-  return (int)std::min<int64_t>(std::max<int64_t>(work_blocks, 1), (int64_t)sm_count() * std::max(per_sm, 1));
-}
-
-template <int LOOK, int TK, bool CE, bool CPLX>
-void pm_rows_run(bool launch, const PmArgs &A, int &grid, cudaStream_t s) {
-  const size_t smem = (size_t)kPmThreads * (A.c_hi - A.c_lo) * (CPLX ? 16 : 8);
-  grid = pm_grid(k_pm_rows<LOOK, TK, CE, CPLX>, kPmThreads, smem, (A.n_rows + kPmThreads - 1) / kPmThreads);
-  if (launch) k_pm_rows<LOOK, TK, CE, CPLX><<<grid, kPmThreads, smem, s>>>(A);
-}
-
-template <int LOOK, bool CE>
-void pm_pairs_run(bool launch, const PmArgs &A, int &grid, cudaStream_t s) {
-  const size_t smem = (size_t)A.c_hi * 16;
-  grid = pm_grid(k_pm_pairs<LOOK, CE>, kPmThreads, smem, (A.n_rows + 31) / 32);
-  if (launch) k_pm_pairs<LOOK, CE><<<grid, kPmThreads, smem, s>>>(A);
-}
-
-template <int LOOK, bool CE, bool CPLX>
-void pm_rows_tk(bool launch, int tk, const PmArgs &A, int &grid, cudaStream_t s) {
-  if (tk == 4) pm_rows_run<LOOK, 4, CE, CPLX>(launch, A, grid, s);
-  else if (tk == 6) pm_rows_run<LOOK, 6, CE, CPLX>(launch, A, grid, s);
-  else pm_rows_run<LOOK, 0, CE, CPLX>(launch, A, grid, s);
-}
-
-// one launch of the walk the basis asks for (launch == false: only the grid)
-void pm_dispatch(bool launch, int look, int tk, bool ce, bool cplx, const PmArgs &A, int &grid, cudaStream_t s) {
-  switch (look) {
-    case PM_NONE: return ce ? pm_pairs_run<PM_NONE, true>(launch, A, grid, s) : pm_pairs_run<PM_NONE, false>(launch, A, grid, s);
-    case PM_INVERSION:
-      return ce ? pm_pairs_run<PM_INVERSION, true>(launch, A, grid, s)
-                : pm_pairs_run<PM_INVERSION, false>(launch, A, grid, s);
-    case PM_GROUP:   // tk only with trivial characters
-      if (ce) return pm_rows_tk<PM_GROUP, true, true>(launch, tk, A, grid, s);
-      return cplx ? pm_rows_tk<PM_GROUP, false, true>(launch, tk, A, grid, s)
-                  : pm_rows_tk<PM_GROUP, false, false>(launch, tk, A, grid, s);
-    default:
-      return ce ? pm_rows_tk<PM_TABLE, true, true>(launch, tk, A, grid, s)
-                : pm_rows_tk<PM_TABLE, false, false>(launch, tk, A, grid, s);
-  }
+// f(kernel) for the walk the basis asks for: k_pm_pairs<LOOK, CE> without permutations, else k_pm_rows<LOOK, TK, CE,
+// CPLX> (TK only with trivial characters).  The class sums are complex (CPLX) with complex vectors or characters;
+// PM_TABLE runs on trivial characters only, so there CPLX == CE.
+template <typename F>
+void with_pm_kernel(int look, int tk, bool ce, bool cplx, F &&f) {
+  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
+    with_bool(ce, [&](auto e) {
+      if constexpr (lk() <= PM_INVERSION) {
+        f(k_pm_pairs<lk(), e()>);
+      } else {
+        with_bool(cplx, [&](auto cx) {
+          with_choice<6, 4, 0>(tk, [&](auto t) {
+            if constexpr (lk() == PM_TABLE ? cx() == e() : cx() || !e()) f(k_pm_rows<lk(), t(), e(), cx()>);
+            else throw std::logic_error("k_pm_rows has no build for these sums");
+          });
+        });
+      }
+    });
+  });
 }
 
 }  // namespace
@@ -379,18 +340,20 @@ int zz_gram_columns(int n_sites) { return 8 * zz_col_tiles(n_sites); }
 size_t zz_gram_size(int n_sites) { return (size_t)16 * zz_row_tiles(n_sites) * zz_gram_columns(n_sites); }
 
 size_t zz_gram_partials(int64_t n, int n_sites) {
-  const int grid = std::max(zz_dispatch<false>(false, n, n_sites, nullptr, nullptr, nullptr, nullptr),
-                            zz_dispatch<true>(false, n, n_sites, nullptr, nullptr, nullptr, nullptr));
-  return (size_t)grid * zz_gram_size(n_sites);
+  auto grid = [&](bool ce) { return with_zz_gram(ce, n_sites, [&](auto kernel) { return zz_grid(kernel, n, n_sites); }); };
+  return (size_t)std::max(grid(false), grid(true)) * zz_gram_size(n_sites);
 }
 
 void launch_zz_gram(int64_t n, bool complex_elements, int n_sites, const uint64_t *reps, const double *x,
                     double *partials, double *gram, cudaStream_t s) {
   if (n_sites < 1 || n_sites > 64) throw std::runtime_error("k_zz_gram: 1 to 64 sites");
-  const int grid = complex_elements ? zz_dispatch<true>(true, n, n_sites, reps, x, partials, s)
-                                    : zz_dispatch<false>(true, n, n_sites, reps, x, partials, s);
-  check_launch("k_zz_gram");
-  launch_reduce_partials(grid, (int)(zz_gram_size(n_sites) / 2), partials, gram, s);
+  with_zz_gram(complex_elements, n_sites, [&](auto kernel) {
+    const int grid = zz_grid(kernel, n, n_sites);
+    kernel<<<grid, zz_threads(n_sites), zz_smem(n_sites), s>>>(n, n_sites, zz_row_tiles(n_sites), zz_slices(n_sites),
+                                                                reps, x, partials);
+    check_launch("k_zz_gram");
+    launch_reduce_partials(grid, (int)(zz_gram_size(n_sites) / 2), partials, gram, s);
+  });
 }
 
 }  // namespace dmv
@@ -503,16 +466,22 @@ void pm_finish(int N, const PmClasses &K, const double *sums, double W, const do
 // sums[2 c + {0, 1}] = class sum c of the vector A.x over this rank's rows (classes < count).  The lane-major walk runs
 // once per group of classes whose slots fit in shared memory.
 void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, double *sums) {
-  const int per_pass = look <= PM_INVERSION ? count : (int)(kPmSmem / ((size_t)kPmThreads * (cplx ? 16 : 8)));
+  const bool pairs = look <= PM_INVERSION;
+  const int per_pass = pairs ? count : (int)(kPmSmem / ((size_t)kPmThreads * (cplx ? 16 : 8)));
   for (int c0 = 0; c0 < count; c0 += per_pass) {
     A.c_lo = c0;
     A.c_hi = std::min(count, c0 + per_pass);
-    int grid = 0;
-    pm_dispatch(false, look, tk, run.ce, cplx, A, grid, run.st);
-    A.partials = run.partials((size_t)grid * (A.c_hi - A.c_lo) * 2);
-    pm_dispatch(true, look, tk, run.ce, cplx, A, grid, run.st);
-    check_launch(look <= PM_INVERSION ? "k_pm_pairs" : "k_pm_rows");
-    launch_reduce_partials(grid, A.c_hi - A.c_lo, A.partials, sums + 2 * c0, run.st);
+    // k_pm_pairs: a tile of 32 rows per CTA and a slot per class; k_pm_rows: a row per thread and a slot per class and
+    // thread
+    const size_t smem = pairs ? (size_t)A.c_hi * 16 : (size_t)kPmThreads * (A.c_hi - A.c_lo) * (cplx ? 16 : 8);
+    const int64_t work = pairs ? (A.n_rows + 31) / 32 : (A.n_rows + kPmThreads - 1) / kPmThreads;
+    with_pm_kernel(look, tk, run.ce, cplx, [&](auto kernel) {
+      const int grid = one_wave(kernel, work, smem, kPmThreads);
+      A.partials = run.partials((size_t)grid * (A.c_hi - A.c_lo) * 2);
+      kernel<<<grid, kPmThreads, smem, run.st>>>(A);
+      check_launch(pairs ? "k_pm_pairs" : "k_pm_rows");
+      launch_reduce_partials(grid, A.c_hi - A.c_lo, A.partials, sums + 2 * c0, run.st);
+    });
   }
 }
 

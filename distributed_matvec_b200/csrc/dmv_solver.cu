@@ -15,8 +15,6 @@
 
 namespace dmv {
 
-void count_launch();
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -608,74 +606,31 @@ __global__ void __launch_bounds__(kThreads) k_quad_update(int64_t n, double *P, 
 
 }  // namespace
 
-int sm_count() {
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  return sms > 0 ? sms : 132;
-}
-
-void check_launch(const char *what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
-  count_launch();
-}
-
 namespace {
 
 constexpr int64_t ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 
-// `ctas` CTAs' worth of work, at least one (so that an empty block still writes its partials), at most per_sm per SM
-int clamp_grid(int64_t ctas, int per_sm) {
-  return (int)std::min<int64_t>(std::max<int64_t>(ctas, 1), (int64_t)sm_count() * std::max(per_sm, 1));
-}
-
 // the vector kernels with atomic or no reductions: eight CTAs per SM at most
-int blocks_for(int64_t n) { return clamp_grid(ceil_div(n, kThreads), 8); }
-
-// one wave of resident CTAs of `kernel` (`threads` each, `smem` bytes of dynamic shared memory: the opt-in above 48 KB
-// is set here) over `ctas` CTAs' worth of work
-template <typename K>
-int one_wave(K kernel, int64_t ctas, size_t smem = 0, int threads = kThreads) {
-  if (smem > 48 * 1024)
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-      throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
-  int per_sm = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem);
-  return clamp_grid(ctas, per_sm);
-}
-
-// f(std::integral_constant<bool, CE>) for complex / real elements
-template <typename F>
-auto with_ce(bool complex_elements, F &&f) {
-  return complex_elements ? f(std::true_type{}) : f(std::false_type{});
-}
+int blocks_for(int64_t n) { return capped_grid(ceil_div(n, kThreads), (int64_t)sm_count() * 8); }
 
 // f(std::integral_constant<int, W>) for the W = 1 .. kMaxBlockRhs vectors of a block or a group
 template <typename F>
 void with_width(int w, F &&f) {
-  switch (w) {
-    case 1: f(std::integral_constant<int, 1>{}); break;
-    case 2: f(std::integral_constant<int, 2>{}); break;
-    case 3: f(std::integral_constant<int, 3>{}); break;
-    case 4: f(std::integral_constant<int, 4>{}); break;
-    case 5: f(std::integral_constant<int, 5>{}); break;
-    default: f(std::integral_constant<int, 6>{}); break;
-  }
+  with_choice<1, 2, 3, 4, 5, 6>(w, f);
 }
 
 }  // namespace
 
 void launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s) {
   if (n <= 0) return;
-  with_ce(complex_elements, [&](auto ce) { k_dot<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2); });
+  with_bool(complex_elements, [&](auto ce) { k_dot<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2); });
   check_launch("k_dot");
 }
 
 void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
                            const double *coef2, double *out1, cudaStream_t s) {
   if (n <= 0) return;
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     k_lanczos_update<ce()><<<blocks_for(ce() ? 2 * n : n), kThreads, 0, s>>>(n, w, v, u, coef2, out1);
   });
   check_launch("k_lanczos_update");
@@ -683,8 +638,7 @@ void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const do
 
 void launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s) {
   if (words <= 0) return;
-  if (accumulate) k_scale<true><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y);
-  else k_scale<false><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y);
+  with_bool(accumulate, [&](auto acc) { k_scale<acc()><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y); });
   check_launch("k_scale");
 }
 
@@ -698,12 +652,12 @@ namespace {
 
 // CTAs of a k_block_dot / k_block_combine launch over n elements
 int block_dot_grid(int64_t n, bool complex_elements) {
-  return with_ce(complex_elements, [&](auto ce) {
+  return with_bool(complex_elements, [&](auto ce) {
     return one_wave(k_block_dot<ce()>, ceil_div(ceil_div(std::max<int64_t>(n, 0), dot_elems<ce()>()), kThreads));
   });
 }
 int block_combine_grid(int64_t n, bool complex_elements) {
-  return with_ce(complex_elements, [&](auto ce) { return one_wave(k_block_combine<ce()>, ceil_div(n, kThreads)); });
+  return with_bool(complex_elements, [&](auto ce) { return one_wave(k_block_combine<ce()>, ceil_div(n, kThreads)); });
 }
 
 }  // namespace
@@ -716,7 +670,7 @@ void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J,
                       double *h, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_dot: bad number of vectors");
   const int grid = block_dot_grid(n, complex_elements);
-  with_ce(complex_elements, [&](auto ce) { k_block_dot<ce()><<<grid, kThreads, 0, s>>>(n, V, J, w, partials); });
+  with_bool(complex_elements, [&](auto ce) { k_block_dot<ce()><<<grid, kThreads, 0, s>>>(n, V, J, w, partials); });
   check_launch("k_block_dot");
   launch_reduce_partials(grid, J + 1, partials, h, s);
 }
@@ -725,7 +679,7 @@ void launch_block_combine(int64_t n, bool complex_elements, double a, const doub
                           const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_combine: bad number of vectors");
   const int grid = block_combine_grid(n, complex_elements);
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     k_block_combine<ce()><<<grid, kThreads, 0, s>>>(n, a, w, V, J, coef, out, partials);
   });
   check_launch("k_block_combine");
@@ -742,7 +696,7 @@ void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_gram: bad number of vectors");
   const int width = J * R + R * R;
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     with_width(R, [&](auto r) {
       constexpr bool CE = ce();
       constexpr int E = gram_elems<CE, r()>();
@@ -759,7 +713,7 @@ void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int
                          int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_update: bad number of vectors");
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     with_width(R, [&](auto r) {
       const int grid = one_wave(k_block_update<ce(), r()>, ceil_div(std::max<int64_t>(n, 0), kThreads));
       k_block_update<ce(), r()><<<grid, kThreads, 0, s>>>(n, V, J, coef, W, w_stride, partials);
@@ -779,7 +733,7 @@ void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int
   if (k < 1 || k > kMaxBlockVectors || l < 1 || l > k) throw std::runtime_error("k_block_rotate: bad shape");
   if (n <= 0) return;
   const size_t smem = (size_t)k * kRotWords * sizeof(double);
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     const int grid = one_wave(k_block_rotate<ce()>, ceil_div(n, ce() ? kRotWords / 2 : kRotWords), smem);
     k_block_rotate<ce()><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
   });
@@ -794,7 +748,7 @@ size_t quad_partials(int G) {
 void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
                       double *x, cudaStream_t s) {
   if (n <= 0) return;
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     k_quad_fill<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
   });
   check_launch("k_quad_fill");
@@ -803,7 +757,7 @@ void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, ui
 void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
                      double *out, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_dot: bad number of vectors");
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     with_width(G, [&](auto g) {
       const int grid = one_wave(k_quad_dot<ce(), g()>, ceil_div(n, kThreads));
       k_quad_dot<ce(), g()><<<grid, kThreads, 0, s>>>(n, A, B, partials);
@@ -816,7 +770,7 @@ void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, c
 void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
                         const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_update: bad number of vectors");
-  with_ce(complex_elements, [&](auto ce) {
+  with_bool(complex_elements, [&](auto ce) {
     with_width(G, [&](auto g) {
       const int grid = one_wave(k_quad_update<ce(), g()>, ceil_div(n, kThreads));
       k_quad_update<ce(), g()><<<grid, kThreads, 0, s>>>(n, P, Q, W, dot, b2, j, partials);

@@ -1,6 +1,6 @@
 """Every build of k_rows that set_option can select, in full vector against the CPU oracle.
 
-launch_rows_e picks one of about 30 instantiations of k_rows: the element type (float64 / complex128), the orbit minimum
+launch_rows picks one of about 30 instantiations of k_rows: the element type (float64 / complex128), the orbit minimum
 (TK = 6 / 4: the square-torus form of the 6x6 / 4x4 lattice; 0: the generic orbit walk), the look-up table (ordered by key
 prefix with 2^rows_table_bits directory blocks and rows_table_buckets buckets per state, hashed homes, or the perfect
 hash) and the CTAs per SM it is compiled for (rows_ctas 2, 3 or 4; the 3- and 4-CTA builds have other register

@@ -59,7 +59,7 @@ def main():
                   f"(median {stacks[len(stacks) // 2]}), static shared {max(i[3] for i in inst)} bytes\n")
             continue
         print("| instance | registers | stack bytes | static shared |\n|---|---|---|---|")
-        for s, reg, stack, shared in inst:
+        for s, reg, stack, shared in sorted(inst):   # by name: the tables do not follow the host's instantiation order
             print(f"| `{s}` | {reg} | {stack} | {shared} |")
         print()
 
