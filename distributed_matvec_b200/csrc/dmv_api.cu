@@ -714,6 +714,9 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   p.mph = basis->mph;
   p.dense = basis->dense_index ? basis->d_dense.ptr : nullptr;
   p.row_split = 1;
+  p.rows_l2 = basis->opt.rows_l2;
+  p.rows_l2_window = (uint32_t)std::min<int64_t>((int64_t)basis->opt.rows_l2_window << 15, basis->table_slots);   // 32-byte buckets
+  p.rows_l2_per_state = (uint32_t)(basis->table_slots / std::max<int64_t>(1, basis->n_states));
   launch_rows(p, elt == DMV_C128, stream);
 }
 
@@ -903,6 +906,9 @@ const OptionRow kOptionTable[] = {
     {"rows_table_bits", &Options::rows_table_bits, 1, 14, {}, STALE_TABLE,
      "1 .. 14 (the directory of 2^bits blocks lives in shared memory)"},
     {"rows_table_buckets", &Options::rows_table_buckets, 0, 0, {2, 4, 8}, STALE_TABLE, "2, 4 or 8 buckets per state"},
+    {"rows_l2", &Options::rows_l2, 0, 2, {}, 0,
+     "0 no L2 hints, 1 far buckets and row data evict_first, 2 and near buckets evict_last"},
+    {"rows_l2_window", &Options::rows_l2_window, 0, 32, {}, 0, "0 .. 32 MB of table on either side of the row"},
     {"rounds", &Options::rounds, -1, 64, {}, STALE_ROUNDS,
      "-1 auto, 0 / 1 one-shot exchange, R <= 64 overlapped rounds"},
     {"gather_walk", &Options::gather_walk, 0, 2, {}, 0,
@@ -1120,6 +1126,8 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "rows")
     return ((use_pull(ctx) && !use_gather(ctx) && use_rows(ctx)) ||
             (ctx->replicated && ctx->global && !use_gather(ctx->global) && use_rows(ctx->global))) ? 1 : 0;
+  if (key == "rows_l2") return ctx->opt.rows_l2;
+  if (key == "rows_l2_window") return ctx->opt.rows_l2_window;
   if (key == "rows_ok") return ctx->rows_ok ? 1 : 0;
   if (key == "rows_dense") return ctx->dense_index ? (int64_t)ctx->mph.n_dense : (ctx->global && ctx->global->dense_index ? (int64_t)ctx->global->mph.n_dense : 0);
   if (key == "rounds") return ctx->rounds.ready ? ctx->rounds.R : 0;

@@ -165,6 +165,14 @@ struct Options {
   int rows_table = 1;
   int rows_table_bits = 14;
   int rows_table_buckets = 8;
+  // k_rows on the ordered layout: L2 eviction priority per access.  0 none; 1 evict_first for the buckets farther than
+  // rows_l2_window MB of table from the row's own place and for the row's state, norm, x and y; 2 and evict_last for the
+  // nearer buckets.  Results do not depend on either.  On an H100 (700 W, L2 flushed) 2 with a 16 MB window against 0:
+  // 6x6 square -4.7 % (complex128) / -4.0 % (float64), chain_32_symm -5.9 / -5.0 %, chain_36_symm +0.4 / -0.3 %; 1 is
+  // within 0.1 ms of 2, and without a window (every bucket evict_first) half of the gain is lost
+  // (profiles/h100_rows_l2_sweep.log)
+  int rows_l2 = 2;
+  int rows_l2_window = 16;
   int rows_batch_min = 2;   // doubles per state (vectors x element width) from which a batch goes through k_rows_batch
   int rows_batch = -1;      // -1 / 1: batched products of symmetric bases go through k_rows_batch | 0: vector by vector
   int exchange = -1;        // -1 auto (replicated x, else peer-direct when possible), 0 NCCL send/recv, 1 peer-direct,

@@ -889,11 +889,54 @@ __device__ __forceinline__ void store256(unsigned char *q, uint64_t a, uint64_t 
   asm volatile("st.global.v2.u64 [%0], {%1, %2};" ::"l"(q), "l"(a), "l"(b) : "memory");
   asm volatile("st.global.v2.u64 [%0+16], {%1, %2};" ::"l"(q), "l"(c), "l"(d) : "memory");
 }
-template <bool CE>
+// L2 eviction priority of single accesses (the ordered table of k_rows, option rows_l2): a policy is made once per
+// thread and handed to each load or store.  It travels in a uniform register, so it is one value per warp and
+// instruction: lanes that want different policies for the same access branch to different instructions.
+enum L2Evict { L2_NORMAL = 0, L2_FIRST = 1, L2_LAST = 2 };
+__device__ __forceinline__ uint64_t l2_policy(int evict) {
+  uint64_t policy;
+  if (evict == L2_FIRST) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(policy));
+  else if (evict == L2_LAST) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(policy));
+  else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(policy));
+  return policy;
+}
+__device__ __forceinline__ void load256_hint(const unsigned char *q, uint64_t policy, uint64_t &a, uint64_t &b, uint64_t &c,
+                                             uint64_t &d) {
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;"
+               : "=l"(a), "=l"(b) : "l"(q), "l"(policy));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%2+16], %3;"
+               : "=l"(c), "=l"(d) : "l"(q), "l"(policy));
+}
+// 8 or 16 bytes that are read or written once per product (a row's state, norm, x and y)
+__device__ __forceinline__ uint64_t load64_hint(const void *q, uint64_t policy) {
+  uint64_t a;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u64 %0, [%1], %2;" : "=l"(a) : "l"(q), "l"(policy));
+  return a;
+}
+__device__ __forceinline__ double load_hint(const double *q, uint64_t policy) {
+  return __longlong_as_double((long long)load64_hint(q, policy));
+}
+__device__ __forceinline__ double2 load_hint(const double2 *q, uint64_t policy) {
+  uint64_t a, b;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;"
+               : "=l"(a), "=l"(b) : "l"(q), "l"(policy));
+  return make_double2(__longlong_as_double((long long)a), __longlong_as_double((long long)b));
+}
+__device__ __forceinline__ void store_hint(double *q, double v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(q), "d"(v), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void store_hint(double2 *q, double2 v, uint64_t policy) {
+  asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(q), "d"(v.x), "d"(v.y), "l"(policy) : "memory");
+}
+// HINT: through load256_hint with `policy`
+template <bool CE, bool HINT = false>
 __device__ __forceinline__ void bucket_load(const unsigned char *__restrict__ table, uint32_t b, ulonglong2 &keys,
-                                            typename ValT<CE>::type &v0, typename ValT<CE>::type &v1) {
+                                            typename ValT<CE>::type &v0, typename ValT<CE>::type &v1,
+                                            uint64_t policy = 0) {
   uint64_t w0, w1, w2, w3;
-  load256(table + (size_t)b * 32, w0, w1, w2, w3);   // one bucket = one 32-byte sector = one request
+  // one bucket = one 32-byte sector = one request
+  if constexpr (HINT) load256_hint(table + (size_t)b * 32, policy, w0, w1, w2, w3);
+  else load256(table + (size_t)b * 32, w0, w1, w2, w3);
   if constexpr (CE) {   // { key, spare, re, im }
     keys = make_ulonglong2(w0, w1);                  // (one slot: the second word is spare)
     v0 = make_double2(__longlong_as_double((long long)w2), __longlong_as_double((long long)w3));
@@ -957,6 +1000,10 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   const E zero = v_make(0.0, 0.0, (E *)nullptr);
   const PerfectHash H = p.mph;
   const unsigned char *__restrict__ dense = reinterpret_cast<const unsigned char *>(p.dense);
+  // ORD, p.rows_l2: the buckets within p.rows_l2_window of the row's own place in the table are the ones the rows in
+  // flight share (near), every other bucket is read once while they pass (far), and so is what belongs to the row alone
+  const uint64_t far_policy = l2_policy(ORD && p.rows_l2 >= 1 ? L2_FIRST : L2_NORMAL);
+  const uint64_t near_policy = l2_policy(ORD && p.rows_l2 == 2 ? L2_LAST : L2_NORMAL);
 
   const int64_t n_rows = p.row_end - p.row_begin;
   const int64_t n_tiles = (n_rows + 31) / 32;
@@ -964,7 +1011,22 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   for (int64_t tile = (int64_t)blockIdx.x * kWarps + warp; tile < n_tiles; tile += warps_total) {
     const int64_t i = p.row_begin + tile * 32 + lane;
     const bool valid = i < p.row_end;
-    const uint64_t b = valid ? __ldg(row_states + i) : 0ull;
+    uint64_t b = 0;
+    if (valid) b = ORD ? load64_hint(row_states + i, far_policy) : __ldg(row_states + i);
+    // near: near_lo <= bucket < near_lo + near_span.  A state of rank r lives in its block's buckets, and those lie
+    // around buckets-per-state * r; rows that are a part of the table's basis (p.row_states) take their own home
+    uint32_t near_lo = 0, near_span = 0;
+    if constexpr (ORD) {
+      uint32_t centre;
+      if (p.row_states == nullptr) {
+        centre = p.rows_l2_per_state * (uint32_t)i;
+      } else {
+        const uint32_t blk = ordered_block(b, p.table_dir.k_lo, p.table_dir.shift, p.table_dir.last);
+        centre = ordered_slot(b, sdir[blk], sdir[blk + 1]);
+      }
+      near_lo = centre > p.rows_l2_window ? centre - p.rows_l2_window : 0u;
+      near_span = centre - near_lo + p.rows_l2_window;
+    }
     const uint64_t bt = TK > 0 ? torus_sq_columns<TK>(b) : 0ull;   // the row's transposed state: see orbit_min_torus_sq_t
     E acc = zero;
     int w = 0;
@@ -1055,6 +1117,11 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
     uint32_t b0 = 0, b1 = 0;
     ulonglong2 k0 = make_ulonglong2(0, 0), k1 = k0;
     E v00 = zero, v01 = zero, v10 = zero, v11 = zero;
+    auto request = [&]() {   // ask for bucket b0
+      if (!ORD || p.rows_l2 == 0) bucket_load<CE>(table, b0, k0, v00, v01);
+      else if (b0 - near_lo < near_span) bucket_load<CE, true>(table, b0, k0, v00, v01, near_policy);
+      else bucket_load<CE, true>(table, b0, k0, v00, v01, far_policy);
+    };
     for (;;) {
       while (valid && rt.mask == 0 && 64 * (w + 1) < p.n_groups) {
         ++w;
@@ -1081,7 +1148,7 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
       // ---- issue a new request: the continuation of a missed one, else the next term of the row
       if (retry) {
         want0 = want_r; c0 = c_r; b0 = b_r;
-        bucket_load<CE>(table, b0, k0, v00, v01);
+        request();
         live0 = true;
       } else if (has) {
         uint64_t flip;
@@ -1096,7 +1163,12 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
         } else {
           b0 = table_slot(want0, n_buckets);
         }
-        bucket_load<CE>(table, b0, k0, v00, v01);
+#ifdef DMV_ROWS_ORBIT_ONLY   // measurement builds only: no look-up, wrong results on purpose (the minimum and the bucket stay live)
+        k0 = make_ulonglong2(want0, want0);
+        v00 = v01 = v_make((double)(b0 & 7u), 0.0, (E *)nullptr);
+#else
+        request();
+#endif
         live0 = true;
       } else {
         live0 = false;
@@ -1104,18 +1176,21 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
     }
     }
     if (valid) {
-      const double inv_nb = 1.0 / __ldg(row_norms + i);
+      const double inv_nb = 1.0 / (ORD ? load_hint(row_norms + i, far_policy) : __ldg(row_norms + i));
       E out;
       if (p.n_diag > 0) {
         double dre, dim;
         diagonal<false>(T, p.n_diag, b, dre, dim);
-        const E xi = load_x<CE>(p.x, p.x_row_offset + i);
+        E xi;
+        if constexpr (ORD) xi = load_hint(reinterpret_cast<const E *>(p.x) + p.x_row_offset + i, far_policy);
+        else xi = load_x<CE>(p.x, p.x_row_offset + i);
         out = v_scale(xi, dre);   // real operator: the diagonal is real
       } else {
         out = reinterpret_cast<const E *>(p.y)[i];
       }
       axpy(out, inv_nb, acc);
-      reinterpret_cast<E *>(p.y)[i] = out;
+      if constexpr (ORD) store_hint(reinterpret_cast<E *>(p.y) + i, out, far_policy);
+      else reinterpret_cast<E *>(p.y)[i] = out;
     }
   }
   if (bad) {

@@ -88,6 +88,10 @@ int dmv_synchronize(dmv_context *ctx);
  *                        states always use hashed homes)
  *          "rows_table_bits" = 1 .. 14 (default 14): the ordered layout's directory has at most 2^bits blocks
  *          "rows_table_buckets" = 2 | 4 | 8 (default 8): complex128 buckets per state of the ordered layout
+ *          "rows_l2" = 0 | 1 | 2 (default): L2 eviction priority of k_rows' accesses on the ordered layout, per
+ *                        instruction (nothing device-wide is set).  1: evict_first for the buckets farther than
+ *                        "rows_l2_window" = 0 .. 32 (default 16) MB of table from the row's own place, and for the row's
+ *                        state, norm, x and y; 2: and evict_last for the nearer buckets; 0: none.  y does not depend on it
  *          "rows_ctas" = 2 (default) | 3 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread
  *                        122 | 80 | 64; at 80 and 64 words of the pipeline state spill, and on an H100 the extra warps do
  *                        not pay for it)
