@@ -1400,7 +1400,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
   require_states(ctx);
   if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
-  if (x == y) throw std::runtime_error("x and y must not alias");
+  if (x == y && ctx->n_states > 0) throw std::runtime_error("x and y must not alias");   // (a rank without states: both null)
   const size_t vec_bytes = (size_t)ctx->n_states * 8 * elt;
   const char *xb = reinterpret_cast<const char *>(x);
   char *yb = reinterpret_cast<char *>(y);

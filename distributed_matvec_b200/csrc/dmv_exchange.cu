@@ -273,8 +273,8 @@ void setup_rounds(dmv_context *ctx) {
   Q.my_off.assign((size_t)R * P, 0);
   for (int r = 0; r < R; ++r)
     for (int q = 0; q < P; ++q) if (q != ctx->rank) Q.my_off[(size_t)r * P + q] = region(q, r, ctx->rank);
-  Q.d_in_betas.alloc((size_t)std::max<int64_t>(1, 2 * Q.in_total));
-  Q.d_in_coeffs.alloc((size_t)std::max<int64_t>(1, 4 * Q.in_total));
+  Q.d_in_betas.alloc((size_t)std::max<int64_t>(1, 2 * Q.in_total));          // two buffers (alternating products)
+  Q.d_in_coeffs.alloc((size_t)std::max<int64_t>(1, 4 * Q.in_total));         // of 2 * in_total doubles each
   Q.d_flags.alloc(P);
   CUDA_CHECK(cudaMemsetAsync(Q.d_flags.ptr, 0, sizeof(unsigned) * P, ctx->stream));
   Q.seq = 0;
@@ -329,7 +329,10 @@ void setup_rounds(dmv_context *ctx) {
   Q.ready = true;
 }
 
-// where my records of (buffer, round, destination) go: [2][R][P] pointers into the peers' incoming buffers
+// where my records of (buffer, round, destination) go: [2][R][P] pointers into the peers' incoming buffers.
+// Buffer b's coefficients start at b * 2 * peer_total doubles, whatever the width: both buffers are laid out for 16-byte
+// records, so that a product of one width never writes into coefficients the owner still reads for the previous product
+// of the other width (nothing but the per-round flags orders the two; see DESIGN.md section 5).
 void upload_round_pointers(dmv_context *ctx, int width) {
   dmv_context::Rounds &Q = ctx->rounds;
   const int P = ctx->num_ranks, R = Q.R;
@@ -339,9 +342,10 @@ void upload_round_pointers(dmv_context *ctx, int width) {
     for (int r = 0; r < R; ++r)
       for (int q = 0; q < P; ++q) {
         if (q == ctx->rank) continue;
-        const int64_t first = (int64_t)b * Q.peer_total[q] + Q.my_off[(size_t)r * P + q];
-        bp[((size_t)b * R + r) * P + q] = reinterpret_cast<uint64_t *>(Q.peer_betas[q]) + first;
-        cp[((size_t)b * R + r) * P + q] = reinterpret_cast<double *>(Q.peer_coeffs[q]) + first * width;
+        const int64_t off = Q.my_off[(size_t)r * P + q];
+        bp[((size_t)b * R + r) * P + q] = reinterpret_cast<uint64_t *>(Q.peer_betas[q]) + b * Q.peer_total[q] + off;
+        cp[((size_t)b * R + r) * P + q] =
+            reinterpret_cast<double *>(Q.peer_coeffs[q]) + b * 2 * Q.peer_total[q] + off * width;
       }
   Q.d_bptr.upload(bp, ctx->stream);
   Q.d_cptr.upload(cp, ctx->stream);
@@ -382,12 +386,12 @@ void rounds_product(dmv_context *ctx, int elt, const void *x_dev, void *y_dev) {
     launch_raise_flags(Q.d_peer_flags.ptr, P, ctx->rank, value, ctx->stream);
     // owner side, second stream: every sender has delivered round r -> search + accumulate its slice
     launch_wait_flags(Q.d_flags.ptr, P, value, ctx->d_status.ptr, Q.acc_stream);
-    const int64_t first = (int64_t)b * Q.in_total + Q.in_slice[r], count = Q.in_slice[r + 1] - Q.in_slice[r];
+    const int64_t count = Q.in_slice[r + 1] - Q.in_slice[r];
     if (count > 0) {
       KernelParams pa = base_params(ctx);
       pa.y = y_dev;
-      launch_accumulate(pa, ctx->proj, cv, elt == DMV_C128, count, Q.d_in_betas.ptr + first,
-                        Q.d_in_coeffs.ptr + first * width, Q.acc_stream);
+      launch_accumulate(pa, ctx->proj, cv, elt == DMV_C128, count, Q.d_in_betas.ptr + b * Q.in_total + Q.in_slice[r],
+                        Q.d_in_coeffs.ptr + b * 2 * Q.in_total + Q.in_slice[r] * width, Q.acc_stream);
     }
   }
   ++Q.seq;
@@ -622,7 +626,7 @@ int dmv_matvec(dmv_context *ctx, int elt, const void *x, void *y) {
   if (!ctx->exchange_decided) decide_exchange(ctx);
   if (ctx->replicated) {
     // ---- replicated-x product: all-gather x into equal slots, then this rank's rows by the row traversal
-    if (x == y) throw std::runtime_error("x and y must not alias");
+    if (x == y && ctx->n_states > 0) throw std::runtime_error("x and y must not alias");   // (a rank without states: both null)
     const size_t esz = (size_t)8 * elt, bytes = (size_t)ctx->n_states * esz;
     CUDA_CHECK(cudaEventRecord(ctx->ev[0], ctx->stream));
     void *y_dev = y;
