@@ -112,6 +112,8 @@ _SIGNATURES = [
                                           C.c_void_p]),
     ("dmv_debug_ordered_table", C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                           C.c_void_p]),
+    ("dmv_debug_dense_order", C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]),
     ("dmv_debug_torus_sq_rows", C.c_int, [C.POINTER(BasisDesc), C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                           C.c_void_p, C.c_void_p]),
 ]

@@ -586,12 +586,114 @@ void do_plan(dmv_context *ctx) {
   ctx->planned = true;
 }
 
+// whether k_rows looks its targets up in the dense ordered table (option rows_dense_order; the perfect-hash index wins)
+bool dense_order_wanted(const dmv_context *ctx) {
+  if (ctx->opt.rows_index == 1) return false;
+  if (ctx->opt.rows_dense_order >= 0) return ctx->opt.rows_dense_order == 1;
+  // auto: in place of the ordered layout, which it beats on every measured workload (one H100 at 700 W, L2 flushed,
+  // 2 MB window: 6x6 square -5.8 % complex128 / -10.4 % float64, chain_32_symm -13 / -10 %, chain_36_symm -16 / -2 %,
+  // profiles/h100_rows_dense_order_sweep.log)
+  return ctx->opt.rows_table == 1;
+}
+
+// Dense ordered table over the ascending reps[0, n) (see DenseOrder): the directory dir[0 .. D.last + 1] of D (one slot
+// per state), the rank blocks and the slot of every state.  Returns the number of states the two levels place.
+uint32_t dord_build(const uint64_t *reps, int64_t n, OrderedDir &D, std::vector<uint32_t> &dir,
+                    std::vector<uint64_t> &blocks, std::vector<uint32_t> &slot_of) {
+  if (n < 1 || n >= 2147483647ll) throw std::runtime_error("dense ordered table: 1 .. 2^31 - 1 states");
+  dir.resize((size_t)D.last + 2);
+  for (uint32_t p = 0; p <= D.last + 1; ++p) dir[p] = ordered_dir_entry(reps, n, D, 1u, p);
+  D.dir = dir.data();
+  const uint32_t nb = (uint32_t)((n + kDordStates - 1) / kDordStates);
+  std::vector<uint32_t> rb((size_t)n), count(nb, 0);
+  std::vector<uint64_t> seen0(2 * (size_t)nb, 0), coll0(2 * (size_t)nb, 0), seen1(nb, 0), coll1(nb, 0);
+  auto mark = [](std::vector<uint64_t> &seen, std::vector<uint64_t> &coll, size_t word, uint32_t bit) {
+    const uint64_t m = 1ull << bit;
+    if (seen[word] & m) coll[word] |= m;
+    seen[word] |= m;
+  };
+  for (int64_t k = 0; k < n; ++k) {
+    const uint64_t h = dord_hash(reps[k]);
+    const uint32_t p = ordered_block(reps[k], D.k_lo, D.shift, D.last);
+    const uint32_t r = dord_block(h, dir[p], dir[p + 1]);
+    rb[k] = r;
+    ++count[r];
+    const uint32_t b0 = dord_bits(h) & 127u;
+    mark(seen0, coll0, 2 * (size_t)r + (b0 >> 6), b0 & 63u);
+  }
+  auto collided = [](const std::vector<uint64_t> &coll, size_t word, uint32_t bit) { return (coll[word] >> bit) & 1ull; };
+  for (int64_t k = 0; k < n; ++k) {   // level 1: the keys that collided at level 0
+    const uint32_t bits = dord_bits(dord_hash(reps[k])), b0 = bits & 127u;
+    if (collided(coll0, 2 * (size_t)rb[k] + (b0 >> 6), b0 & 63u)) mark(seen1, coll1, rb[k], (bits >> 8) & 63u);
+  }
+  std::vector<uint64_t> seen2(nb, 0), coll2(nb, 0);
+  for (int64_t k = 0; k < n; ++k) {   // level 2: the keys that collided at level 1 too
+    const uint32_t bits = dord_bits(dord_hash(reps[k])), b0 = bits & 127u;
+    if (collided(coll0, 2 * (size_t)rb[k] + (b0 >> 6), b0 & 63u) && collided(coll1, rb[k], (bits >> 8) & 63u))
+      mark(seen2, coll2, rb[k], bits >> 16);
+  }
+  blocks.assign(4 * (size_t)nb, 0);
+  uint64_t first = 0, placed = 0;
+  for (uint32_t r = 0; r < nb; ++r) {
+    uint64_t *w = blocks.data() + 4 * (size_t)r;
+    w[0] = seen0[2 * (size_t)r] & ~coll0[2 * (size_t)r];
+    w[1] = seen0[2 * (size_t)r + 1] & ~coll0[2 * (size_t)r + 1];
+    w[2] = seen1[r] & ~coll1[r];
+    const uint64_t l2 = seen2[r] & ~coll2[r];
+    const uint32_t in_levels = dord_popc(w[0]) + dord_popc(w[1]) + dord_popc(w[2]) + dord_popc(l2);
+    if (count[r] - in_levels > 255) throw std::runtime_error("dense ordered table: more than 255 leftovers in a rank block");
+    w[3] = first | l2 << 32 | (uint64_t)(count[r] - in_levels) << 56;
+    first += count[r];
+    placed += in_levels;
+    count[r] = 0;   // from here: leftovers of the rank block given a slot so far
+  }
+  slot_of.resize((size_t)n);
+  for (int64_t k = 0; k < n; ++k) {   // leftovers take their rank block's last slots in key order
+    const uint64_t *w = blocks.data() + 4 * (size_t)rb[k];
+    const uint32_t bits = dord_bits(dord_hash(reps[k])), b0 = bits & 127u;
+    const bool placed_here = ((w[b0 >> 6] >> (b0 & 63u)) & 1ull) || ((w[2] >> ((bits >> 8) & 63u)) & 1ull) ||
+                             ((w[3] >> (32 + (bits >> 16))) & 1ull);
+    uint32_t end = 0;
+    const uint32_t s = dord_slot(w[0], w[1], w[2], w[3], bits, end);
+    slot_of[k] = placed_here ? s : s + count[rb[k]]++;
+  }
+  return (uint32_t)placed;
+}
+
 // hash table of k_rows over ctx's representatives: keys once per basis and element type, values once per product
 void ensure_table(dmv_context *ctx, int elt) {
   if (ctx->table_elt == elt) return;
   const int64_t n = ctx->n_states;
   cudaStream_t st = ctx->stream;
   const bool ce = elt == DMV_C128;
+  ctx->dense_order = dense_order_wanted(ctx) && n >= 1;
+  ctx->dord = DenseOrder{};
+  if (ctx->dense_order) {   // ---- the dense ordered table: built on the host, one slot per state
+    ctx->dense_index = false;
+    ctx->mph = PerfectHash{};
+    std::vector<uint64_t> reps((size_t)n);
+    CUDA_CHECK(cudaMemcpyAsync(reps.data(), ctx->d_reps.ptr, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));
+    OrderedDir D = ordered_plan(reps[0], reps[n - 1], ctx->opt.rows_table_bits);
+    std::vector<uint32_t> dir, slot_of;
+    std::vector<uint64_t> blocks;
+    ctx->dord.n_placed = dord_build(reps.data(), n, D, dir, blocks, slot_of);
+    ctx->d_table.release();   // (the open-addressing table is not used; release() waits for the device)
+    ctx->d_table_dir.upload(dir, st);
+    ctx->d_dord_blocks.upload(blocks, st);
+    ctx->d_slot_of.upload(slot_of, st);
+    const size_t bytes = (size_t)n * (ce ? 32 : 16);
+    ctx->d_dense.alloc(bytes);
+    CUDA_CHECK(cudaMemsetAsync(ctx->d_dense.ptr, 0xff, bytes, st));
+    CUDA_CHECK(cudaStreamSynchronize(st));   // the host vectors go out of scope
+    D.dir = ctx->d_table_dir.ptr;
+    ctx->table_dir = D;
+    ctx->dord.blocks = ctx->d_dord_blocks.ptr;
+    ctx->dord.n_blocks = (uint32_t)(blocks.size() / 4);
+    ctx->table_slots = (uint32_t)n;
+    ctx->table_elt = elt;
+    return;
+  }
   // ---- dense index: two perfect-hash levels of 4 bits per state; what they cannot place goes to the table below
   const uint64_t *left_keys = ctx->d_reps.ptr;
   int64_t n_left = n;
@@ -702,7 +804,8 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   if (fill) {   // (a product cut into row chunks refreshes the values once, with its first chunk)
     CUDA_CHECK(cudaEventRecord(timer->ev_fill[0], stream));
     launch_table_fill(basis->n_states, elt == DMV_C128, x_all, basis->d_norms.ptr, pos, basis->d_slot_of.ptr,
-                      basis->d_reps.ptr, basis->d_table.ptr, basis->dense_index ? basis->d_dense.ptr : nullptr, stream);
+                      basis->d_reps.ptr, basis->d_table.ptr,
+                      basis->dense_index || basis->dense_order ? basis->d_dense.ptr : nullptr, stream);
     CUDA_CHECK(cudaEventRecord(timer->ev_fill[1], stream));
     timer->fill_timed = true;
   }
@@ -712,10 +815,13 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   p.table_slots = basis->table_slots;
   p.table_dir = basis->table_dir;
   p.mph = basis->mph;
-  p.dense = basis->dense_index ? basis->d_dense.ptr : nullptr;
+  p.dense = basis->dense_index || basis->dense_order ? basis->d_dense.ptr : nullptr;
+  p.dord = basis->dord;
   p.row_split = 1;
   p.rows_l2 = basis->opt.rows_l2;
-  p.rows_l2_window = (uint32_t)std::min<int64_t>((int64_t)basis->opt.rows_l2_window << 15, basis->table_slots);   // 32-byte buckets
+  // the window in slots: 32-byte buckets, or the dense ordered table's 32-byte (complex128) / 16-byte (float64) slots
+  const int slot_shift = basis->dense_order && elt != DMV_C128 ? 16 : 15;
+  p.rows_l2_window = (uint32_t)std::min<int64_t>((int64_t)basis->opt.rows_l2_window << slot_shift, basis->table_slots);
   p.rows_l2_per_state = (uint32_t)(basis->table_slots / std::max<int64_t>(1, basis->n_states));
   launch_rows(p, elt == DMV_C128, stream);
 }
@@ -906,6 +1012,8 @@ const OptionRow kOptionTable[] = {
     {"rows_table_bits", &Options::rows_table_bits, 1, 14, {}, STALE_TABLE,
      "1 .. 14 (the directory of 2^bits blocks lives in shared memory)"},
     {"rows_table_buckets", &Options::rows_table_buckets, 0, 0, {2, 4, 8}, STALE_TABLE, "2, 4 or 8 buckets per state"},
+    {"rows_dense_order", &Options::rows_dense_order, -1, 1, {}, STALE_TABLE,
+     "-1 auto, 0 off, 1 dense ordered table (one slot per state in key order)"},
     {"rows_l2", &Options::rows_l2, 0, 2, {}, 0,
      "0 no L2 hints, 1 far buckets and row data evict_first, 2 and near buckets evict_last"},
     {"rows_l2_window", &Options::rows_l2_window, 0, 32, {}, 0, "0 .. 32 MB of table on either side of the row"},
@@ -1129,7 +1237,13 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "rows_l2") return ctx->opt.rows_l2;
   if (key == "rows_l2_window") return ctx->opt.rows_l2_window;
   if (key == "rows_ok") return ctx->rows_ok ? 1 : 0;
+  // states the perfect-hash index places (rows_index = 1): 0 for every other table, the dense ordered one included
   if (key == "rows_dense") return ctx->dense_index ? (int64_t)ctx->mph.n_dense : (ctx->global && ctx->global->dense_index ? (int64_t)ctx->global->mph.n_dense : 0);
+  if (key == "rows_dense_order") return ctx->opt.rows_dense_order;
+  if (key == "rows_dense_order_on") return ctx->dense_order ? 1 : (ctx->global && ctx->global->dense_order ? 1 : 0);
+  // states the three levels of the dense ordered table place (the rest are its leftovers); 0 when it is not built
+  if (key == "rows_dense_order_placed")
+    return ctx->dense_order ? (int64_t)ctx->dord.n_placed : (ctx->global && ctx->global->dense_order ? (int64_t)ctx->global->dord.n_placed : 0);
   if (key == "rounds") return ctx->rounds.ready ? ctx->rounds.R : 0;
   if (key == "peer_gather") return (ctx->replicated && ctx->peer_gather) ? 1 : 0;
   if (key == "complex_coefficients") return ctx->complex_coefficients ? 1 : 0;
@@ -1655,6 +1769,37 @@ int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int bucke
     if (home) home[k] = h;
     if (probes) probes[k] = count;
   }
+  API_END
+}
+
+int dmv_debug_dense_order(const uint64_t *reps, int64_t n, int bits, uint32_t *block, uint32_t *slot, uint32_t *probes,
+                          int64_t *info) {
+  API_BEGIN
+  if (n < 1 || !reps || bits < 1 || bits > 14) throw std::runtime_error("bad arguments");
+  for (int64_t k = 1; k < n; ++k)
+    if (reps[k] <= reps[k - 1]) throw std::runtime_error("representatives must be ascending");
+  OrderedDir D = ordered_plan(reps[0], reps[n - 1], bits);
+  std::vector<uint32_t> dir, slot_of;
+  std::vector<uint64_t> blocks;
+  const uint32_t placed = dord_build(reps, n, D, dir, blocks, slot_of);
+  std::vector<uint64_t> keys((size_t)n, kEmptyKey);
+  for (int64_t k = 0; k < n; ++k) {
+    if (slot_of[k] >= (uint64_t)n || keys[slot_of[k]] != kEmptyKey) throw std::runtime_error("dense ordered table: slot taken twice");
+    keys[slot_of[k]] = reps[k];
+  }
+  for (int64_t k = 0; k < n; ++k) {   // the look-up of k_rows
+    const uint64_t h = dord_hash(reps[k]);
+    const uint32_t p = ordered_block(reps[k], D.k_lo, D.shift, D.last);
+    const uint64_t *w = blocks.data() + 4 * (size_t)dord_block(h, dir[p], dir[p + 1]);
+    uint32_t end = 0, count = 1;
+    uint32_t s = dord_slot(w[0], w[1], w[2], w[3], dord_bits(h), end);
+    while (s < end && keys[s] != reps[k]) { ++s; ++count; }
+    if (s >= end) throw std::runtime_error("dense ordered table: a representative is not found");
+    if (block) block[k] = p;
+    if (slot) slot[k] = s;
+    if (probes) probes[k] = count;
+  }
+  if (info) { info[0] = placed; info[1] = (int64_t)(blocks.size() / 4); }
   API_END
 }
 

@@ -165,14 +165,21 @@ struct Options {
   int rows_table = 1;
   int rows_table_bits = 14;
   int rows_table_buckets = 8;
+  // the dense ordered table instead (DenseOrder in dmv_device.cuh: one slot per state in key order, found through a
+  // perfect hash per rank block; its directory has 2^rows_table_bits blocks): -1 auto (see dense_order_wanted), 0 off,
+  // 1 on.  The perfect-hash index (rows_index = 1) takes precedence.
+  int rows_dense_order = -1;
   // k_rows on the ordered layout: L2 eviction priority per access.  0 none; 1 evict_first for the buckets farther than
   // rows_l2_window MB of table from the row's own place and for the row's state, norm, x and y; 2 and evict_last for the
   // nearer buckets.  Results do not depend on either.  On an H100 (700 W, L2 flushed) 2 with a 16 MB window against 0:
   // 6x6 square -4.7 % (complex128) / -4.0 % (float64), chain_32_symm -5.9 / -5.0 %, chain_36_symm +0.4 / -0.3 %; 1 is
   // within 0.1 ms of 2, and without a window (every bucket evict_first) half of the gain is lost
-  // (profiles/h100_rows_l2_sweep.log)
+  // (profiles/h100_rows_l2_sweep.log).  The dense ordered table, whose 12.6 MB of rank blocks (6x6 square) also take
+  // evict_last, is fastest with the smallest window measured, 2 MB (16 MB: +3.7 % complex128 on the 6x6 square,
+  // profiles/h100_rows_dense_order_sweep.log).  The ordered layout (rows_dense_order = 0) is 1 % slower at 2 MB than at
+  // 16 MB (complex128, 6x6 square); a caller who selects it may want rows_l2_window = 16
   int rows_l2 = 2;
-  int rows_l2_window = 16;
+  int rows_l2_window = 2;
   int rows_batch_min = 2;   // doubles per state (vectors x element width) from which a batch goes through k_rows_batch
   int rows_batch = -1;      // -1 / 1: batched products of symmetric bases go through k_rows_batch | 0: vector by vector
   int exchange = -1;        // -1 auto (replicated x, else peer-direct when possible), 0 NCCL send/recv, 1 peer-direct,
@@ -223,6 +230,9 @@ struct dmv_context {
   DevBuf<unsigned char> d_mph_blocks, d_dense;   // dense index: perfect-hash blocks, dense table of (key, value) slots
   PerfectHash mph{};
   bool dense_index = false;
+  DevBuf<uint64_t> d_dord_blocks;   // dense ordered table: rank blocks; its slots live in d_dense, its directory in d_table_dir
+  DenseOrder dord{};
+  bool dense_order = false;
   DevBuf<uint32_t> d_slot_of;
   uint32_t table_slots = 0;
   DevBuf<uint32_t> d_table_dir;

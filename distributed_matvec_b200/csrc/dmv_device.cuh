@@ -366,6 +366,79 @@ __host__ __device__ __forceinline__ uint32_t mph_rank(uint64_t w0, uint64_t w1, 
 }
 
 // ---------------------------------------------------------------------------------------------
+// Dense ordered table for k_rows (option rows_dense_order): ONE slot per state (32 bytes {key, spare, re, im} /
+// 16 bytes {key, value}), the slots in key order at the granularity of the ordered layout's prefix blocks, so a near
+// window of the table holds 8 times as many states as with 8 buckets per state.  The directory is the ordered layout's
+// with one slot per state (dir[p] = first representative of prefix block p).  A key of block p hashes to a virtual
+// position in [dir[p], dir[p + 1]); positions are cut into rank blocks of kDordStates states, and a rank block is one
+// 32-byte sector { w0, w1, w2, first | level-2 bits << 32 | leftovers << 56 }:
+//   level 0: 128 bits (w0, w1); bit b is set iff exactly one key of the rank block hashes to b;
+//   level 1: 64 bits (w2) over the keys that collided at level 0, likewise;
+//   level 2: 24 bits over the keys that collided at level 1, likewise;
+//   the keys no level places ("leftovers", 0.3 % on the 6x6 square) follow the placed ones in key order.
+// The keys of rank block R own slots [first, first + count): level-0 keys by rank among the set bits of w0 w1, then
+// level-1 and level-2 keys, then the leftovers, found by a short scan.  first = number of keys of the rank blocks before
+// R, so a key of block p lands in [dir[p], dir[p + 1]) up to about one rank block on either side (the rank blocks at the
+// block's ends also hold keys of its neighbours, as many as hash there).  One rank-block read (L2-resident:
+// 6.4 bits per state) and one slot read per look-up, both independent of how full the table is.
+// ---------------------------------------------------------------------------------------------
+constexpr uint32_t kDordStates = 40;
+struct DenseOrder {
+  const uint64_t *blocks;   // [n_blocks][4]; null: not in use
+  uint32_t n_blocks;
+  uint32_t n_placed;        // states the two levels place (the rest are leftovers)
+};
+__host__ __device__ __forceinline__ uint64_t dord_hash(uint64_t key) {
+  uint64_t h = key * 0x9E3779B97F4A7C15ull;
+  h ^= h >> 29;
+  h *= 0xBF58476D1CE4E5B9ull;
+  return h ^ (h >> 31);
+}
+// rank block of a key with hash h whose prefix block holds states [lo, hi); level bits b0 | b1 << 8
+__host__ __device__ __forceinline__ uint32_t dord_block(uint64_t h, uint32_t lo, uint32_t hi) {
+  const uint32_t v = lo + (uint32_t)(((h >> 32) * (uint64_t)(hi - lo)) >> 32);
+  return v / kDordStates;
+}
+__host__ __device__ __forceinline__ uint32_t dord_bits(uint64_t h) {
+  return (uint32_t)(h & 127u) | (uint32_t)((h >> 7) & 63u) << 8 | (uint32_t)((((h >> 13) & 0xffffu) * 24u) >> 16) << 16;
+}
+__host__ __device__ __forceinline__ uint32_t dord_popc(uint64_t w) {
+#ifdef __CUDA_ARCH__
+  return (uint32_t)__popcll(w);
+#else
+  return (uint32_t)__builtin_popcountll(w);
+#endif
+}
+// first slot to read for a key of the rank block { w0, w1, w2, w3 }, and the end of the slots it may be in: one slot
+// when a level places the key, else the block's leftovers (end == slot: none, the key is not a basis state)
+__host__ __device__ __forceinline__ uint32_t dord_slot(uint64_t w0, uint64_t w1, uint64_t w2, uint64_t w3, uint32_t bits,
+                                                       uint32_t &end) {
+  const uint32_t b0 = bits & 127u, b1 = (bits >> 8) & 63u, first = (uint32_t)w3;
+  const uint64_t m = b0 < 64 ? w0 : w1;
+  const uint32_t p0 = dord_popc(w0);
+  if ((m >> (b0 & 63u)) & 1ull) {
+    const uint32_t s = first + (b0 < 64 ? 0u : p0) + dord_popc(m & ((1ull << (b0 & 63u)) - 1ull));
+    end = s + 1;
+    return s;
+  }
+  const uint32_t p01 = p0 + dord_popc(w1);
+  if ((w2 >> b1) & 1ull) {
+    const uint32_t s = first + p01 + dord_popc(w2 & ((1ull << b1) - 1ull));
+    end = s + 1;
+    return s;
+  }
+  const uint32_t p012 = p01 + dord_popc(w2), w3b = (uint32_t)(w3 >> 32) & 0xffffffu, b2 = bits >> 16;
+  if ((w3b >> b2) & 1u) {
+    const uint32_t s = first + p012 + dord_popc(w3b & ((1u << b2) - 1u));
+    end = s + 1;
+    return s;
+  }
+  const uint32_t s = first + p012 + dord_popc(w3b);
+  end = s + (uint32_t)(w3 >> 56);
+  return s;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Bit permutations
 // ---------------------------------------------------------------------------------------------
 __host__ __device__ __forceinline__ uint64_t butterfly(uint64_t s, uint64_t mask, int delta) {

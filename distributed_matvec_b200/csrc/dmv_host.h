@@ -122,9 +122,12 @@ struct KernelParams {
   // `table` then only holds the few per cent of the states the two levels could not place
   PerfectHash mph;
   const void *dense;
+  // ... or the dense ordered table (dord.blocks not null): rank blocks -> slot of `dense`, table_dir its directory
+  DenseOrder dord;
   int32_t rows_ctas;           // k_rows / k_rows_batch: resident CTAs per SM the kernel is compiled for (2 default | 3 | 4)
   // k_rows on the ordered table: L2 eviction priorities (option rows_l2: 0 none | 1 far buckets and the row's own
   // accesses evict_first | 2 and near buckets evict_last); near = within rows_l2_window buckets of per_state * the row's rank
+  // (the dense ordered table: slots of the row's rank, and its rank blocks take the near priority)
   int32_t rows_l2;
   uint32_t rows_l2_window, rows_l2_per_state;
 };

@@ -947,6 +947,30 @@ __device__ __forceinline__ void bucket_load(const unsigned char *__restrict__ ta
     v1 = __longlong_as_double((long long)w3);
   }
 }
+// slot s of the dense tables (perfect hash, dense ordered): complex128 { key, spare, re, im }, float64 { key, value }
+template <bool CE, bool HINT = false>
+__device__ __forceinline__ void slot_load(const unsigned char *__restrict__ dense, uint32_t s, uint64_t &key,
+                                          typename ValT<CE>::type &v, uint64_t policy = 0) {
+  uint64_t a, b;
+  if constexpr (CE) {
+    uint64_t c, d;
+    if constexpr (HINT) load256_hint(dense + (size_t)s * 32, policy, a, b, c, d);
+    else load256(dense + (size_t)s * 32, a, b, c, d);
+    key = a;
+    v = make_double2(__longlong_as_double((long long)c), __longlong_as_double((long long)d));
+  } else {
+    const unsigned char *q = dense + (size_t)s * 16;
+    if constexpr (HINT) {
+      asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;"
+                   : "=l"(a), "=l"(b) : "l"(q), "l"(policy));
+    } else {
+      const ulonglong2 t = __ldg(reinterpret_cast<const ulonglong2 *>(q));
+      a = t.x; b = t.y;
+    }
+    key = a;
+    v = __longlong_as_double((long long)b);
+  }
+}
 __device__ __forceinline__ void axpy(double &acc, double c, double v) { acc = fma(c, v, acc); }
 __device__ __forceinline__ void axpy(double2 &acc, double c, double2 v) { acc.x = fma(c, v.x, acc.x); acc.y = fma(c, v.y, acc.y); }
 
@@ -969,7 +993,8 @@ __host__ __device__ inline RowsSmem rows_smem(const KernelParams &p, const SmemL
 // latency is hidden inside the lane, not by occupancy
 // ORD: ordered table layout (see ordered_block); its directory is staged into shared memory behind the other tables, so
 // a home costs two shared-memory reads and adds no dependent global access to the pipeline
-template <bool CE, int TK, bool MPH, int CTAS, bool ORD>
+// DORD (with ORD): the dense ordered table (see DenseOrder); request 0 is the rank block, request 1 the slot
+template <bool CE, int TK, bool MPH, int CTAS, bool ORD, bool DORD = false>
 __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
   using E = typename ValT<CE>::type;
   extern __shared__ __align__(16) unsigned char smem[];
@@ -1032,7 +1057,72 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
     int w = 0;
     RowTerms rt = row_terms<false>(T, 0, 0, min(64, p.n_groups), b);
     if (!valid) rt.mask = 0;
-    if constexpr (MPH) {
+    if constexpr (DORD) {
+      // ---- dense ordered table: request 0 holds the rank block of its state, request 1 a slot of the dense table (the
+      // state's own, or the next of its rank block's leftovers)
+      static_assert(ORD, "the dense ordered table uses the ordered directory");
+      const DenseOrder DO = p.dord;
+      bool live0 = false, live1 = false;
+      uint64_t want0 = 0, want1 = 0;
+      double c0 = 0.0, c1 = 0.0;
+      uint32_t bits0 = 0, s1 = 0, end1 = 0;
+      uint64_t A0 = 0, A1 = 0, A2 = 0, A3 = 0, k1 = 0;
+      E v1 = zero;
+      auto request1 = [&]() {   // ask for slot s1
+        if (p.rows_l2 == 0) slot_load<CE>(dense, s1, k1, v1);
+        else if (s1 - near_lo < near_span) slot_load<CE, true>(dense, s1, k1, v1, near_policy);
+        else slot_load<CE, true>(dense, s1, k1, v1, far_policy);
+      };
+      for (;;) {
+        while (valid && rt.mask == 0 && 64 * (w + 1) < p.n_groups) {
+          ++w;
+          rt = row_terms<false>(T, w, 64 * w, min(64 * w + 64, p.n_groups), b);
+        }
+        const bool has = rt.mask != 0;
+        if (!has && !live0 && !live1) break;
+        // ---- consume request 1
+        if (live1) {
+          if (k1 == want1) {
+            axpy(acc, c1, v1);
+          } else if (s1 + 1 < end1) {   // a leftover of the rank block that is not this state: the next one; request 0
+            ++s1;                       // and the row wait one trip
+            request1();
+            continue;
+          } else if (c1 != 0.0) {       // the slot belongs to another state: not in the basis (DMV:115-118)
+            ++bad; bad_state = want1;
+          }
+        }
+        // ---- request 0 -> request 1: the slot from the rank block
+        live1 = false;
+        if (live0) {
+          want1 = want0; c1 = c0;
+          s1 = dord_slot(A0, A1, A2, A3, bits0, end1);
+          if (s1 < end1) {
+            request1();
+            live1 = true;
+          } else if (c1 != 0.0) {       // not placed and the rank block has no leftovers: not in the basis
+            ++bad; bad_state = want1;
+          }
+        }
+        // ---- a new request 0: the next term of the row
+        live0 = has;
+        if (has) {
+          uint64_t flip;
+          const uint64_t flip_t = TK > 0 ? sgxt[64 * w + __ffsll((long long)rt.mask) - 1] : 0ull;
+          c0 = pop_term<false>(T, rt, 64 * w, b, any_s_out, flip);
+          const uint64_t raw = b ^ flip;
+          if constexpr (TK > 0) want0 = orbit_min_torus_sq_t<TK>(orbit, raw, bt ^ flip_t);
+          else want0 = orbit_representative(orbit, raw);
+          const uint64_t h = dord_hash(want0);
+          const uint32_t blk = ordered_block(want0, p.table_dir.k_lo, p.table_dir.shift, p.table_dir.last);
+          const unsigned char *q = reinterpret_cast<const unsigned char *>(DO.blocks) +
+                                   (size_t)dord_block(h, sdir[blk], sdir[blk + 1]) * 32;
+          bits0 = dord_bits(h);
+          if (p.rows_l2 == 0) load256(q, A0, A1, A2, A3);
+          else load256_hint(q, near_policy, A0, A1, A2, A3);
+        }
+      }
+    } else if constexpr (MPH) {
       // ---- dense index: request 0 holds the two perfect-hash blocks of its state (L2 hits), request 1 the slot of
       // the dense table (or, for the few states the two levels could not place, a bucket of the open-addressing table)
       bool live0 = false, live1 = false, in_table1 = false;
@@ -1671,7 +1761,8 @@ int planned_grid(int64_t rows, int row_split) {   // grid of the planned launche
 // 6x6 square (31.1 / 31.5 ms against 31.5 ms, complex128) and lose on chain_36_symm (79.4 ms against 71.3)
 void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  const int k = rows_torus_k(p.orbit, p.dense != nullptr, p.rows_ctas);
+  const bool mph = p.dense != nullptr && p.dord.blocks == nullptr;
+  const int k = rows_torus_k(p.orbit, mph, p.rows_ctas);
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
   auto launch = [&](auto kernel, bool ord, int tk) {
     const size_t smem = rows_smem(p, L, ord, tk).total;
@@ -1681,13 +1772,17 @@ void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stre
   };
   with_bool(complex_elements, [&](auto ce) {
     with_choice<6, 4, 0>(k, [&](auto tk) {
-      if (p.dense != nullptr) {   // the dense index (perfect hash) is built for two CTAs per SM and the hashed layout only
+      if (mph) {   // the dense index (perfect hash) is built for two CTAs per SM and the hashed layout only
         launch(k_rows<ce(), tk(), true, 2, false>, false, tk());
         return;
       }
       with_choice<2, 3, 4>(p.rows_ctas, [&](auto ctas) {
+        constexpr int TK = ctas() == 4 && tk() == 4 ? 0 : tk();   // no 4x4 build at 64 registers (see rows_torus_k)
+        if (p.dord.blocks != nullptr) {   // the dense ordered table (on the ordered layout's directory)
+          launch(k_rows<ce(), TK, false, ctas(), true, true>, true, TK);
+          return;
+        }
         with_bool(p.table_dir.dir != nullptr, [&](auto ord) {   // the ordered table layout
-          constexpr int TK = ctas() == 4 && tk() == 4 ? 0 : tk();   // no 4x4 build at 64 registers (see rows_torus_k)
           launch(k_rows<ce(), TK, false, ctas(), ord()>, ord(), TK);
         });
       });

@@ -153,6 +153,8 @@ struct PmArgs {
   const unsigned char *table;   // PM_TABLE: k_rows' table (table_slot / ordered layout), filled from x
   uint32_t table_slots;
   OrderedDir table_dir;
+  DenseOrder dord;              // ... or the dense ordered table (blocks not null), its slots in `dense`
+  const unsigned char *dense;
   const int16_t *class_of;   // [N * N]: class of the ordered pair (i, j), -1 on the diagonal
   const uint16_t *pairs;     // pair-major walk: the unordered pairs i | j << 8
   int n_sites, n_pairs, c_lo, c_hi;   // classes [c_lo, c_hi) of this pass
@@ -186,6 +188,21 @@ __device__ __forceinline__ double2 pm_target(const PmArgs &A, uint64_t a, unsign
     }
   }
   if constexpr (LOOK == PM_TABLE) {
+    if (A.dord.blocks != nullptr) {   // dense ordered table: the rank block, then the slot (or the block's leftovers)
+      const uint64_t h = dord_hash(key);
+      const uint32_t p = ordered_block(key, A.table_dir.k_lo, A.table_dir.shift, A.table_dir.last);
+      const uint64_t *w = A.dord.blocks + 4 * (size_t)dord_block(h, __ldg(A.table_dir.dir + p), __ldg(A.table_dir.dir + p + 1));
+      uint32_t end = 0;
+      for (uint32_t s = dord_slot(__ldg(w), __ldg(w + 1), __ldg(w + 2), __ldg(w + 3), dord_bits(h), end); s < end; ++s) {
+        const size_t width = CE ? 32 : 16;
+        const ulonglong2 kv = __ldg(reinterpret_cast<const ulonglong2 *>(A.dense + s * width));
+        if (kv.x != key) continue;
+        if (CE) return __ldg(reinterpret_cast<const double2 *>(A.dense + s * width + 16));
+        return make_double2(__longlong_as_double((long long)kv.y), 0.0);
+      }
+      ++bad; bad_state = key;
+      return make_double2(0.0, 0.0);
+    }
     uint32_t bk = table_home(key, A.table_slots, A.table_dir);
     for (;;) {
       const ulonglong2 k = __ldg(reinterpret_cast<const ulonglong2 *>(A.table + (size_t)bk * 32));
@@ -581,6 +598,8 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
     A.table = basis->d_table.ptr;
     A.table_slots = basis->table_slots;
     A.table_dir = basis->table_dir;
+    A.dord = basis->dord;
+    A.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
   }
   const size_t gram_size = zz_gram_size(N);
   double *d_gram = run.scalars(gram_size + 2 * (size_t)count), *d_sums = d_gram + gram_size;
@@ -592,7 +611,7 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
     A.x = P > 1 ? gather_x(ctx, elt, xv) : xv;
     if (look == PM_TABLE)
       launch_table_fill(basis->n_states, run.ce, A.x, basis->d_norms.ptr, A.pos, basis->d_slot_of.ptr,
-                        basis->d_reps.ptr, basis->d_table.ptr, nullptr, st);
+                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
     pm_sums(run, A, count, look, tk, cplx, d_sums);
     run.all_reduce(d_sums, 2 * (size_t)count);
     CUDA_CHECK(cudaMemcpyAsync(sums.data(), d_sums, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));

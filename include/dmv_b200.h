@@ -88,10 +88,17 @@ int dmv_synchronize(dmv_context *ctx);
  *                        states always use hashed homes)
  *          "rows_table_bits" = 1 .. 14 (default 14): the ordered layout's directory has at most 2^bits blocks
  *          "rows_table_buckets" = 2 | 4 | 8 (default 8): complex128 buckets per state of the ordered layout
- *          "rows_l2" = 0 | 1 | 2 (default): L2 eviction priority of k_rows' accesses on the ordered layout, per
- *                        instruction (nothing device-wide is set).  1: evict_first for the buckets farther than
- *                        "rows_l2_window" = 0 .. 32 (default 16) MB of table from the row's own place, and for the row's
- *                        state, norm, x and y; 2: and evict_last for the nearer buckets; 0: none.  y does not depend on it
+ *          "rows_dense_order" = -1 auto (on wherever "rows_table" = 1) | 0 off | 1 on: instead of the ordered layout, the
+ *                        dense ordered table -- one slot per state in key order at the granularity of the ordered
+ *                        layout's blocks ("rows_table_bits"), found through a perfect hash per rank block of 40 states
+ *                        (32 bytes each, L2-resident); "rows_index" = 1 takes precedence.  Info: "rows_dense_order_on"
+ *                        whether it is built, "rows_dense_order_placed" the states its hash levels place ("rows_dense"
+ *                        counts the states of the perfect-hash index only)
+ *          "rows_l2" = 0 | 1 | 2 (default): L2 eviction priority of k_rows' accesses on the ordered layouts, per
+ *                        instruction (nothing device-wide is set).  1: evict_first for the buckets / slots farther than
+ *                        "rows_l2_window" = 0 .. 32 (default 2) MB of table from the row's own place, and for the row's
+ *                        state, norm, x and y; 2: and evict_last for the nearer buckets / slots and the dense ordered
+ *                        table's rank blocks; 0: none.  y does not depend on it
  *          "rows_ctas" = 2 (default) | 3 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread
  *                        122 | 80 | 64; at 80 and 64 words of the pipeline state spill, and on an H100 the extra warps do
  *                        not pay for it)
@@ -399,7 +406,12 @@ void ls_chpl_enumerate_representatives(const void *ls_hs_basis_ptr, uint64_t low
  * dmv_debug_ordered_table: builds the ordered layout of the k_rows table (complex128: one-slot buckets,
  *   `buckets_per_state` per state, at most 2^bits blocks) over the `n` ascending representatives `reps` with the device
  *   functions compiled for the host, inserts them in order and looks every one up again: block[k] = prefix block of
- *   reps[k], home[k] = its home bucket, probes[k] = buckets its look-up reads.  Fails when a state is not found. */
+ *   reps[k], home[k] = its home bucket, probes[k] = buckets its look-up reads.  Fails when a state is not found.
+ * dmv_debug_dense_order: builds the dense ordered table of k_rows (option rows_dense_order, at most 2^bits prefix blocks)
+ *   over the `n` ascending representatives with the library's host builder, and looks every one up again with the
+ *   device functions compiled for the host: block[k] = prefix block of reps[k], slot[k] = its slot, probes[k] = slots
+ *   its look-up reads; info[0] = states the two perfect-hash levels place, info[1] = rank blocks.  Fails when two
+ *   states share a slot or a state is not found. */
 int dmv_debug_tridiagonal_lowest(int k, const double *diag, const double *offdiag, double *eigenvalue, double *vector);
 /* dmv_debug_tridiagonal_expm: host half of dmv_expm_multiply, c = exp(z T) e_1 for the symmetric tridiagonal T
  *   (diag a[0..k), off-diag b[0..k-1)), c interleaved (re, im), 2k doubles */
@@ -428,6 +440,8 @@ int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t 
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
                             uint32_t *home, uint32_t *probes);
+int dmv_debug_dense_order(const uint64_t *reps, int64_t n, int bits, uint32_t *block, uint32_t *slot, uint32_t *probes,
+                          int64_t *info);
 int dmv_debug_torus_sq_rows(const dmv_basis_desc *basis, int64_t count, const uint64_t *states, int64_t n_flips,
                             const uint64_t *flips, uint64_t *rows, uint64_t *single);
 
