@@ -204,37 +204,38 @@ void launch_push_block(const void *x, int64_t n_doubles, int num_ranks, void *co
 void launch_raise_flags(unsigned *const *peer_flags, int num_ranks, int rank, unsigned value, cudaStream_t stream);
 void launch_wait_flags(const unsigned *flags, int num_ranks, unsigned epoch, unsigned long long *status,
                        cudaStream_t stream);
-// Lanczos vector kernels (dmv_solver.cu); n = elements, words = 8-byte words
-void launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s);
-void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
-                           const double *coef2, double *out1, cudaStream_t s);
-void launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s);
-void launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s);
+// Lanczos vector kernels (dmv_solver.cu); n = elements, words = 8-byte words.  Every launcher of dmv_solver.cu but
+// launch_reduce_partials returns the CTAs of its main launch (0 when it launched nothing).
+int launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s);
+int launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
+                          const double *coef2, double *out1, cudaStream_t s);
+int launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s);
+int launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s);
 // Krylov block kernels (dmv_solver.cu, used by dmv_expm_multiply): the stored vectors travel as a kernel parameter
 constexpr int kMaxBlockVectors = 65;
 struct VecList { const double *p[kMaxBlockVectors]; };
 // CTAs of the largest block launch over n elements: `partials` must hold that many * (J + 1) * 2 doubles
 int block_partials_grid(int64_t n, bool complex_elements);
 // h[2k], h[2k + 1] = <V_k, w> for k < J (real vectors: imaginary part 0), h[2J] = |w|^2; w is read once
-void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
-                      double *h, cudaStream_t s);
+int launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
+                     double *h, cudaStream_t s);
 // out = a w - sum_{k < J} c_k V_k (c: J interleaved complex coefficients in device memory; w may be null, out may alias
 // w), nrm2[0] = |out|^2
-void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
-                          const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s);
+int launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
+                         const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s);
 // Block kernels of dmv_eigsh: W = R <= kMaxBlockRhs vectors, w_stride elements apart; V and W are read once per call.
 constexpr int kMaxBlockRhs = 6;
 // doubles the `partials` buffer of launch_block_gram / launch_block_update must hold
 size_t block_gram_partials();
 // h[2 (k R + r) + {0, 1}] = <V_k, W_r> for k < J, h[2 (J R + r R + s) + {0, 1}] = <W_r, W_s> (real vectors: imaginary 0)
-void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
-                       int R, double *partials, double *h, cudaStream_t s);
+int launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
+                      int R, double *partials, double *h, cudaStream_t s);
 // W_r -= sum_{k < J} c_{kr} V_k (c[2 (k R + r) + {0, 1}] in device memory), nrm2[2 r] = |W_r|^2 after
-void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
-                         int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s);
+int launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
+                        int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s);
 // in place V_j <- sum_{i < k} S_{ij} V_i for j < l <= k (S[2 (i l + j) + {0, 1}] in device memory); no second basis
-void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
-                         cudaStream_t s);
+int launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
+                        cudaStream_t s);
 // out[2k + {0, 1}] = sum over b < blocks of partials[(b * width + k) * 2 + {0, 1}], in a fixed order (k_reduce_partials)
 void launch_reduce_partials(int blocks, int width, const double *partials, double *out, cudaStream_t s);
 // Kernels of dmv_lanczos_quadrature (dmv_solver.cu): G <= kMaxBlockRhs recurrences, vector g at offset g n elements.
@@ -246,15 +247,15 @@ __host__ __device__ inline bool quad_breakdown(double b2_next, double dot, doubl
 // doubles the `partials` buffer of launch_quad_dot / launch_quad_update must hold for G vectors
 size_t quad_partials(int G);
 // x[g n + i] = seeded start value of vector first + g at representative reps[i], g < G
-void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
-                      double *x, cudaStream_t s);
+int launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
+                     double *x, cudaStream_t s);
 // out[2 g + {0, 1}] = <A_g, B_g> (A may equal B)
-void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
-                     double *out, cudaStream_t s);
+int launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
+                    double *out, cudaStream_t s);
 // step j: P <- r_{j+1} from P = r_{j-1}, Q = r_j, W = H r_j and the stored dot / b2 of steps j - 1 and j;
 // nrm2[2 g] = |r_{j+1}|^2
-void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
-                        const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s);
+int launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
+                       const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s);
 // Spin-spin Gram block of dmv_zz_correlations (dmv_observe.cu): gram[i * zz_gram_columns + j] = sum_b |x_b|^2 a_i s_j
 // with s_j = +-1 for bit j of reps[b] and a = (s, 1); zz_gram_size doubles (rows padded to 16, columns to 8).
 // `partials` must hold zz_gram_partials(n, n_sites) doubles.

@@ -11,7 +11,7 @@
 #include <string>
 #include <type_traits>
 
-#include "dmv_host.h"
+#include "dmv_context.h"
 
 namespace dmv {
 
@@ -615,37 +615,45 @@ int blocks_for(int64_t n) { return capped_grid(ceil_div(n, kThreads), (int64_t)s
 
 // f(std::integral_constant<int, W>) for the W = 1 .. kMaxBlockRhs vectors of a block or a group
 template <typename F>
-void with_width(int w, F &&f) {
-  with_choice<1, 2, 3, 4, 5, 6>(w, f);
+auto with_width(int w, F &&f) {
+  return with_choice<1, 2, 3, 4, 5, 6>(w, f);
 }
 
 }  // namespace
 
-void launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s) {
-  if (n <= 0) return;
-  with_bool(complex_elements, [&](auto ce) { k_dot<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, a, b, out2); });
+int launch_dot(int64_t n, bool complex_elements, const double *a, const double *b, double *out2, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int grid = blocks_for(n);
+  with_bool(complex_elements, [&](auto ce) { k_dot<ce()><<<grid, kThreads, 0, s>>>(n, a, b, out2); });
   check_launch("k_dot");
+  return grid;
 }
 
-void launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
-                           const double *coef2, double *out1, cudaStream_t s) {
-  if (n <= 0) return;
+int launch_lanczos_update(int64_t n, bool complex_elements, double *w, const double *v, const double *u,
+                          const double *coef2, double *out1, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int grid = blocks_for(complex_elements ? 2 * n : n);
   with_bool(complex_elements, [&](auto ce) {
-    k_lanczos_update<ce()><<<blocks_for(ce() ? 2 * n : n), kThreads, 0, s>>>(n, w, v, u, coef2, out1);
+    k_lanczos_update<ce()><<<grid, kThreads, 0, s>>>(n, w, v, u, coef2, out1);
   });
   check_launch("k_lanczos_update");
+  return grid;
 }
 
-void launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s) {
-  if (words <= 0) return;
-  with_bool(accumulate, [&](auto acc) { k_scale<acc()><<<blocks_for(words), kThreads, 0, s>>>(words, scale, x, y); });
+int launch_scale(int64_t words, double scale, const double *x, double *y, bool accumulate, cudaStream_t s) {
+  if (words <= 0) return 0;
+  const int grid = blocks_for(words);
+  with_bool(accumulate, [&](auto acc) { k_scale<acc()><<<grid, kThreads, 0, s>>>(words, scale, x, y); });
   check_launch("k_scale");
+  return grid;
 }
 
-void launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s) {
-  if (words <= 0) return;
-  k_fill<<<blocks_for(words), kThreads, 0, s>>>(words, seed, offset, x);
+int launch_fill(int64_t words, uint64_t seed, uint64_t offset, double *x, cudaStream_t s) {
+  if (words <= 0) return 0;
+  const int grid = blocks_for(words);
+  k_fill<<<grid, kThreads, 0, s>>>(words, seed, offset, x);
   check_launch("k_fill");
+  return grid;
 }
 
 namespace {
@@ -666,17 +674,18 @@ int block_partials_grid(int64_t n, bool complex_elements) {
   return std::max(block_dot_grid(n, complex_elements), block_combine_grid(n, complex_elements));
 }
 
-void launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
-                      double *h, cudaStream_t s) {
+int launch_block_dot(int64_t n, bool complex_elements, const VecList &V, int J, const double *w, double *partials,
+                     double *h, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_dot: bad number of vectors");
   const int grid = block_dot_grid(n, complex_elements);
   with_bool(complex_elements, [&](auto ce) { k_block_dot<ce()><<<grid, kThreads, 0, s>>>(n, V, J, w, partials); });
   check_launch("k_block_dot");
   launch_reduce_partials(grid, J + 1, partials, h, s);
+  return grid;
 }
 
-void launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
-                          const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s) {
+int launch_block_combine(int64_t n, bool complex_elements, double a, const double *w, const VecList &V, int J,
+                         const double *coef, double *out, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors) throw std::runtime_error("k_block_combine: bad number of vectors");
   const int grid = block_combine_grid(n, complex_elements);
   with_bool(complex_elements, [&](auto ce) {
@@ -684,6 +693,7 @@ void launch_block_combine(int64_t n, bool complex_elements, double a, const doub
   });
   check_launch("k_block_combine");
   launch_reduce_partials(grid, 1, partials, nrm2, s);
+  return grid;
 }
 
 size_t block_gram_partials() {
@@ -691,13 +701,13 @@ size_t block_gram_partials() {
   return (size_t)sm_count() * 8 * (kMaxBlockVectors * kMaxBlockRhs + kMaxBlockRhs * kMaxBlockRhs) * 2;
 }
 
-void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
-                       int R, double *partials, double *h, cudaStream_t s) {
+int launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J, const double *W, int64_t w_stride,
+                      int R, double *partials, double *h, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_gram: bad number of vectors");
   const int width = J * R + R * R;
-  with_bool(complex_elements, [&](auto ce) {
-    with_width(R, [&](auto r) {
+  return with_bool(complex_elements, [&](auto ce) {
+    return with_width(R, [&](auto r) {
       constexpr bool CE = ce();
       constexpr int E = gram_elems<CE, r()>();
       const size_t smem = (size_t)(kThreads / 32) * width * (CE ? 2 : 1) * sizeof(double);
@@ -705,20 +715,22 @@ void launch_block_gram(int64_t n, bool complex_elements, const VecList &V, int J
       k_block_gram<CE, r()><<<grid, kThreads, smem, s>>>(n, V, J, W, w_stride, partials);
       check_launch("k_block_gram");
       launch_reduce_partials(grid, width, partials, h, s);
+      return grid;
     });
   });
 }
 
-void launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
-                         int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s) {
+int launch_block_update(int64_t n, bool complex_elements, const VecList &V, int J, const double *coef, double *W,
+                        int64_t w_stride, int R, double *partials, double *nrm2, cudaStream_t s) {
   if (J < 0 || J > kMaxBlockVectors || R < 1 || R > kMaxBlockRhs)
     throw std::runtime_error("k_block_update: bad number of vectors");
-  with_bool(complex_elements, [&](auto ce) {
-    with_width(R, [&](auto r) {
+  return with_bool(complex_elements, [&](auto ce) {
+    return with_width(R, [&](auto r) {
       const int grid = one_wave(k_block_update<ce(), r()>, ceil_div(std::max<int64_t>(n, 0), kThreads));
       k_block_update<ce(), r()><<<grid, kThreads, 0, s>>>(n, V, J, coef, W, w_stride, partials);
       check_launch("k_block_update");
       launch_reduce_partials(grid, R, partials, nrm2, s);
+      return grid;
     });
   });
 }
@@ -728,16 +740,18 @@ void launch_reduce_partials(int blocks, int width, const double *partials, doubl
   check_launch("k_reduce_partials");
 }
 
-void launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
-                         cudaStream_t s) {
+int launch_block_rotate(int64_t n, bool complex_elements, const VecList &V, int k, int l, const double *S,
+                        cudaStream_t s) {
   if (k < 1 || k > kMaxBlockVectors || l < 1 || l > k) throw std::runtime_error("k_block_rotate: bad shape");
-  if (n <= 0) return;
+  if (n <= 0) return 0;
   const size_t smem = (size_t)k * kRotWords * sizeof(double);
-  with_bool(complex_elements, [&](auto ce) {
-    const int grid = one_wave(k_block_rotate<ce()>, ceil_div(n, ce() ? kRotWords / 2 : kRotWords), smem);
-    k_block_rotate<ce()><<<grid, kThreads, smem, s>>>(n, V, k, l, S);
+  const int grid = with_bool(complex_elements, [&](auto ce) {
+    const int g = one_wave(k_block_rotate<ce()>, ceil_div(n, ce() ? kRotWords / 2 : kRotWords), smem);
+    k_block_rotate<ce()><<<g, kThreads, smem, s>>>(n, V, k, l, S);
+    return g;
   });
   check_launch("k_block_rotate");
+  return grid;
 }
 
 size_t quad_partials(int G) {
@@ -745,39 +759,226 @@ size_t quad_partials(int G) {
   return (size_t)sm_count() * 8 * G * 2;
 }
 
-void launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
-                      double *x, cudaStream_t s) {
-  if (n <= 0) return;
+int launch_quad_fill(int64_t n, bool complex_elements, const uint64_t *reps, uint64_t seed, int first, int G,
+                     double *x, cudaStream_t s) {
+  if (n <= 0) return 0;
+  const int grid = blocks_for(n);
   with_bool(complex_elements, [&](auto ce) {
-    k_quad_fill<ce()><<<blocks_for(n), kThreads, 0, s>>>(n, reps, seed, first, G, x);
+    k_quad_fill<ce()><<<grid, kThreads, 0, s>>>(n, reps, seed, first, G, x);
   });
   check_launch("k_quad_fill");
+  return grid;
 }
 
-void launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
-                     double *out, cudaStream_t s) {
+int launch_quad_dot(int64_t n, bool complex_elements, int G, const double *A, const double *B, double *partials,
+                    double *out, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_dot: bad number of vectors");
-  with_bool(complex_elements, [&](auto ce) {
-    with_width(G, [&](auto g) {
+  return with_bool(complex_elements, [&](auto ce) {
+    return with_width(G, [&](auto g) {
       const int grid = one_wave(k_quad_dot<ce(), g()>, ceil_div(n, kThreads));
       k_quad_dot<ce(), g()><<<grid, kThreads, 0, s>>>(n, A, B, partials);
       check_launch("k_quad_dot");
       launch_reduce_partials(grid, G, partials, out, s);
+      return grid;
     });
   });
 }
 
-void launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
-                        const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s) {
+int launch_quad_update(int64_t n, bool complex_elements, int G, double *P, double *Q, const double *W,
+                       const double *dot, const double *b2, int j, double *partials, double *nrm2, cudaStream_t s) {
   if (G < 1 || G > kMaxBlockRhs) throw std::runtime_error("k_quad_update: bad number of vectors");
-  with_bool(complex_elements, [&](auto ce) {
-    with_width(G, [&](auto g) {
+  return with_bool(complex_elements, [&](auto ce) {
+    return with_width(G, [&](auto g) {
       const int grid = one_wave(k_quad_update<ce(), g()>, ceil_div(n, kThreads));
       k_quad_update<ce(), g()><<<grid, kThreads, 0, s>>>(n, P, Q, W, dot, b2, j, partials);
       check_launch("k_quad_update");
       launch_reduce_partials(grid, G, partials, nrm2, s);
+      return grid;
     });
   });
 }
 
 }  // namespace dmv
+
+// ---- dmv_debug_solver_kernel (include/dmv_b200.h): one launcher above on host data, for the tests -------------------
+
+namespace {
+
+struct PrivateStream {
+  cudaStream_t s = nullptr;
+  PrivateStream() { CUDA_CHECK(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
+  ~PrivateStream() {
+    cudaStreamSynchronize(s);
+    cudaStreamDestroy(s);
+  }
+};
+
+}  // namespace
+
+extern "C" int dmv_debug_solver_kernel(const char *kernel, int elt, int64_t n, const int64_t *args, int n_args,
+                                       double scalar, double *arena, int64_t arena_words, const double *coef,
+                                       int64_t coef_words, double *out, int64_t out_words, int *grid) {
+  API_BEGIN
+  if (grid) *grid = 0;
+  if (!kernel) throw std::runtime_error("kernel must not be null");
+  const std::string k = kernel;
+  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  if (n < 0) throw std::runtime_error(k + ": n must be >= 0");
+  if (n_args < 0 || (n_args > 0 && !args) || arena_words < 0 || (arena_words > 0 && !arena) || coef_words < 0 ||
+      (coef_words > 0 && !coef) || out_words < 0 || (out_words > 0 && !out))
+    throw std::runtime_error(k + ": bad array");
+  const bool ce = elt == DMV_C128;
+  const int64_t vec = ce ? 2 * n : n;   // words of one vector
+  auto arg = [&](int i) {
+    if (i >= n_args) throw std::runtime_error(k + ": too few arguments");
+    return args[i];
+  };
+  auto count = [&](int i) {   // a number of vectors or a step: the launchers take int
+    const int64_t v = arg(i);
+    if (v < -(1 << 20) || v > (1 << 20)) throw std::runtime_error(k + ": argument " + std::to_string(i) + " out of range");
+    return (int)v;
+  };
+  // a vector argument of `words` words at a word offset into the arena (-1: null, where the launcher takes null);
+  // complex elements load as double2, so their offsets must be even
+  auto vector = [&](int64_t off, int64_t words, bool nullable, bool pairs) {
+    if (off == -1 && nullable) return;
+    if (off < 0 || off > arena_words || words > arena_words - off)
+      throw std::runtime_error(k + ": a vector argument lies past the arena");
+    if (pairs && ce && (off & 1)) throw std::runtime_error(k + ": odd word offset for complex elements");
+  };
+  // fixed arguments, then `listed` stored-vector offsets
+  auto shape = [&](int fixed, int listed) {
+    if (n_args != fixed + std::max(listed, 0))
+      throw std::runtime_error(k + ": expects " + std::to_string(fixed) + " arguments and " +
+                               std::to_string(std::max(listed, 0)) + " vector offsets");
+    for (int i = 0; i < listed; ++i) vector(args[fixed + i], vec, false, true);
+  };
+  int64_t need_coef = 0, need_out = 0;
+  int list_at = 0, listed = 0;
+  if (k == "dot") {
+    shape(2, 0);
+    vector(arg(0), vec, false, true);
+    vector(arg(1), vec, false, true);
+    need_out = 2;
+  } else if (k == "lanczos_update") {
+    shape(3, 0);
+    vector(arg(0), vec, false, true);
+    vector(arg(1), vec, false, true);
+    vector(arg(2), vec, true, true);
+    need_coef = 2;
+    need_out = 1;
+  } else if (k == "scale" || k == "fill") {   // word kernels: n is in words
+    shape(3, 0);
+    vector(arg(0), n, false, false);
+    if (k == "scale") vector(arg(1), n, false, false);
+  } else if (k == "block_dot" || k == "block_combine") {
+    const int J = count(0), fixed = k == "block_dot" ? 2 : 3;
+    shape(fixed, J);
+    list_at = fixed, listed = J;
+    vector(arg(1), vec, k == "block_combine", true);
+    if (k == "block_combine") {
+      vector(arg(2), vec, false, true);
+      need_coef = 2 * (int64_t)std::max(J, 0);
+      need_out = 2;
+    } else {
+      need_out = 2 * ((int64_t)std::max(J, 0) + 1);
+    }
+  } else if (k == "block_gram" || k == "block_update") {
+    const int J = count(0), R = count(1);
+    shape(4, J);
+    list_at = 4, listed = J;
+    const int64_t w_stride = arg(3);
+    if (w_stride < n) throw std::runtime_error(k + ": w_stride must be at least n");
+    const int64_t Rv = std::max(R, 1), Jv = std::max(J, 0);
+    if (w_stride > (int64_t(1) << 40)) throw std::runtime_error(k + ": w_stride out of range");
+    vector(arg(2), ((Rv - 1) * w_stride + n) * (ce ? 2 : 1), false, true);
+    if (k == "block_gram") {
+      need_out = 2 * (Jv * Rv + Rv * Rv);
+    } else {
+      need_coef = 2 * Jv * Rv;
+      need_out = 2 * Rv;
+    }
+  } else if (k == "block_rotate") {
+    const int kk = count(0), l = count(1);
+    shape(2, kk);
+    list_at = 2, listed = kk;
+    need_coef = 2 * (int64_t)std::max(kk, 0) * std::max(l, 0);
+  } else if (k == "quad_fill") {
+    shape(4, 0);
+    const int G = count(3);
+    vector(arg(0), std::max(G, 0) * vec, false, true);
+    need_coef = n;   // the representatives, as uint64 bit patterns
+  } else if (k == "quad_dot" || k == "quad_update") {
+    const bool update = k == "quad_update";
+    shape(update ? 6 : 3, 0);
+    const int G = count(0);
+    const int64_t Gv = std::max(G, 0);
+    for (int i = 1; i < (update ? 4 : 3); ++i) vector(arg(i), Gv * vec, false, true);
+    if (update) {
+      const int j = count(4);
+      const int64_t b2_at = arg(5);
+      if (j < 0) throw std::runtime_error(k + ": j must be >= 0");
+      const int64_t steps = 2 * ((int64_t)j + 1) * Gv;   // dot and b2 of steps 0 .. j
+      if (b2_at < 0 || b2_at > coef_words) throw std::runtime_error(k + ": too few coefficients");
+      need_coef = std::max(steps, b2_at + steps);
+    }
+    need_out = 2 * Gv;
+  } else {
+    throw std::runtime_error("unknown kernel " + k);
+  }
+  if (coef_words < need_coef) throw std::runtime_error(k + ": too few coefficients");
+  if (out_words < need_out) throw std::runtime_error(k + ": too few outputs");
+  // the partials buffer, sized as the solvers size it (after the checks above: the sizes query the device)
+  int64_t partial_words = 0;
+  if (k == "block_dot" || k == "block_combine")
+    partial_words = (int64_t)block_partials_grid(n, ce) * (std::max((int)args[0], 0) + 1) * 2;
+  else if (k == "block_gram" || k == "block_update")
+    partial_words = (int64_t)block_gram_partials();
+  else if (k == "quad_dot" || k == "quad_update")
+    partial_words = (int64_t)quad_partials(std::max((int)args[0], 1));
+
+  PrivateStream ps;   // declared first: the buffers are freed before the stream goes
+  const cudaStream_t st = ps.s;
+  host::DevBuf<double> d_arena, d_coef, d_out, d_partials;
+  d_arena.alloc(arena_words);
+  d_coef.alloc(coef_words);
+  d_out.alloc(need_out);
+  d_partials.alloc(partial_words);
+  if (arena_words)
+    CUDA_CHECK(cudaMemcpyAsync(d_arena.ptr, arena, arena_words * 8, cudaMemcpyHostToDevice, st));
+  if (coef_words) CUDA_CHECK(cudaMemcpyAsync(d_coef.ptr, coef, coef_words * 8, cudaMemcpyHostToDevice, st));
+  // k_dot and k_lanczos_update add to their output; every other output and the partials start as NaN bytes, so a
+  // slot no CTA writes shows
+  if (k == "dot" || k == "lanczos_update")
+    CUDA_CHECK(cudaMemcpyAsync(d_out.ptr, out, need_out * 8, cudaMemcpyHostToDevice, st));
+  else if (need_out)
+    CUDA_CHECK(cudaMemsetAsync(d_out.ptr, 0xff, need_out * 8, st));
+  if (partial_words) CUDA_CHECK(cudaMemsetAsync(d_partials.ptr, 0xff, partial_words * 8, st));
+  auto at = [&](int64_t off) { return off == -1 ? nullptr : d_arena.ptr + off; };
+  VecList V{};
+  for (int i = 0; i < std::min(listed, kMaxBlockVectors); ++i) V.p[i] = at(args[list_at + i]);
+  double *const c = d_coef.ptr, *const o = d_out.ptr, *const pt = d_partials.ptr;
+  int g = 0;
+  if (k == "dot") g = launch_dot(n, ce, at(args[0]), at(args[1]), o, st);
+  else if (k == "lanczos_update") g = launch_lanczos_update(n, ce, at(args[0]), at(args[1]), at(args[2]), c, o, st);
+  else if (k == "scale") g = launch_scale(n, scalar, at(args[0]), at(args[1]), args[2] != 0, st);
+  else if (k == "fill") g = launch_fill(n, (uint64_t)args[1], (uint64_t)args[2], at(args[0]), st);
+  else if (k == "block_dot") g = launch_block_dot(n, ce, V, (int)args[0], at(args[1]), pt, o, st);
+  else if (k == "block_combine")
+    g = launch_block_combine(n, ce, scalar, at(args[1]), V, (int)args[0], c, at(args[2]), pt, o, st);
+  else if (k == "block_gram") g = launch_block_gram(n, ce, V, (int)args[0], at(args[2]), args[3], (int)args[1], pt, o, st);
+  else if (k == "block_update")
+    g = launch_block_update(n, ce, V, (int)args[0], c, at(args[2]), args[3], (int)args[1], pt, o, st);
+  else if (k == "block_rotate") g = launch_block_rotate(n, ce, V, (int)args[0], (int)args[1], c, st);
+  else if (k == "quad_fill")
+    g = launch_quad_fill(n, ce, reinterpret_cast<const uint64_t *>(c), (uint64_t)args[1], (int)args[2], (int)args[3],
+                         at(args[0]), st);
+  else if (k == "quad_dot") g = launch_quad_dot(n, ce, (int)args[0], at(args[1]), at(args[2]), pt, o, st);
+  else g = launch_quad_update(n, ce, (int)args[0], at(args[1]), at(args[2]), at(args[3]), c, c + args[5], (int)args[4],
+                              pt, o, st);
+  if (arena_words) CUDA_CHECK(cudaMemcpyAsync(arena, d_arena.ptr, arena_words * 8, cudaMemcpyDeviceToHost, st));
+  if (need_out) CUDA_CHECK(cudaMemcpyAsync(out, d_out.ptr, need_out * 8, cudaMemcpyDeviceToHost, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  if (grid) *grid = g;
+  API_END
+}

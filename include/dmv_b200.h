@@ -444,6 +444,32 @@ int dmv_debug_dense_order(const uint64_t *reps, int64_t n, int bits, uint32_t *b
                           int64_t *info);
 int dmv_debug_torus_sq_rows(const dmv_basis_desc *basis, int64_t count, const uint64_t *states, int64_t n_flips,
                             const uint64_t *flips, uint64_t *rows, uint64_t *single);
+/* dmv_debug_solver_kernel: runs one launcher of the solver vector kernels (csrc/dmv_solver.cu) on the current device
+ *   and a private stream, on host data, for the tests (needs a device, unlike the entries above).  kernel: "dot",
+ *   "lanczos_update", "scale", "fill", "block_dot", "block_combine", "block_gram", "block_update", "block_rotate",
+ *   "quad_fill", "quad_dot" or "quad_update"; elt: DMV_F64 | DMV_C128; n: elements of a vector (8-byte words for
+ *   "scale" and "fill").  Every vector argument is a word offset into `arena` (arena_words doubles), which is copied
+ *   to the device, run on, and copied back whole; offsets must be even for complex elements, -1 is null where the
+ *   launcher takes null.  args (n_args), by kernel, with the small device inputs in `coef` and the small outputs in
+ *   `out` (2 doubles per complex value):
+ *     dot            {a, b}                              out[2] += <a, b>
+ *     lanczos_update {w, v, u | -1}      coef {alpha, beta}            out[0] += |w|^2 after
+ *     scale          {x, y, accumulate}  scalar = s
+ *     fill           {x, seed, offset}
+ *     block_dot      {J, w, V_0 .. V_{J-1}}                            out: h, 2 (J + 1)
+ *     block_combine  {J, w | -1, out, V_0 .. V_{J-1}}  scalar = a, coef: c, 2 J    out: |out|^2, 2
+ *     block_gram     {J, R, W, w_stride, V_0 .. V_{J-1}}               out: h, 2 (J R + R R)
+ *     block_update   {J, R, W, w_stride, V_0 .. V_{J-1}}  coef: c, 2 J R  out: |W_r|^2, 2 R
+ *     block_rotate   {k, l, V_0 .. V_{k-1}}              coef: S, 2 k l
+ *     quad_fill      {x, seed, first, G}                 coef: n representatives (uint64 bits)
+ *     quad_dot       {G, A, B}                                         out: 2 G
+ *     quad_update    {G, P, Q, W, j, b2}   coef: dot from 0, b2 from word b2, 2 (j + 1) G each   out: |r_{j+1}|^2, 2 G
+ *   The outputs of dot and lanczos_update are read first (the kernels add to them); every other output and the
+ *   partials buffer (sized as the solvers size it) are NaN bytes before the launch.  *grid = CTAs of the main launch
+ *   (0 when the launcher launched nothing).  The launchers' own checks apply (J <= 65, 1 <= R, G <= 6, 1 <= l <= k). */
+int dmv_debug_solver_kernel(const char *kernel, int elt, int64_t n, const int64_t *args, int n_args, double scalar,
+                            double *arena, int64_t arena_words, const double *coef, int64_t coef_words, double *out,
+                            int64_t out_words, int *grid);
 
 #ifdef __cplusplus
 }
