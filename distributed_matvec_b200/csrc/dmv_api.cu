@@ -823,7 +823,7 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   const int slot_shift = basis->dense_order && elt != DMV_C128 ? 16 : 15;
   p.rows_l2_window = (uint32_t)std::min<int64_t>((int64_t)basis->opt.rows_l2_window << slot_shift, basis->table_slots);
   p.rows_l2_per_state = (uint32_t)(basis->table_slots / std::max<int64_t>(1, basis->n_states));
-  launch_rows(p, elt == DMV_C128, stream);
+  basis->rows_ctas_resident = launch_rows(p, elt == DMV_C128, stream);
 }
 
 // the same for `nv` vectors at once (single rank; x / y: nv device vectors `stride` elements apart): k_rows_batch
@@ -1005,12 +1005,12 @@ const OptionRow kOptionTable[] = {
     {"rows_batch_min", &Options::rows_batch_min, 2, 6, {}, 0, "2 .. 6 doubles per state"},
     {"rows_batch", &Options::rows_batch, -1, 1, {}, 0,
      "-1 auto / 1 k_rows_batch for batched products, 0 vector by vector"},
-    {"rows_ctas", &Options::rows_ctas, 2, 4, {}, 0, "2, 3 or 4 resident CTAs per SM of k_rows"},
+    {"rows_ctas", &Options::rows_ctas, 0, 0, {-1, 2, 3, 4}, 0, "-1 auto, 2, 3 or 4 resident CTAs per SM of k_rows"},
     {"rows_index", &Options::rows_index, -1, 1, {}, STALE_TABLE,
      "-1 auto / 0 open-addressing table, 1 dense index (perfect hash)"},
     {"rows_table", &Options::rows_table, 0, 1, {}, STALE_TABLE, "0 hashed home, 1 ordered by key prefix"},
     {"rows_table_bits", &Options::rows_table_bits, 1, 14, {}, STALE_TABLE,
-     "1 .. 14 (the directory of 2^bits blocks lives in shared memory)"},
+     "1 .. 14 (a directory of 2^bits blocks)"},
     {"rows_table_buckets", &Options::rows_table_buckets, 0, 0, {2, 4, 8}, STALE_TABLE, "2, 4 or 8 buckets per state"},
     {"rows_dense_order", &Options::rows_dense_order, -1, 1, {}, STALE_TABLE,
      "-1 auto, 0 off, 1 dense ordered table (one slot per state in key order)"},
@@ -1234,6 +1234,9 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "rows")
     return ((use_pull(ctx) && !use_gather(ctx) && use_rows(ctx)) ||
             (ctx->replicated && ctx->global && !use_gather(ctx->global) && use_rows(ctx->global))) ? 1 : 0;
+  // CTAs per SM the last k_rows launch had resident (the whole-basis twin's, for the replicated-x product); 0: none yet
+  if (key == "rows_ctas_resident")
+    return ctx->rows_ctas_resident ? ctx->rows_ctas_resident : (ctx->global ? ctx->global->rows_ctas_resident : 0);
   if (key == "rows_l2") return ctx->opt.rows_l2;
   if (key == "rows_l2_window") return ctx->opt.rows_l2_window;
   if (key == "rows_ok") return ctx->rows_ok ? 1 : 0;

@@ -149,21 +149,24 @@ struct Options {
   int bitparallel = 1;  // 0: walk the groups one by one even when the bit-parallel test applies
   int gather = -1;      // row traversal kernel: -1 auto (k_gather when it applies), 0 always the queued k_pull
   int rows = -1;        // -1 auto (k_rows when it applies), 0 the queued k_pull
-  int rows_ctas = 2;    // k_rows: resident CTAs per SM: 2 (122 registers, default) | 3 (80 registers) | 4 (64 registers)
+  // k_rows: resident CTAs per SM: -1 auto (three for the square-torus forms when three are resident, else two; see
+  // launch_rows) | 2 (106-128 registers) | 3 (80 registers) | 4 (64 registers)
+  int rows_ctas = -1;
   int gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
                         // (measured slower), 2 per-lane walk from the bottom bit (round 1)
   int gather_split = -1;  // k_gather: lanes per row, -1 auto (choose_row_split), else 1 | 2 | 4 | 8 | 16 | 32
   int rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (kept for reference:
                          // the dense table is still many times L2, so a look-up still costs a random sector)
   // layout of the open-addressing table without the dense index: 0 hashed home (table_slot), 1 ordered by key prefix
-  // (ordered_block in dmv_device.cuh; its directory of at most 2^bits blocks lives in shared memory, so bits <= 14),
+  // (ordered_block in dmv_device.cuh; its directory of at most 2^bits blocks is staged in each CTA's shared memory, so
+  // bits <= 14, and at 2^12 blocks (16 KB) three CTAs of k_rows fit an SM on the 6x6 square, see launch_rows),
   // complex128 with `buckets` one-slot buckets per state (float64: two-slot buckets, 2 per state, in both layouts).
   // Ordered, 2^14 blocks and 8 buckets per state: on an H100 (700 W, L2 flushed) 6.6 % faster than hashed on the 6x6
   // square, 3.4 % on chain_32_symm and 7.3 % on chain_36_symm (complex128), 1.7 / 0.3 / 5.5 % (float64).  With 4 or 2
   // buckets per state the extra probes of linear probing (1.17 / 1.5 per look-up against 1.07) cost more than the
   // smaller table saves: 5-15 % / 35-60 % slower (profiles/h100_rows_table_sweep*.log)
   int rows_table = 1;
-  int rows_table_bits = 14;
+  int rows_table_bits = 12;
   int rows_table_buckets = 8;
   // the dense ordered table instead (DenseOrder in dmv_device.cuh: one slot per state in key order, found through a
   // perfect hash per rank block; its directory has 2^rows_table_bits blocks): -1 auto (see dense_order_wanted), 0 off,
@@ -226,6 +229,7 @@ struct dmv_context {
   // k_rows applicability (bases with permutation symmetries, trivial characters, real bit-parallel operator) and its
   // hash table over this context's representatives (see table_slot in dmv_device.cuh)
   bool rows_ok = false;
+  int rows_ctas_resident = 0;   // CTAs per SM the last k_rows launch over this context's table had resident
   DevBuf<unsigned char> d_table;
   DevBuf<unsigned char> d_mph_blocks, d_dense;   // dense index: perfect-hash blocks, dense table of (key, value) slots
   PerfectHash mph{};

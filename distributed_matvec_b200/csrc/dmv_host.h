@@ -124,7 +124,7 @@ struct KernelParams {
   const void *dense;
   // ... or the dense ordered table (dord.blocks not null): rank blocks -> slot of `dense`, table_dir its directory
   DenseOrder dord;
-  int32_t rows_ctas;           // k_rows / k_rows_batch: resident CTAs per SM the kernel is compiled for (2 default | 3 | 4)
+  int32_t rows_ctas;           // k_rows: resident CTAs per SM the kernel is compiled for (-1 auto | 2 | 3 | 4)
   // k_rows on the ordered table: L2 eviction priorities (option rows_l2: 0 none | 1 far buckets and the row's own
   // accesses evict_first | 2 and near buckets evict_last); near = within rows_l2_window buckets of per_state * the row's rank
   // (the dense ordered table: slots of the row's rank, and its rank blocks take the near priority)
@@ -140,8 +140,9 @@ void launch_pull(const KernelParams &p, Projection proj, bool complex_values, bo
 // row traversal without queue / atomics for bit-parallel operators on unprojected or inversion-only bases
 void launch_gather(const KernelParams &p, bool inversion, bool complex_values, bool complex_elements,
                    bool narrow, bool lin, bool uniform, cudaStream_t stream);
-// k_rows applies to real operators with a bit-parallel emit test on bases with trivial characters
-void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream);
+// k_rows applies to real operators with a bit-parallel emit test on bases with trivial characters; returns the CTAs per
+// SM the launch had resident
+int launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream);
 // side of the square-torus orbit minimum k_rows is compiled for (4 | 6), 0: the generic orbit walk
 int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas);
 // hash table of k_rows: insert every state (slot_of[i] = its slot), then per product table[slot_of[i]] = x[src(i)] * norm[i]
@@ -295,14 +296,19 @@ void opt_in_smem(K kernel, size_t smem) {
       throw std::runtime_error("cannot opt in to " + std::to_string(smem) + " bytes of shared memory");
 }
 
-// one wave of resident CTAs of `kernel` (`threads` each, `smem` bytes of dynamic shared memory) over `ctas` CTAs' worth
-// of work
+// CTAs of `kernel` (`threads` each, `smem` bytes of dynamic shared memory) that are resident on one SM at once
 template <typename K>
-int one_wave(K kernel, int64_t ctas, size_t smem = 0, int threads = 32 * kWarpsPerCta) {
+int resident_ctas(K kernel, size_t smem = 0, int threads = 32 * kWarpsPerCta) {
   opt_in_smem(kernel, smem);
   int per_sm = 0;
   CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-  return capped_grid(ctas, (int64_t)sm_count() * std::max(per_sm, 1));
+  return per_sm;
+}
+
+// one wave of resident CTAs of `kernel` over `ctas` CTAs' worth of work
+template <typename K>
+int one_wave(K kernel, int64_t ctas, size_t smem = 0, int threads = 32 * kWarpsPerCta) {
+  return capped_grid(ctas, (int64_t)sm_count() * std::max(resident_ctas(kernel, smem, threads), 1));
 }
 
 // f(std::integral_constant<bool, B>) for the runtime flag b

@@ -989,8 +989,8 @@ __host__ __device__ inline RowsSmem rows_smem(const KernelParams &p, const SmemL
   return R;
 }
 
-// two CTAs per SM: the pipeline state must stay in registers (a spilled request waits for its load at once), and the
-// latency is hidden inside the lane, not by occupancy
+// CTAS resident CTAs per SM (see launch_rows): the pipeline state must stay in registers (a spilled request waits for its
+// load at once); within that, more warps per scheduler hide more of the latency the lane's pipeline leaves
 // ORD: ordered table layout (see ordered_block); its directory is staged into shared memory behind the other tables, so
 // a home costs two shared-memory reads and adds no dependent global access to the pipeline
 // DORD (with ORD): the dense ordered table (see DenseOrder); request 0 is the rank block, request 1 the slot
@@ -1115,8 +1115,13 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
           else want0 = orbit_representative(orbit, raw);
           const uint64_t h = dord_hash(want0);
           const uint32_t blk = ordered_block(want0, p.table_dir.k_lo, p.table_dir.shift, p.table_dir.last);
-          const unsigned char *q = reinterpret_cast<const unsigned char *>(DO.blocks) +
-                                   (size_t)dord_block(h, sdir[blk], sdir[blk + 1]) * 32;
+          const uint32_t rb = dord_block(h, sdir[blk], sdir[blk + 1]);
+#ifdef DMV_ROWS_ORBIT_ONLY   // measurement builds only: no look-up, wrong results on purpose (minimum and rank block stay live)
+          axpy(acc, c0, v_make((double)(rb & 7u), 0.0, (E *)nullptr));
+          live0 = false;
+          continue;
+#endif
+          const unsigned char *q = reinterpret_cast<const unsigned char *>(DO.blocks) + (size_t)rb * 32;
           bits0 = dord_bits(h);
           if (p.rows_l2 == 0) load256(q, A0, A1, A2, A3);
           else load256_hint(q, near_policy, A0, A1, A2, A3);
@@ -1756,18 +1761,24 @@ int planned_grid(int64_t rows, int row_split) {   // grid of the planned launche
   return capped_grid(((rows + rows_per_tile - 1) / rows_per_tile + kWarps - 1) / kWarps, (int64_t)sm_count() * 4);
 }
 
-// k_rows: two CTAs per SM by default (122 registers, nothing spills), three (80 registers, a few words of the pipeline
-// state spill) or four (64 registers) on request.  On an H100 (400 W, L2 flushed between products) three CTAs tie on the
-// 6x6 square (31.1 / 31.5 ms against 31.5 ms, complex128) and lose on chain_36_symm (79.4 ms against 71.3)
-void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream) {
-  if (p.row_end <= p.row_begin) return;
+// k_rows: CTAs per SM (rows_ctas) 2 (106-128 registers, nothing spills beyond a few words), 3 (80 registers) or 4 (64
+// registers).  Auto (-1) runs three with the square-torus forms, whose three-CTA builds spill no more than their two-CTA
+// ones, when the occupancy query finds three resident (the shared memory of a CTA decides: the directory of the ordered
+// table is staged in it, 16 KB at the default 2^12 blocks), and two with the generic orbit walk, whose three-CTA build
+// spills 100 bytes or more of the pipeline state.  On an H100 (700 W, L2 flushed, 6x6 square, 2^12 blocks) three CTAs take
+// 19.1 ms against 20.7 ms at two (complex128), 18.3 against 19.9 ms (float64); a three-CTA build with only two resident
+// is twice as slow as the two-CTA one.  Returns the CTAs per SM the launch had resident.
+int launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream) {
+  if (p.row_end <= p.row_begin) return 0;
   const bool mph = p.dense != nullptr && p.dord.blocks == nullptr;
   const int k = rows_torus_k(p.orbit, mph, p.rows_ctas);
   const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
+  const int64_t work = ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps;
+  int resident = 0;
   auto launch = [&](auto kernel, bool ord, int tk) {
     const size_t smem = rows_smem(p, L, ord, tk).total;
-    const int grid = one_wave(kernel, ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps, smem);
-    kernel<<<grid, kThreads, smem, stream>>>(p);
+    resident = resident_ctas(kernel, smem);
+    kernel<<<capped_grid(work, (int64_t)sm_count() * std::max(resident, 1)), kThreads, smem, stream>>>(p);
     check_launch("k_rows");
   };
   with_bool(complex_elements, [&](auto ce) {
@@ -1776,18 +1787,23 @@ void launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stre
         launch(k_rows<ce(), tk(), true, 2, false>, false, tk());
         return;
       }
-      with_choice<2, 3, 4>(p.rows_ctas, [&](auto ctas) {
+      const bool ord = p.table_dir.dir != nullptr;   // the ordered layout, or the dense ordered table on its directory
+      auto kernel_at = [&](auto ctas) {               // the build of k_rows for p's table at `ctas` CTAs per SM
         constexpr int TK = ctas() == 4 && tk() == 4 ? 0 : tk();   // no 4x4 build at 64 registers (see rows_torus_k)
-        if (p.dord.blocks != nullptr) {   // the dense ordered table (on the ordered layout's directory)
-          launch(k_rows<ce(), TK, false, ctas(), true, true>, true, TK);
-          return;
-        }
-        with_bool(p.table_dir.dir != nullptr, [&](auto ord) {   // the ordered table layout
-          launch(k_rows<ce(), TK, false, ctas(), ord()>, ord(), TK);
-        });
+        if (p.dord.blocks != nullptr) return k_rows<ce(), TK, false, ctas(), true, true>;
+        return ord ? k_rows<ce(), TK, false, ctas(), true> : k_rows<ce(), TK, false, ctas(), false>;
+      };
+      int ctas = p.rows_ctas;
+      if (ctas < 0) {
+        const size_t smem = rows_smem(p, L, ord, tk()).total;
+        ctas = tk() > 0 && resident_ctas(kernel_at(std::integral_constant<int, 3>{}), smem) >= 3 ? 3 : 2;
+      }
+      with_choice<2, 3, 4>(ctas, [&](auto c) {
+        launch(kernel_at(c), ord, c() == 4 && tk() == 4 ? 0 : tk());
       });
     });
   });
+  return resident;
 }
 
 int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {

@@ -86,7 +86,9 @@ int dmv_synchronize(dmv_context *ctx);
  *          "rows_table" = 1 (default) open-addressing table of k_rows laid out by key prefix, so that the look-ups of
  *                        neighbouring rows share L2 | 0 homes hashed over the whole table (the perfect hash's leftover
  *                        states always use hashed homes)
- *          "rows_table_bits" = 1 .. 14 (default 14): the ordered layout's directory has at most 2^bits blocks
+ *          "rows_table_bits" = 1 .. 14 (default 12): the ordered layout's directory has at most 2^bits blocks (4 bytes
+ *                        each, staged in the shared memory of every CTA of k_rows: at 2^14 only two CTAs fit an SM on
+ *                        the 6x6 square)
  *          "rows_table_buckets" = 2 | 4 | 8 (default 8): complex128 buckets per state of the ordered layout
  *          "rows_dense_order" = -1 auto (on wherever "rows_table" = 1) | 0 off | 1 on: instead of the ordered layout, the
  *                        dense ordered table -- one slot per state in key order at the granularity of the ordered
@@ -99,9 +101,12 @@ int dmv_synchronize(dmv_context *ctx);
  *                        "rows_l2_window" = 0 .. 32 (default 2) MB of table from the row's own place, and for the row's
  *                        state, norm, x and y; 2: and evict_last for the nearer buckets / slots and the dense ordered
  *                        table's rank blocks; 0: none.  y does not depend on it
- *          "rows_ctas" = 2 (default) | 3 | 4 resident CTAs per SM of k_rows (k_rows_batch: always 2) (registers per thread
- *                        122 | 80 | 64; at 80 and 64 words of the pipeline state spill, and on an H100 the extra warps do
- *                        not pay for it)
+ *          "rows_ctas" = -1 auto (default) | 2 | 3 | 4 CTAs per SM k_rows is compiled for (k_rows_batch and the perfect-hash
+ *                        index: always 2) (registers per thread 106-128 | 80 | 64).  Auto: 3 with the square-torus
+ *                        forms of the orbit minimum, whose 3-CTA builds spill nothing more, when the occupancy query
+ *                        finds 3 resident, else 2; 2 with the generic orbit walk, whose 3-CTA build spills ~100 bytes of
+ *                        the pipeline state.  Info "rows_ctas_resident": the CTAs per SM the last k_rows launch had
+ *                        resident (a build for more CTAs than fit runs with fewer, and slower)
  *          "rows_batch" = -1 auto, 1: dmv_matvec_batch on bases with permutation symmetries takes up to six doubles per
  *                        state (six real / three complex vectors) through k_rows_batch | 0 vector by vector;
  *                        "rows_batch_min" = doubles per state (vectors x element width, default 2) from which it is used

@@ -2,9 +2,11 @@
 """Time k_rows with the hashed and the ordered layout of its look-up table (rows_table = 0 / 1), the ordered one at
 several directory sizes (rows_table_bits) and, for complex128, buckets per state (rows_table_buckets), each ordered
 configuration with every asked L2 eviction mode (rows_l2) and window (rows_l2_window, MB; modes other than 0), and the
-dense ordered table (rows_dense_order = 1: one slot per state in key order) at 2^14 blocks with every asked L2 mode and
-window (--dense-windows).  The configurations alternate in rounds; each product is timed with CUDA events, the L2 flushed before it, and every
-configuration's y is compared with the hashed layout's by the element criterion of bench.py.
+dense ordered table (rows_dense_order = 1: one slot per state in key order) at every asked directory size (--dense-bits)
+with every asked L2 mode and window (--dense-windows); every configuration at every asked number of CTAs per SM of
+k_rows (--ctas: rows_ctas, -1 auto), with the CTAs the launch had resident.  The configurations alternate in rounds; each
+product is timed with CUDA events, the L2 flushed before it, and every configuration's y is compared with the first's
+(the hashed layout's unless --no-hashed) by the element criterion of bench.py.
 Usage: python tools/rows_table_sweep.py [--rounds R] [--products K] [workload ...]"""
 import argparse
 import os
@@ -31,11 +33,15 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--products", type=int, default=6, help="timed products per configuration and round")
     ap.add_argument("--dtypes", default="c128,f64")
-    ap.add_argument("--bits", default="10,12,14", help="directory sizes of the ordered layout (rows_table_bits)")
+    ap.add_argument("--bits", default="10,12,14", help="directory sizes of the ordered layout (rows_table_bits; empty: not timed)")
     ap.add_argument("--buckets", default="2,4,8", help="complex128 buckets per state of the ordered layout")
     ap.add_argument("--l2", default="0", help="L2 eviction modes of the ordered layout (rows_l2)")
     ap.add_argument("--l2-window", default="16", help="near windows in MB of table (rows_l2_window)")
     ap.add_argument("--dense-windows", default="", help="near windows in MB of the dense ordered table (empty: not timed)")
+    ap.add_argument("--dense-bits", default="14", help="directory sizes of the dense ordered table (rows_table_bits)")
+    ap.add_argument("--no-hashed", action="store_true",
+                    help="leave the hashed layout out: the first configuration is then the reference of times and y")
+    ap.add_argument("--ctas", default="2", help="CTAs per SM of k_rows (rows_ctas; -1: auto)")
     ap.add_argument("workloads", nargs="*", default=["heisenberg_square_6x6", "heisenberg_chain_32_symm",
                                                      "heisenberg_chain_36_symm"])
     args = ap.parse_args()
@@ -57,21 +63,26 @@ def main():
             xd = torch.from_numpy(x).cuda()
             yd = torch.zeros_like(xd)
             # (float64: two-slot buckets, 2 per state in both layouts)
-            configs = [("hashed", 0, 14, 8, 0, 0, 0)] + [
+            tables = ([] if args.no_hashed else [("hashed", 0, 14, 8, 0, 0, 0)]) + [
                 (f"ordered D={d} b={b} l2={m}" + (f" W={w}" if m != "0" else ""), 1, int(d), int(b), int(m), int(w), 0)
-                for d in args.bits.split(",")
+                for d in args.bits.split(",") if d
                 for b in (args.buckets.split(",") if cplx else ["2"])
                 for m in args.l2.split(",")
                 for w in (args.l2_window.split(",") if m != "0" else ["0"])] + [
-                (f"dense D=14 l2={m}" + (f" W={w}" if m != "0" else ""), 1, 14, 8, int(m), int(w), 1)
+                (f"dense D={d} l2={m}" + (f" W={w}" if m != "0" else ""), 1, int(d), 8, int(m), int(w), 1)
+                for d in args.dense_bits.split(",")
                 for m in args.l2.split(",") if args.dense_windows
                 for w in (args.dense_windows.split(",") if m != "0" else ["0"])]
+            ctas_list = [int(c) for c in args.ctas.split(",")]
+            configs = [(c[0] + (f" ctas={k}" if len(ctas_list) > 1 else ""), *c[1:], k) for c in tables for k in ctas_list]
             times = {c[0]: [] for c in configs}
             worst = {c[0]: 0.0 for c in configs}
             ref = None
             placed = {}
+            resident = {}
             for _ in range(args.rounds):
-                for label, table, bits, buckets, l2, window, dense in configs:
+                for label, table, bits, buckets, l2, window, dense, ctas in configs:
+                    op.set_option("rows_ctas", ctas)
                     op.set_option("rows_dense_order", dense)
                     op.set_option("rows_l2", l2)
                     op.set_option("rows_l2_window", window)
@@ -83,6 +94,7 @@ def main():
                     torch.cuda.synchronize()
                     assert op.info("rows") == 1, "k_rows does not apply"
                     assert op.info("rows_dense_order_on") == dense
+                    resident[label] = op.info("rows_ctas_resident")
                     if dense and label not in placed:
                         placed[label] = op.info("rows_dense_order_placed")
                     for k in range(args.products):
@@ -101,14 +113,15 @@ def main():
                     bound = torch.clamp(1e-12 * torch.maximum(yd.abs(), ref.abs()), min=1e-14)
                     bad = int((diff > bound).sum())
                     if bad:
-                        raise SystemExit(f"{label}: {bad} elements differ from the hashed layout")
+                        raise SystemExit(f"{label}: {bad} elements differ from {configs[0][0]}")
                     worst[label] = max(worst[label], float(diff.max() / ref.abs().max()))
-            base = float(np.median(times["hashed"]))
+            base = float(np.median(times[configs[0][0]]))
             for label, *_ in configs:
                 t = np.array(times[label])
                 med = float(np.median(t))
                 print(f"  {dt:4s} {label:30s} median {med:8.3f} ms  min {t.min():8.3f}  max {t.max():8.3f}  "
-                      f"({len(t)} products)  vs hashed {100 * (med / base - 1):+6.1f} %  max rel diff {worst[label]:.1e}"
+                      f"({len(t)} products)  vs first {100 * (med / base - 1):+6.1f} %  max rel diff {worst[label]:.1e}"
+                      f"  resident CTAs/SM {resident[label]}"
                       + (f"  placed {placed[label]} of {n} ({n - placed[label]} left over)" if label in placed else ""),
                       flush=True)
         op.close()
