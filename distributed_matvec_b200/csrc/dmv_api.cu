@@ -154,6 +154,11 @@ bool use_gather(const dmv_context *ctx) {   // the lean row-gather kernel applie
 bool use_rows(const dmv_context *ctx) {   // the pipelined row kernel for bases with permutation symmetries
   return ctx->rows_ok && ctx->opt.rows != 0 && ctx->opt.bitparallel != 0 && ctx->orbit.trivial_characters;
 }
+// At 64 sites every 64-bit key is a state, ~0 (kEmptyKey, the free-slot marker of the open-addressing tables) included:
+// a look-up of ~0 would "hit" a free slot, and k_table_insert cannot claim one for it.  Such bases take the dense ordered
+// table, whose slots are all occupied and compared by key only, and products vector by vector instead of k_rows_batch.
+bool open_addressing_ok(const dmv_context *ctx) { return ctx->n_sites < 64; }
+bool use_rows_batch(const dmv_context *ctx) { return use_rows(ctx) && ctx->opt.rows_batch != 0 && open_addressing_ok(ctx); }
 bool use_pull(const dmv_context *ctx) {
   // auto: one rank, bit-parallel operator, no permutation symmetries -> k_gather (rows, no atomics, see
   // dmv_gather.cu); everything else -> push (k_generate).  "mode" = 1 forces the row traversal (k_gather
@@ -588,6 +593,7 @@ void do_plan(dmv_context *ctx) {
 
 // whether k_rows looks its targets up in the dense ordered table (option rows_dense_order; the perfect-hash index wins)
 bool dense_order_wanted(const dmv_context *ctx) {
+  if (!open_addressing_ok(ctx)) return true;   // whatever the options: see open_addressing_ok
   if (ctx->opt.rows_index == 1) return false;
   if (ctx->opt.rows_dense_order >= 0) return ctx->opt.rows_dense_order == 1;
   // auto: in place of the ordered layout, which it beats on every measured workload (one H100 at 700 W, L2 flushed,
@@ -1315,6 +1321,13 @@ int dmv_basis_build(dmv_context *ctx) {
   }
   const uint64_t first_rank = fixed ? fixed_hamming_rank(lo) : lo;
   const uint64_t last_rank = fixed ? fixed_hamming_rank(hi) : hi;
+  // every candidate is tested, in chunks of at most 4096 whose bounds are kept on the host: 2^40 candidates take 2^28
+  // chunks (4 GB of bounds).  A wider range -- 2^64 at 64 sites without a fixed magnetisation, where the count below
+  // wraps to 0 -- cannot be enumerated this way.
+  if (last_rank - first_rank >= (1ull << 40))
+    throw std::runtime_error("basis build: the candidate range holds more than 2^40 states (" + std::to_string(n) +
+                             " sites" + (fixed ? ", hamming weight " + std::to_string(w) : std::string(", free magnetisation")) +
+                             ") and cannot be enumerated");
   const uint64_t total = last_rank - first_rank + 1;
   uint64_t chunk_len = total / (132ull * 128 * 16);
   chunk_len = std::min<uint64_t>(std::max<uint64_t>(chunk_len, 64), 4096);
@@ -1536,7 +1549,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
                     ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);
     }
   }
-  if (ctx->num_ranks == 1 && use_pull(ctx) && !use_gather(ctx) && use_rows(ctx) && ctx->opt.rows_batch != 0 &&
+  if (ctx->num_ranks == 1 && use_pull(ctx) && !use_gather(ctx) && use_rows_batch(ctx) &&
       is_device_pointer(x) == is_device_pointer(y)) {
     // bases with permutation symmetries: up to six doubles per state share one orbit minimum and one look-up per term
     // (host vectors -- what PRIMME hands over -- are staged a batch at a time)

@@ -378,6 +378,8 @@ namespace dmv { namespace host {
 
 bool use_gather(const dmv_context *ctx);
 bool use_rows(const dmv_context *ctx);
+bool open_addressing_ok(const dmv_context *ctx);
+bool use_rows_batch(const dmv_context *ctx);
 bool use_pull(const dmv_context *ctx);
 void use_device(const dmv_context *ctx);
 bool complex_values(const dmv_context *ctx, int elt);

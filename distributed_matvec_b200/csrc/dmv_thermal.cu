@@ -28,7 +28,7 @@ int dmv_lanczos_quadrature(dmv_context *ctx, int elt, int num_vectors, int steps
   // on k_rows_batch, else one
   int width = 1;
   if (P == 1 && use_pull(ctx) && use_gather(ctx)) width = 4;
-  else if (P == 1 && use_pull(ctx) && use_rows(ctx) && ctx->opt.rows_batch != 0) width = kMaxBlockRhs / elt;
+  else if (P == 1 && use_pull(ctx) && use_rows_batch(ctx)) width = kMaxBlockRhs / elt;
   const int G = std::min(width, num_vectors);
   double *partials = run.partials(quad_partials(G));
   // steps cap at the GLOBAL dimension (every rank takes the same decision, as dmv_lanczos)
