@@ -176,6 +176,10 @@ int gather_row_split(const dmv_context *g, int64_t rows) {
   if (g->opt.gather_split > 0) return g->opt.gather_split;
   return choose_row_split(rows, (int)g->h_pull.groups.size());
 }
+int push_row_split(const dmv_context *ctx) {
+  if (ctx->opt.push_split > 0) return ctx->opt.push_split;
+  return choose_row_split(ctx->n_states, (int)ctx->h_push.groups.size());
+}
 
 KernelParams base_params(dmv_context *ctx) {
   KernelParams p{};
@@ -536,7 +540,7 @@ void do_plan(dmv_context *ctx) {
   require_states(ctx);
   const int P = ctx->num_ranks;
   const bool exact_regions = P <= 32;
-  ctx->row_split = choose_row_split(ctx->n_states, (int)ctx->h_push.groups.size());
+  ctx->row_split = push_row_split(ctx);
   ctx->plan_grid = planned_grid(ctx->n_states, ctx->row_split);
   const size_t n_warps = (size_t)ctx->plan_grid * kWarpsPerCta;
   ctx->d_out_count.alloc(P);
@@ -1029,6 +1033,8 @@ const OptionRow kOptionTable[] = {
      "0 per-lane from the top bit, 1 group-major, 2 per-lane from the bottom bit"},
     {"gather_split", &Options::gather_split, 0, 0, {-1, 1, 2, 4, 8, 16, 32}, 0,
      "-1 auto, else 1, 2, 4, 8, 16 or 32 lanes per row of k_gather"},
+    {"push_split", &Options::push_split, 0, 0, {-1, 1, 2, 4, 8, 16, 32}, STALE_PLAN,
+     "-1 auto, else 1, 2, 4, 8, 16 or 32 lanes per source state of k_generate"},
     {"peer_gather", &Options::peer_gather, -1, 0, {}, STALE_EXCHANGE, "-1 auto, 0 NCCL all-gather of x"},
     {"rows", &Options::rows, -1, 0, {}, 0, "-1 auto, 0 off (queued k_pull / k_generate for symmetric bases)"},
     {"canon", &Options::canon, -1, 2, {}, STALE_ORBIT,
@@ -1226,6 +1232,7 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "gather_narrow") return ctx->gather_narrow ? 1 : 0;
   if (key == "gather_uniform") return ctx->gather_uniform ? 1 : 0;
   if (key == "gather_split") return gather_row_split(ctx, ctx->n_states);
+  if (key == "push_split") return ctx->rounds.ready ? 1 : push_row_split(ctx);   // (the rounds always run S = 1)
   if (key == "peer_direct") return ctx->peer_direct ? 1 : 0;
   if (key == "replicated") return ctx->replicated ? 1 : 0;
   if (key == "replicated_block") return ctx->repl_block;
@@ -1443,7 +1450,8 @@ int dmv_generate(dmv_context *ctx, int elt, const void *x, void *y) {
   use_device(ctx);
   require_states(ctx);
   if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
-  if (!is_device_pointer(x) || !is_device_pointer(y))
+  // (a rank that owns no state has empty vectors, whose pointers may be null: it still plans and routes nothing)
+  if (ctx->n_states > 0 && (!is_device_pointer(x) || !is_device_pointer(y)))
     throw std::runtime_error("dmv_generate needs device pointers (y is accumulated into by later steps)");
   do_generate(ctx, elt, x, y);
   check_status(ctx);
@@ -1465,7 +1473,8 @@ int dmv_accumulate(dmv_context *ctx, int elt, int64_t count, const uint64_t *bet
   API_BEGIN
   use_device(ctx);
   require_states(ctx);
-  if (!is_device_pointer(y)) throw std::runtime_error("dmv_accumulate needs a device y");
+  // a rank without states may still be sent records of states of norm zero (dropped), with an empty, possibly null y
+  if (ctx->n_states > 0 && !is_device_pointer(y)) throw std::runtime_error("dmv_accumulate needs a device y");
   const int width = complex_values(ctx, elt) ? 2 : 1;
   InArg<uint64_t> b(betas, (size_t)count, ctx->stream);
   InArg<double> c(coeffs, (size_t)count * width, ctx->stream);

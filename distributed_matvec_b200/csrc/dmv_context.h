@@ -155,6 +155,9 @@ struct Options {
   int gather_walk = 0;  // k_gather: 0 per-lane walk from the top bit (default), 1 group-major warp-uniform walk
                         // (measured slower), 2 per-lane walk from the bottom bit (round 1)
   int gather_split = -1;  // k_gather: lanes per row, -1 auto (choose_row_split), else 1 | 2 | 4 | 8 | 16 | 32
+  // k_generate and its counting pass (dmv_plan): lanes per source state, -1 auto (choose_row_split), else 1 | 2 | 4 |
+  // 8 | 16 | 32.  The plan's grid and per-warp offsets depend on it: a change re-plans.  The overlapped rounds run S = 1
+  int push_split = -1;
   int rows_index = -1;   // -1 auto / 0 open-addressing table; 1 dense index through a perfect hash (kept for reference:
                          // the dense table is still many times L2, so a look-up still costs a random sector)
   // layout of the open-addressing table without the dense index: 0 hashed home (table_slot), 1 ordered by key prefix
@@ -411,6 +414,8 @@ void upload_orbit(dmv_context *ctx);
 // lanes per row of a k_gather launch over `rows` rows with the tables of `g`: option "gather_split", else
 // choose_row_split (every k_gather launch and info("gather_split") take it from here)
 int gather_row_split(const dmv_context *g, int64_t rows);
+// lanes per source state of the planned k_generate launches (do_plan): option "push_split", else choose_row_split
+int push_row_split(const dmv_context *ctx);
 uint64_t fixed_hamming_rank(uint64_t s);
 uint64_t fixed_hamming_unrank(uint64_t r, int weight);
 void zero_y_if_diag(dmv_context *ctx, int elt, void *y);

@@ -115,6 +115,10 @@ int dmv_synchronize(dmv_context *ctx);
  *          "gather_split" = -1 auto (more lanes per row of k_gather on bases of fewer than 16 warps of rows per SM, never
  *                        more lanes than flip-mask groups) | 1, 2, 4, 8, 16 or 32 lanes per row, each walking every
  *                        S-th group.  Applies to the single, batched and replicated-x products
+ *          "push_split" = -1 auto (the same rule over the scatter tables) | 1, 2, 4, 8, 16 or 32 lanes per source state
+ *                        of k_generate, each taking every S-th flip-mask group (only slice 0 adds the diagonal).  Applies
+ *                        to the scatter product and its counting pass (dmv_plan); a change re-plans.  The overlapped
+ *                        rounds of the record exchange always run S = 1
  *          "index"    = -1 auto (identity / Lin tables / directory) | 0 directory + binary search | 2 combinadic rank
  *                        | 3 Lin tables (full fixed-Hamming bases)
  *          "bitparallel" = 1 | 0 walk the flip-mask groups one by one
@@ -130,7 +134,8 @@ int dmv_synchronize(dmv_context *ctx);
  *               "canon_mode", "torus_mode", "peer_direct", "replicated", "replicated_block", "peer_gather", "rounds",
  *               "global_states", "complex_coefficients", "quadrature_group", "rows_tk" (side of the square-torus orbit minimum k_rows is
  *               compiled for with the current options: 4 | 6, 0 the generic walk), "gather_split" (lanes per row the next
- *               single-rank k_gather launch uses), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
+ *               single-rank k_gather launch uses), "push_split" (lanes per source state the next k_generate launch and
+ *               its plan use), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
  *               context of the replicated-x product (-1 while there is none) */
 int dmv_set_option(dmv_context *ctx, const char *name, int64_t value);
 int64_t dmv_get_info(const dmv_context *ctx, const char *name);

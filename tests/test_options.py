@@ -26,6 +26,7 @@ REJECTED = {
     "rows_batch": (-2, 2), "rows_ctas": (0, 1, 5), "rows_index": (-2, 2), "rows_table": (-1, 2),
     "rows_table_bits": (0, 15), "rows_table_buckets": (1, 3, 16), "rounds": (-2, 65), "gather_walk": (-1, 3),
     "gather_split": (-2, 0, 3, 64), "peer_gather": (-2, 1), "rows": (-2, 1), "canon": (-2, 3), "bitparallel": (-1, 2),
+    "push_split": (-2, 0, 3, 64),
 }
 
 # the twin's models: k_rows (6x6 square, weight 7) and k_gather (chain of 16 sites).  Per model, each option with a
@@ -35,9 +36,10 @@ TWIN_CASES = {
     "torus_6x6_w7": [("canon", 0, {"canon_mode": 0, "rows_tk": 0}), ("bitparallel", 0, {"rows": 0}),
                      ("rows", 0, {"rows": 0}), ("rows_table", 0, {"rows": 1})],
     "chain_16": [("gather", 0, {"gather": 0}), ("index", 0, {"index_mode": INDEX_DIRECTORY}),
-                 ("gather_split", 4, {"gather_split": 4})],
+                 ("gather_split", 4, {"gather_split": 4}), ("push_split", 2, {"push_split": 2})],
 }
-DEFAULTS = {"canon": -1, "bitparallel": 1, "rows": -1, "rows_table": 1, "gather": -1, "index": -1, "gather_split": -1}
+DEFAULTS = {"canon": -1, "bitparallel": 1, "rows": -1, "rows_table": 1, "gather": -1, "index": -1, "gather_split": -1,
+            "push_split": -1}
 
 
 def _matrix(name):
@@ -67,7 +69,7 @@ def test_every_option_rejects_out_of_range_values(need_cuda):
     try:
         op.basis.build()
         x = _x(op.basis.representatives().shape[0], True)
-        keys = ("gather", "rows", "pull", "index_mode", "gather_split", "rows_tk", "canon_mode")
+        keys = ("gather", "rows", "pull", "index_mode", "gather_split", "push_split", "rows_tk", "canon_mode")
         before = {k: op.info(k) for k in keys}
         y_before = _product(op, x)
         for name, values in REJECTED.items():
