@@ -317,12 +317,30 @@ void check_status(dmv_context *ctx) {
 }
 const Binomials &binom() { static Binomials b; return b; }
 
+// whether ix finds every installed representative at its own position: index(reps[i]) == i for all i
+bool index_verified(dmv_context *ctx, const StateIndex &ix) {
+  CUDA_CHECK(cudaMemsetAsync(ctx->d_status.ptr, 0, 4 * sizeof(unsigned long long), ctx->stream));
+  launch_verify_rank(ix, ctx->d_status.ptr, ctx->stream);
+  unsigned long long bad = 0;
+  CUDA_CHECK(cudaMemcpyAsync(&bad, ctx->d_status.ptr, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
+  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
+  CUDA_CHECK(cudaMemsetAsync(ctx->d_status.ptr, 0, 4 * sizeof(unsigned long long), ctx->stream));
+  return bad == 0;
+}
+
 // Which state -> index kernel applies (the reference's per-basis `state_index_kernel`, FFI:90-93).
 //   auto (-1): identity when it applies; two-table Lin lookup for full fixed-Hamming bases on one rank
 //   (<= 40 sites); directory search otherwise.  0 forces the directory, 2 the combinadic rank, 3 Lin.
+// Every mode but the directory is checked against the installed block, which dmv_set_representatives may have made
+// any ascending set of states: a weight sector of a free-magnetisation basis is not indexed by the identity.
 void select_index_mode(dmv_context *ctx) {
   ctx->index_mode = INDEX_DIRECTORY;
-  if (ctx->identity_index && ctx->num_ranks == 1) { ctx->index_mode = INDEX_IDENTITY; return; }
+  if (ctx->identity_index && ctx->num_ranks == 1) {
+    StateIndex ix{};
+    ix.reps = ctx->d_reps.ptr; ix.n = ctx->n_states; ix.site_mask = ctx->site_mask; ix.mode = INDEX_IDENTITY;
+    if (index_verified(ctx, ix)) ctx->index_mode = INDEX_IDENTITY;
+    return;
+  }
   const int n = ctx->n_sites, w = ctx->hamming_weight;
   const int want = ctx->opt.index;
   if (want == 0) return;
@@ -361,14 +379,8 @@ void select_index_mode(dmv_context *ctx) {
     ix.mode = INDEX_LIN; ix.lin_a = ctx->d_lin_a.ptr; ix.lin_b = ctx->d_lin_b.ptr; ix.lin_bits = lb;
   }
   ctx->rank_total = total;
-  // the block must be exactly the first `expect` fixed-weight states: index(reps[i]) == i for all i
-  CUDA_CHECK(cudaMemsetAsync(ctx->d_status.ptr, 0, 4 * sizeof(unsigned long long), ctx->stream));
-  launch_verify_rank(ix, ctx->d_status.ptr, ctx->stream);
-  unsigned long long bad = 0;
-  CUDA_CHECK(cudaMemcpyAsync(&bad, ctx->d_status.ptr, sizeof(bad), cudaMemcpyDeviceToHost, ctx->stream));
-  CUDA_CHECK(cudaStreamSynchronize(ctx->stream));
-  CUDA_CHECK(cudaMemsetAsync(ctx->d_status.ptr, 0, 4 * sizeof(unsigned long long), ctx->stream));
-  if (bad == 0) ctx->index_mode = ix.mode;
+  // the block must be exactly the first `expect` fixed-weight states
+  if (index_verified(ctx, ix)) ctx->index_mode = ix.mode;
 }
 
 void install_directory(dmv_context *ctx) {
@@ -1489,7 +1501,8 @@ int dmv_local_matvec(dmv_context *ctx, int elt, const void *x, void *y) {
   require_states(ctx);
   if (ctx->num_ranks != 1) throw std::runtime_error("dmv_local_matvec needs num_ranks == 1; use dmv_matvec");
   if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
-  if (x == y) throw std::runtime_error("x and y must not alias");
+  // (an empty block has empty vectors, whose pointers may both be null)
+  if (x == y && ctx->n_states > 0) throw std::runtime_error("x and y must not alias");
   VecStage v = stage_vectors(ctx, elt, x, y);
   const bool host_result = v.y_host;
   if (use_pull(ctx) && (use_gather(ctx) || use_rows(ctx)) && v.y_host && ctx->n_states >= (1 << 16)) {

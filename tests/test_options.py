@@ -24,7 +24,8 @@ P = 3
 REJECTED = {
     "mode": (-2, 2), "index": (-2, 1, 4), "exchange": (-2, 3), "gather": (-2, 1), "rows_batch_min": (1, 7),
     "rows_batch": (-2, 2), "rows_ctas": (0, 1, 5), "rows_index": (-2, 2), "rows_table": (-1, 2),
-    "rows_table_bits": (0, 15), "rows_table_buckets": (1, 3, 16), "rounds": (-2, 65), "gather_walk": (-1, 3),
+    "rows_table_bits": (0, 15), "rows_table_buckets": (1, 3, 16), "rows_dense_order": (-2, 2), "rows_l2": (-1, 3),
+    "rows_l2_window": (-1, 33), "rounds": (-2, 65), "gather_walk": (-1, 3),
     "gather_split": (-2, 0, 3, 64), "peer_gather": (-2, 1), "rows": (-2, 1), "canon": (-2, 3), "bitparallel": (-1, 2),
     "push_split": (-2, 0, 3, 64),
 }
