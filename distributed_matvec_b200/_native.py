@@ -86,6 +86,8 @@ _SIGNATURES = [
                             C.POINTER(C.c_int)]),
     ("dmv_zz_correlations", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("dmv_pm_correlations", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    ("dmv_apply_spin", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                 C.c_void_p]),
     ("dmv_lanczos_quadrature", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     ("dmv_last_timings", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_int]),
@@ -108,6 +110,8 @@ _SIGNATURES = [
     ("dmv_debug_zz_symmetrize", C.c_int, [C.POINTER(BasisDesc), C.c_void_p, C.c_void_p, C.c_void_p]),
     ("dmv_debug_pm_classes", C.c_int, [C.POINTER(BasisDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.c_double, C.c_void_p, C.c_void_p]),
+    ("dmv_debug_spin_weights", C.c_int, [C.POINTER(BasisDesc), C.POINTER(BasisDesc), C.c_int, C.c_int, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     ("dmv_debug_compile_group", C.c_int, [C.POINTER(BasisDesc), C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                           C.c_void_p]),
     ("dmv_debug_ordered_table", C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p,

@@ -351,6 +351,95 @@ void with_pm_kernel(int look, int tk, bool ce, bool cplx, F &&f) {
   });
 }
 
+// ---- one-site operators between two bases (dmv_apply_spin).  Row r of the target basis is
+//     y_r = 1 / n_t(r) sum_k K_k <r| o_k |psi>,   psi = B_s x,
+// with o_k = σ⁺_k on the set bits of r and σ⁻_k on its clear bits (the source state r ^ (1 << k)), or the diagonal
+// factor sum_k K_k s_k(r) (σᶻ) or sum_k K_k (1).  pm_target gives psi at any state of the source's sector: chi (n x)[rep]
+// with the orbit minimum and character of the source (PM_GROUP, PM_TABLE), x[index] without a group (PM_NONE), chi
+// x[index] with spin inversion alone, whose norm sqrt(1/2) is src_scale.  The host forms K (spin_weights below).
+enum SpinWalk {
+  SPIN_SELF = 0,    // σᶻ / 1: the row's own state, times c0 + sum over its set bits of k_set + over its clear bits of k_clear
+  SPIN_CLEAR = 1,   // σ⁻: the clear bits of the row (k_clear)
+  SPIN_SET = 2,     // σ⁺: the set bits (k_set)
+  SPIN_BOTH = 3,    // σ^± with spin inversion in the target group at free weight: both, each with its own coefficients
+};
+
+struct SpinArgs {
+  PmArgs src;                 // the source's look-up; its rows / classes are unused
+  const uint64_t *rows;       // this rank's rows of the target basis and their norms (null: row_norm for every row)
+  const double *row_norms;
+  double row_norm, src_scale;
+  const double *k;            // [2][N] complex: k_set, then k_clear
+  double2 c0;
+  uint64_t diag_mask;         // SPIN_SELF: the sites whose k_set / k_clear enter the row factor (0 for the identity)
+  int64_t n_rows;
+  double *y;
+};
+
+// One lane owns one row of the target basis and walks its sites; one store of y per row, no atomics.
+template <int LOOK, int TK, int WALK, bool CE>
+__global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
+  __shared__ double2 s_k[128];   // k_set [0, N), k_clear [N, 2 N)
+  const int N = A.src.n_sites;
+  for (int t = threadIdx.x; t < 2 * N; t += blockDim.x) s_k[t] = __ldg(reinterpret_cast<const double2 *>(A.k) + t);
+  __syncthreads();
+  unsigned long long bad = 0;
+  uint64_t bad_state = 0;
+  const uint64_t mask = A.src.site_mask;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.n_rows; i += (int64_t)gridDim.x * blockDim.x) {
+    const uint64_t r = __ldg(A.rows + i);
+    double2 acc = make_double2(0.0, 0.0);
+    auto add = [&](double2 k, double2 v) {
+      acc.x += k.x * v.x - (CE ? k.y * v.y : 0.0);
+      if constexpr (CE) acc.y += k.x * v.y + k.y * v.x;
+    };
+    if constexpr (WALK == SPIN_SELF) {
+      double2 c = A.c0;
+      for (uint64_t m = r & A.diag_mask; m; m &= m - 1) {
+        const double2 k = s_k[__ffsll((long long)m) - 1];
+        c.x += k.x; c.y += k.y;
+      }
+      for (uint64_t m = ~r & A.diag_mask; m; m &= m - 1) {
+        const double2 k = s_k[N + __ffsll((long long)m) - 1];
+        c.x += k.x; c.y += k.y;
+      }
+      add(c, pm_target<LOOK, TK, CE>(A.src, r, bad, bad_state));
+    } else {
+      if constexpr (WALK & SPIN_SET)
+        for (uint64_t m = r & mask; m; m &= m - 1) {
+          const int k = __ffsll((long long)m) - 1;
+          add(s_k[k], pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+        }
+      if constexpr (WALK & SPIN_CLEAR)
+        for (uint64_t m = ~r & mask; m; m &= m - 1) {
+          const int k = __ffsll((long long)m) - 1;
+          add(s_k[N + k], pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+        }
+    }
+    const double s = A.src_scale / (A.row_norms ? __ldg(A.row_norms + i) : A.row_norm);
+    if constexpr (CE) reinterpret_cast<double2 *>(A.y)[i] = make_double2(acc.x * s, acc.y * s);
+    else A.y[i] = acc.x * s;
+  }
+  if (bad && atomicAdd(A.src.status, bad) == 0) A.src.status[1] = bad_state;
+}
+
+constexpr int kSpinThreads = 256;
+
+// f(k_spin_rows<LOOK, TK, WALK, CE>); TK (the square-torus orbit minimum) only for the orbit look-ups
+template <typename F>
+void with_spin_kernel(int look, int tk, int walk, bool ce, F &&f) {
+  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
+    with_choice<SPIN_SELF, SPIN_CLEAR, SPIN_SET, SPIN_BOTH>(walk, [&](auto wk) {
+      with_bool(ce, [&](auto e) {
+        with_choice<6, 4, 0>(tk, [&](auto t) {
+          if constexpr (lk() >= PM_GROUP || t() == 0) f(k_spin_rows<lk(), t(), wk(), e()>);
+          else throw std::logic_error("k_spin_rows has no square-torus build without a group");
+        });
+      });
+    });
+  });
+}
+
 }  // namespace
 
 int zz_gram_columns(int n_sites) { return 8 * zz_col_tiles(n_sites); }
@@ -502,6 +591,121 @@ void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, d
   }
 }
 
+// ---- host half of dmv_apply_spin: the checks and the per-site coefficients K.  With psi = B_s x in the source's irrep,
+// the target projector P_t = 1 / |G_t| sum_g conj chi_t(g) U_g turns O = sum_j w_j o_j into
+//     P_t O psi = sum_k K_k o'_k psi,   K_k = 1 / |G_t| sum_{g in G_t} chi_t(g) conj chi_s(g) w_{p_g^-1(k)},
+// where o'_k = o_k for an element without a flip, and with a flip -σᶻ_k for σᶻ_k and σ∓_k for σ±_k (a global spin flip
+// swaps raising and lowering).  The direction of p_g and the characters are pinned against the dense construction
+// (tests/test_spin_operators.py).
+struct SpinBasis {
+  int n_sites, hamming_weight;
+  ZzGroup G;
+  std::vector<double> chars;   // [order] interleaved (re, im)
+};
+
+SpinBasis spin_basis(int n_sites, int hamming_weight, bool has_permutations, int64_t group_order, const int32_t *perms,
+                     const uint8_t *flips, const double *characters, int spin_inversion) {
+  SpinBasis B{n_sites, hamming_weight, zz_group(n_sites, has_permutations, group_order, perms, flips, spin_inversion), {}};
+  if (has_permutations) {
+    if (!characters) throw std::runtime_error("the basis has permutations but no characters");
+    B.chars.assign(characters, characters + 2 * group_order);
+  } else {
+    B.chars = {1.0, 0.0};
+    if (spin_inversion != 0) B.chars.insert(B.chars.end(), {(double)spin_inversion, 0.0});
+  }
+  return B;
+}
+
+SpinBasis spin_basis(const dmv_context *c) {
+  return spin_basis(c->n_sites, c->hamming_weight, c->has_permutations, c->k_group_order, c->k_perms.data(),
+                    c->k_flips.data(), c->k_chars.data(), c->spin_inversion);
+}
+
+struct SpinPlan {
+  int walk = SPIN_SELF;
+  std::vector<double> k;        // [2][N] complex: k_set, then k_clear
+  double c0[2] = {0.0, 0.0};
+  bool diag_sites = false;      // SPIN_SELF: the row factor sums k_set / k_clear over the sites (σᶻ)
+};
+
+const char *const kSpinKinds[4] = {"DMV_SPIN_ONE", "DMV_SPIN_Z", "DMV_SPIN_PLUS", "DMV_SPIN_MINUS"};
+
+SpinPlan spin_plan(const SpinBasis &src, const SpinBasis &tgt, int elt, int kind, const double *w) {
+  if (kind < DMV_SPIN_ONE || kind > DMV_SPIN_MINUS)
+    throw std::runtime_error("kind must be DMV_SPIN_ONE, DMV_SPIN_Z, DMV_SPIN_PLUS or DMV_SPIN_MINUS (got " +
+                             std::to_string(kind) + ")");
+  if (!w) throw std::runtime_error("weights must not be null");
+  if (elt != DMV_F64 && elt != DMV_C128) throw std::runtime_error("elt must be DMV_F64 or DMV_C128");
+  const int N = src.n_sites;
+  if (tgt.n_sites != N)
+    throw std::runtime_error("the target has " + std::to_string(tgt.n_sites) + " sites and the source " +
+                             std::to_string(N) + ": both bases need the same number of sites");
+  const int delta = kind == DMV_SPIN_PLUS ? 1 : kind == DMV_SPIN_MINUS ? -1 : 0;
+  const bool both_free = src.hamming_weight < 0 && tgt.hamming_weight < 0;
+  if (!both_free && (src.hamming_weight < 0 || tgt.hamming_weight != src.hamming_weight + delta))
+    throw std::runtime_error(std::string("Hamming weights: ") + kSpinKinds[kind] + " needs target = source" +
+                             (delta > 0 ? " + 1" : delta < 0 ? " - 1" : "") + " or both free, got source " +
+                             std::to_string(src.hamming_weight) + " and target " + std::to_string(tgt.hamming_weight));
+  // the source element of every target element, compared as (permutation, flip)
+  std::map<std::pair<std::vector<int32_t>, int>, int64_t> where;
+  for (int64_t e = 0; e < src.G.order; ++e)
+    where.emplace(std::make_pair(std::vector<int32_t>(src.G.perms.begin() + e * N, src.G.perms.begin() + (e + 1) * N),
+                                 src.G.flips[e] ? 1 : 0), e);
+  if (elt == DMV_F64) {
+    bool real = true;
+    for (int j = 0; j < N; ++j) real &= w[2 * j + 1] == 0.0;
+    for (size_t e = 1; e < src.chars.size(); e += 2) real &= src.chars[e] == 0.0;
+    for (size_t e = 1; e < tgt.chars.size(); e += 2) real &= tgt.chars[e] == 0.0;
+    if (!real)
+      throw std::runtime_error("DMV_F64 needs real weights and real characters in both bases: use DMV_C128");
+  }
+  SpinPlan S;
+  S.k.assign(4 * (size_t)N, 0.0);
+  double *k_set = S.k.data(), *k_clear = S.k.data() + 2 * N;
+  bool any_flip = false;
+  std::vector<int32_t> inv(N);
+  for (int64_t e = 0; e < tgt.G.order; ++e) {
+    const int32_t *p = tgt.G.perms.data() + e * N;
+    const int f = tgt.G.flips[e] ? 1 : 0;
+    const auto it = where.find(std::make_pair(std::vector<int32_t>(p, p + N), f));
+    if (it == where.end()) {
+      std::string perm;
+      for (int i = 0; i < N && i < 12; ++i) perm += (i ? " " : "") + std::to_string(p[i]);
+      throw std::runtime_error("the target group is not a subgroup of the source group: its element " +
+                               std::to_string(e) + " (permutation " + perm + (N > 12 ? " ..." : "") + ", flip " +
+                               std::to_string(f) + ") is not in the source group");
+    }
+    any_flip |= f != 0;
+    const double ct_re = tgt.chars[2 * e], ct_im = tgt.chars[2 * e + 1];
+    const double cs_re = src.chars[2 * it->second], cs_im = src.chars[2 * it->second + 1];
+    double chi_re = ct_re * cs_re + ct_im * cs_im, chi_im = ct_im * cs_re - ct_re * cs_im;   // chi_t conj(chi_s)
+    if (kind == DMV_SPIN_Z && f) { chi_re = -chi_re; chi_im = -chi_im; }
+    for (int i = 0; i < N; ++i) inv[p[i]] = i;
+    // σ⁺ terms walk the set bits of the row, σ⁻ terms its clear bits; a flip swaps them
+    const bool to_set = kind == DMV_SPIN_Z || kind == DMV_SPIN_ONE || ((kind == DMV_SPIN_PLUS) != (f != 0));
+    double *dst = to_set ? k_set : k_clear;
+    for (int k = 0; k < N; ++k) {
+      const double wr = w[2 * inv[k]], wi = w[2 * inv[k] + 1];
+      dst[2 * k] += chi_re * wr - chi_im * wi;
+      dst[2 * k + 1] += chi_re * wi + chi_im * wr;
+    }
+  }
+  const double scale = 1.0 / (double)tgt.G.order;
+  for (double &v : S.k) v *= scale;
+  if (kind == DMV_SPIN_ONE) {   // a constant: sum_k K_k
+    for (int k = 0; k < N; ++k) { S.c0[0] += k_set[2 * k]; S.c0[1] += k_set[2 * k + 1]; }
+    std::fill(S.k.begin(), S.k.end(), 0.0);
+  } else if (kind == DMV_SPIN_Z) {   // s_k = +1 on a set bit, -1 on a clear one
+    for (int t = 0; t < 2 * N; ++t) k_clear[t] = -k_set[t];
+    S.diag_sites = true;
+  }
+  S.walk = kind <= DMV_SPIN_Z ? SPIN_SELF
+           : any_flip         ? SPIN_BOTH
+           : kind == DMV_SPIN_PLUS ? SPIN_SET
+                                   : SPIN_CLEAR;
+  return S;
+}
+
 }  // namespace
 
 extern "C" {
@@ -620,6 +824,110 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
   }
   CUDA_CHECK(cudaMemcpyAsync(pm, out.data(), out.size() * sizeof(double), cudaMemcpyDefault, st));
   CUDA_CHECK(cudaStreamSynchronize(st));
+  API_END
+}
+
+// ---- one-site operators between bases (DESIGN.md section 3, "dmv_apply_spin"): per vector one k_spin_rows pass over
+// the target's rows of this rank, the source's states found as dmv_pm_correlations finds its targets.  On several ranks
+// in the source's whole-basis twin against the gathered x.
+int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights, int num_vectors,
+                   const void *x, void *y) {
+  API_BEGIN
+  if (!target || !source) throw std::runtime_error("target and source must not be null");
+  SolverRun run(source, elt, "dmv_apply_spin", false);
+  require_states(target);
+  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
+  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
+    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt, kind, weights);
+  if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
+  if (!x) throw std::runtime_error("x must not be null");
+  if (!y) throw std::runtime_error("y must not be null");
+  const int N = source->n_sites, P = run.P;
+  cudaStream_t st = run.st;
+  dmv_context *basis = source;   // where the source states are looked up
+  if (P > 1) {
+    if (!source->exchange_decided) decide_exchange(source);   // collective: every rank reaches the same decision
+    if (!source->replicated)
+      throw std::runtime_error("dmv_apply_spin on several ranks needs the source's whole basis on every rank (the "
+                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
+                               "fit in device memory");
+    basis = source->global;
+  }
+  const bool trivial = source->proj != PROJ_GROUP || source->orbit.trivial_characters;
+  const int look = source->proj == PROJ_NONE        ? PM_NONE
+                   : source->proj == PROJ_INVERSION ? PM_INVERSION
+                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
+                                                                     : PM_GROUP;
+  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
+                                                            basis->opt.rows_ctas) : 0;
+  DevBuf<double> d_k;
+  d_k.upload(S.k, st);
+  SpinArgs A{};
+  A.src.index = base_params(basis).index;
+  A.src.orbit = basis->orbit;
+  A.src.norms = basis->d_norms.ptr;
+  A.src.pos = P > 1 ? source->d_pos.ptr : nullptr;
+  A.src.site_mask = source->site_mask;
+  A.src.inversion_character = (double)source->spin_inversion;
+  A.src.n_sites = N;
+  A.src.status = source->d_status.ptr;
+  A.rows = target->d_reps.ptr;
+  A.row_norms = target->proj == PROJ_GROUP ? target->d_norms.ptr : nullptr;
+  A.row_norm = target->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
+  A.src_scale = source->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
+  A.k = d_k.ptr;
+  A.c0 = make_double2(S.c0[0], S.c0[1]);
+  A.diag_mask = S.diag_sites ? source->site_mask : 0;
+  A.n_rows = target->n_states;
+  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
+    cudaStream_t keep = basis->stream;
+    basis->stream = st;
+    ensure_table(basis, elt);
+    basis->stream = keep;
+    A.src.table = basis->d_table.ptr;
+    A.src.table_slots = basis->table_slots;
+    A.src.table_dir = basis->table_dir;
+    A.src.dord = basis->dord;
+    A.src.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
+  }
+  const size_t out_words = (size_t)target->n_states * elt;
+  const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
+  OutArg<double> yout(static_cast<double *>(y), (size_t)num_vectors * out_words);
+  for (int v = 0; v < num_vectors; ++v) {
+    const double *xv = xin.ptr + (size_t)v * run.words;
+    A.src.x = P > 1 ? gather_x(source, elt, xv) : xv;
+    A.y = yout.ptr + (size_t)v * out_words;
+    if (look == PM_TABLE)
+      launch_table_fill(basis->n_states, run.ce, A.src.x, basis->d_norms.ptr, A.src.pos, basis->d_slot_of.ptr,
+                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
+    if (A.n_rows > 0)
+      with_spin_kernel(look, tk, S.walk, run.ce, [&](auto kernel) {
+        const int grid = one_wave(kernel, (A.n_rows + kSpinThreads - 1) / kSpinThreads, 0, kSpinThreads);
+        kernel<<<grid, kSpinThreads, 0, st>>>(A);
+        check_launch("k_spin_rows");
+      });
+  }
+  yout.finish(st);
+  check_status(source);   // synchronises
+  API_END
+}
+
+// host-only self-check entry for the host half of dmv_apply_spin (no device needed)
+int dmv_debug_spin_weights(const dmv_basis_desc *source, const dmv_basis_desc *target, int elt, int kind,
+                           const double *weights, double *k, double *c0, int *walk) {
+  API_BEGIN
+  if (!source || !target) throw std::runtime_error("source and target must not be null");
+  for (const dmv_basis_desc *b : {source, target})
+    if (b->number_sites < 1 || b->number_sites > 64) throw std::runtime_error("number_sites must be between 1 and 64");
+  auto basis = [](const dmv_basis_desc *b) {
+    return spin_basis(b->number_sites, b->hamming_weight, b->has_permutations != 0, b->group_order, b->perms, b->flips,
+                      b->characters, b->spin_inversion);
+  };
+  const SpinPlan S = spin_plan(basis(source), basis(target), elt, kind, weights);
+  if (k) std::copy(S.k.begin(), S.k.end(), k);
+  if (c0) { c0[0] = S.c0[0]; c0[1] = S.c0[1]; }
+  if (walk) *walk = S.walk;
   API_END
 }
 

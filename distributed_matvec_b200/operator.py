@@ -400,6 +400,42 @@ class Operator:
         S2 = 0.25 * S.sum(axis=(-2, -1))
         return (S, float(S2)) if S.ndim == 2 else (S, S2)
 
+    _SPIN_KINDS = {"1": 0, "z": 1, "+": 2, "-": 3}
+
+    def apply_spin(self, kind: str, weights, x, target: "Operator"):
+        """y = B_targetᴴ O B_this x with O = sum_j weights[j] o_j, o_j = 1, σᶻ_j, σ⁺_j or σ⁻_j for kind "1", "z", "+",
+        "-" (dmv_apply_spin): the projection of O psi onto the target's sector.  `target` is another Operator on the
+        same device and sites whose group is a subgroup of this one's (a target without symmetries unfolds x into the
+        plain basis).  x: shape (n,) or (k, n), float64 (real weights and characters only) or complex128, a numpy array
+        or a torch CUDA tensor (then y is a torch tensor on torch's current stream).  Collective when num_ranks > 1.
+        -> y of shape (n_target,) or (k, n_target), of x's kind and type."""
+        if kind not in self._SPIN_KINDS:
+            raise ValueError(f"kind must be one of {sorted(self._SPIN_KINDS)}, got {kind!r}")
+        elt = _elt_of(x)
+        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        w = np.ascontiguousarray(np.asarray(weights, dtype=np.complex128).reshape(-1))
+        if w.shape[0] != N:
+            raise ValueError(f"weights must have {N} entries")
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        m = target.basis.numberStates()
+        shape = (m,) if x.ndim == 1 else (k, m)
+        if _is_torch(x):
+            import torch
+            if not x.is_cuda:
+                raise ValueError("a torch x must be a CUDA tensor")
+            self.use_torch_stream()
+            target.use_torch_stream()
+            x = x.contiguous()
+            y = torch.empty(shape, dtype=x.dtype, device=x.device)
+        else:
+            x = np.ascontiguousarray(x)
+            y = np.empty(shape, dtype=x.dtype)
+        nat.check(nat.lib().dmv_apply_spin(target._ctx, self._ctx, elt, self._SPIN_KINDS[kind], w.ctypes.data, k,
+                                           _ptr(x), _ptr(y)))
+        return y
+
     def lanczos_quadrature(self, num_vectors: int, steps: int, seed: int = 42, start=None,
                            complex_vectors: bool = False):
         """Finite-temperature Lanczos (stochastic Lanczos quadrature) on the device (dmv_lanczos_quadrature): for each

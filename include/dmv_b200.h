@@ -326,6 +326,32 @@ int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
  * call is bit-identical. */
 int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm);
 
+/* ---- one-site operators between symmetry sectors on the device (row f8; not in the reference): the start vectors of
+ * dynamical structure factors S(q, ω).  y = B_targetᴴ · O · B_source · x with O = Σ_j w_j o_j, o_j = 1, σᶻ_j, σ⁺_j or σ⁻_j
+ * (kind), σᶻ = +1 on a set bit, σ⁺ turning a 0 bit into a 1 bit (the conventions of the expressions and of
+ * dmv_pm_correlations); weights: N complex numbers, interleaved (re, im).  B is the symmetry-adapted basis of a context
+ * (column k = P|r_k> / ‖P|r_k>‖, P = 1/|G| Σ_g conj χ(g) U_g).  So y is the projection of Oψ onto the target sector; it
+ * is not assumed that Oψ lies wholly in that sector.
+ * Accepted: both contexts on the same device with the same number of sites, rank and number of ranks; Hamming weights
+ * equal for DMV_SPIN_ONE / DMV_SPIN_Z, target = source + 1 for DMV_SPIN_PLUS and source - 1 for DMV_SPIN_MINUS, or both
+ * free (-1); the target group a subset of the source group, compared as sets of (permutation, flip) (characters may
+ * differ; a target without symmetries is always allowed, and unfolds a symmetric state into the plain basis).  elt
+ * applies to x and y; DMV_F64 only when the weights and the characters of both bases are real.  x: num_vectors source
+ * vectors, y: num_vectors target vectors, [num_vectors, n] layout (n = dmv_number_states of each context, this rank's
+ * hashed block), host or device.  Anything else fails with a message naming the reason, and nothing is written.
+ * Method: with psi = B_source x in the source's irrep, P_target O psi = Σ_k K_k o'_k psi with
+ *     K_k = 1/|G_t| Σ_{g in G_t} χ_t(g) conj χ_s(g) w_{p_g⁻¹(k)},
+ * o'_k = o_k for elements without a flip; a flip turns σᶻ into -σᶻ and swaps σ⁺ and σ⁻ (free weight with spin inversion:
+ * the row walks both its set and its clear bits).  One lane per target row (k_spin_rows) finds psi at the row's own
+ * state or at its one-bit neighbours through the source's orbit minimum, character and look-up (k_rows' table refilled
+ * from x when the source has trivial characters, else the index and the norms).  A source state outside the source
+ * basis adds nothing when its projection vanishes and is an error otherwise.  One store per row and no atomics: a
+ * repeated call is bit-identical.  Collective when num_ranks > 1 (needs dmv_comm_init on the source and its whole basis
+ * on every rank, as dmv_pm_correlations); the rows are this rank's rows of the target basis. */
+enum { DMV_SPIN_ONE = 0, DMV_SPIN_Z = 1, DMV_SPIN_PLUS = 2, DMV_SPIN_MINUS = 3 };
+int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
+                   int num_vectors, const void *x, void *y);
+
 /* ---- finite-temperature Lanczos on the device (row f6; not in the reference): the random-vector quadrature of the
  * finite-temperature Lanczos method (Jaklič & Prelovšek 1994), also called stochastic Lanczos quadrature.  For each of
  * num_vectors start vectors r, `steps` steps of the three-term recurrence (no reorthogonalisation, no stored basis) give
@@ -446,6 +472,13 @@ int dmv_debug_zz_symmetrize(const dmv_basis_desc *basis, const double *gram, dou
  *   dmv_pm_correlations finishes it.  The group is that of dmv_debug_zz_symmetrize. */
 int dmv_debug_pm_classes(const dmv_basis_desc *basis, int32_t *class_of, int32_t *class_size, int32_t *num_classes,
                          const double *sums, double W, const double *magnetization, double *pm);
+/* dmv_debug_spin_weights: host half of dmv_apply_spin, with its checks (sites, Hamming weights, subgroup, kind, elt and
+ *   real weights / characters for DMV_F64).  k (4 N doubles, may be NULL): the complex coefficients of the set-bit
+ *   walk, then of the clear-bit walk (DMV_SPIN_Z: K on the set bits and -K on the clear bits of the row's own state;
+ *   DMV_SPIN_ONE: zero); c0 (2 doubles, may be NULL): the constant of the row factor (DMV_SPIN_ONE: Σ_k K_k);
+ *   *walk (may be NULL): 0 the row's own state, 1 its clear bits, 2 its set bits, 3 both. */
+int dmv_debug_spin_weights(const dmv_basis_desc *source, const dmv_basis_desc *target, int elt, int kind,
+                           const double *weights, double *k, double *c0, int *walk);
 int dmv_debug_compile_group(const dmv_basis_desc *basis, int64_t *info, int64_t count,
                             const uint64_t *states, uint64_t *reps, int32_t *stab);
 int dmv_debug_ordered_table(const uint64_t *reps, int64_t n, int bits, int buckets_per_state, uint32_t *block,
