@@ -120,6 +120,11 @@ _SIGNATURES = [
                                         C.c_void_p]),
     ("dmv_debug_torus_sq_rows", C.c_int, [C.POINTER(BasisDesc), C.c_int64, C.c_void_p, C.c_int64, C.c_void_p,
                                           C.c_void_p, C.c_void_p]),
+    ("dmv_debug_rows_store", C.c_int, [C.c_void_p, C.c_int, C.c_int]),
+    ("dmv_debug_rows_store_plan", C.c_int, [C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int64, C.c_int64, C.c_int,
+                                            C.c_int, C.c_void_p, C.c_void_p]),
+    ("dmv_debug_rows_store_coefficients", C.c_int, [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                                    C.POINTER(C.c_int)]),
     ("dmv_debug_solver_kernel", C.c_int, [C.c_char_p, C.c_int, C.c_int64, C.c_void_p, C.c_int, C.c_double, C.c_void_p,
                                           C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
                                           C.POINTER(C.c_int)]),

@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libdmv_b200.so")
 SOURCES = ["dmv_kernels.cu", "dmv_gather.cu", "dmv_solver.cu", "dmv_group.cu", "dmv_api.cu", "dmv_exchange.cu",
-           "dmv_lanczos.cu", "dmv_krylov.cu", "dmv_eigsh.cu", "dmv_observe.cu", "dmv_thermal.cu", "dmv_plugin.cu"]
+           "dmv_lanczos.cu", "dmv_krylov.cu", "dmv_eigsh.cu", "dmv_observe.cu", "dmv_thermal.cu", "dmv_plugin.cu", "dmv_store.cu"]
 HEADERS = ["dmv_device.cuh", "dmv_host.h", "dmv_context.h", "dmv_dense.h", "dmv_solve.h", os.path.join("..", "..", "include", "dmv_b200.h")]
 ARCH = "arch=compute_90a,code=sm_90a"
 NVCC_FLAGS = ["-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17",

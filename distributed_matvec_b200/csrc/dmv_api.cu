@@ -401,6 +401,7 @@ void install_directory(dmv_context *ctx) {
   ctx->planned = false;
   ctx->table_elt = 0;
   ctx->table_batch_slots = 0;
+  ctx->store.release();   // (release() waits for the device)
   // a new block also invalidates the exchange set-up: the replicated-x twin / slot table and the record plan
   ctx->exchange_decided = false;
   ctx->replicated = false;
@@ -819,6 +820,10 @@ void ensure_table(dmv_context *ctx, int elt) {
 void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_all, const uint32_t *pos,
                   cudaStream_t stream, bool fill, dmv_context *timer) {
   if (!timer) timer = basis;   // whose event timeline the refill belongs to (the rank's context in the replicated form)
+  select_tables(basis, p, true, false);
+  p.uni_re = basis->gather_uni[0]; p.uni_im = basis->gather_uni[1];
+  // the term store when it applies (dmv_store.cu): no orbit minimum and no table look-up per product
+  if (rows_store_product(basis, p, elt, x_all, pos, stream, fill, timer)) return;
   cudaStream_t keep = basis->stream;
   basis->stream = stream;
   ensure_table(basis, elt);
@@ -831,8 +836,6 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
     CUDA_CHECK(cudaEventRecord(timer->ev_fill[1], stream));
     timer->fill_timed = true;
   }
-  select_tables(basis, p, true, false);
-  p.uni_re = basis->gather_uni[0]; p.uni_im = basis->gather_uni[1];
   p.table = basis->d_table.ptr;
   p.table_slots = basis->table_slots;
   p.table_dir = basis->table_dir;
@@ -1262,6 +1265,16 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   // CTAs per SM the last k_rows launch had resident (the whole-basis twin's, for the replicated-x product); 0: none yet
   if (key == "rows_ctas_resident")
     return ctx->rows_ctas_resident ? ctx->rows_ctas_resident : (ctx->global ? ctx->global->rows_ctas_resident : 0);
+  // the term store of the last rows product (the whole-basis twin's, for the replicated-x product): whether it ran on
+  // one, its column blocks, its size and how many stores the context has built
+  {
+    const RowsStore &S = ctx->replicated && ctx->global ? ctx->global->store : ctx->store;
+    if (key == "rows_store") return S.active ? 1 : 0;
+    if (key == "rows_store_chunks") return S.built ? S.view.chunks : 0;
+    if (key == "rows_store_mb") return S.built ? (S.bytes + (1 << 20) - 1) >> 20 : 0;
+    if (key == "rows_store_terms") return S.built ? S.terms : 0;
+    if (key == "rows_store_builds") return S.builds;
+  }
   if (key == "rows_l2") return ctx->opt.rows_l2;
   if (key == "rows_l2_window") return ctx->opt.rows_l2_window;
   if (key == "rows_ok") return ctx->rows_ok ? 1 : 0;
@@ -1287,6 +1300,17 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "eigsh_rotate_vectors") return ctx->eg_rotate_vectors;
   if (key == "quadrature_group") return ctx->qd_group;
   return -1;
+}
+
+int dmv_debug_rows_store(dmv_context *ctx, int mode, int chunks) {
+  API_BEGIN
+  if (!ctx) throw std::runtime_error("null context");
+  if (mode < -1 || mode > 1) throw std::runtime_error("rows store mode: -1 auto, 0 never, 1 always");
+  if (chunks < 0 || chunks > kStoreMaxChunks) throw std::runtime_error("rows store chunks: 0 .. 64");
+  ctx->opt.rows_store = mode;
+  ctx->opt.rows_store_chunks = chunks;
+  if (ctx->global) { ctx->global->opt.rows_store = mode; ctx->global->opt.rows_store_chunks = chunks; }
+  API_END
 }
 
 int dmv_synchronize(dmv_context *ctx) {

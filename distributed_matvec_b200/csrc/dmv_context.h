@@ -188,10 +188,49 @@ struct Options {
   int rows_l2_window = 2;
   int rows_batch_min = 2;   // doubles per state (vectors x element width) from which a batch goes through k_rows_batch
   int rows_batch = -1;      // -1 / 1: batched products of symmetric bases go through k_rows_batch | 0: vector by vector
+  // the term store of k_rows_stored (dmv_store.cu), set through dmv_debug_rows_store rather than dmv_set_option:
+  // -1 auto (rows_store_plan), 0 never, 1 whenever the store can be built; chunks: 0 the plan's column blocks, else C
+  int rows_store = -1;
+  int rows_store_chunks = 0;
   int exchange = -1;        // -1 auto (replicated x, else peer-direct when possible), 0 NCCL send/recv, 1 peer-direct,
                             // 2 replicated x
   int peer_gather = -1;     // -1 auto, 0 NCCL all-gather
   int rounds = -1;          // -1 auto, 0 / 1 off (generate everything, fence, accumulate), R > 1
+};
+
+// The term store of k_rows_stored (RowsStoreView in dmv_host.h) over the rows of a product on a basis: built on the first
+// product that chooses it, kept across element-type and option changes (the targets are the orbit minima whatever the
+// canonical form or table), released with the basis or when the rows change
+struct RowsStore {
+  bool built = false;
+  const uint64_t *rows_of = nullptr;     // the rows it is for: row_states (null: the basis itself) and their number
+  int64_t n_rows = 0;
+  int mode = 0, chunks_asked = 0;        // the setting it was built under (Options::rows_store, rows_store_chunks)
+  // what keeps these rows without a store: refused (a missing target or a coefficient without a code: for good),
+  // overflow_chunks (a row with more than 255 entries in a block at that many blocks), exact_terms (the term count of
+  // a build the memory rule stopped: a later product checks the rule again without a count pass)
+  bool refused = false;
+  int overflow_chunks = 0;
+  int64_t exact_terms = 0;
+  RowsStoreView view{};
+  DevBuf<uint32_t> entries;
+  DevBuf<uint64_t> tile_off;
+  DevBuf<uint8_t> counts;
+  DevBuf<double> diag;
+  DevBuf<double> xs, partial;   // compact scaled x (two doubles per state) and the rows' partial sums (two per row)
+  int64_t terms = 0, bytes = 0;
+  int64_t builds = 0;           // stores built over the context's life
+  int per_pass = 1;             // blocks per pass of the current product
+  bool active = false;          // the current (last) rows product runs on it
+  void release_buffers() {
+    built = false; view = RowsStoreView{}; terms = 0; bytes = 0;
+    entries.release(); tile_off.release(); counts.release(); diag.release(); xs.release(); partial.release();
+  }
+  void release() {
+    release_buffers();
+    rows_of = nullptr; n_rows = 0; mode = 0; chunks_asked = 0; refused = false; overflow_chunks = 0; exact_terms = 0;
+    active = false;
+  }
 };
 
 struct dmv_context {
@@ -250,6 +289,7 @@ struct dmv_context {
   DevBuf<unsigned char> d_table_batch;
   DevBuf<uint32_t> d_slot_of_batch;
   uint32_t table_batch_slots = 0;
+  RowsStore store;
   double gather_uni[2] = {0.0, 0.0};
   int index_mode = INDEX_DIRECTORY;
   DevBuf<uint32_t> d_binom, d_lin_a, d_lin_b;
@@ -431,6 +471,21 @@ void do_plan(dmv_context *ctx);
 void ensure_table(dmv_context *ctx, int elt);
 void rows_product_batch(dmv_context *ctx, int elt, int nv, const void *x, void *y, int64_t stride);
 void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_all, const uint32_t *pos, cudaStream_t stream, bool fill = true, dmv_context *timer = nullptr);
+// the term store (dmv_store.cu): the plan of a store from sizes alone, and the product on it (false: the product is
+// k_rows', the store does not apply or cannot be built)
+struct StorePlan {
+  bool use = false;
+  int chunks = 0, per_pass = 0;     // column blocks, blocks per pass
+  int64_t block_states = 0, bytes = 0;
+  double ms_store = 0.0, ms_rows = 0.0;   // the cost model's estimates (auto)
+  const char *why = "";
+};
+int store_per_pass(int chunks_asked, int elt, int chunks);
+StorePlan rows_store_plan(int64_t n_states, int64_t n_rows, int64_t terms, int elt, int64_t l2_bytes, int64_t free_bytes,
+                          int mode, int chunks);
+bool store_coefficients(const HostTables &h, std::vector<double> &coef);
+bool rows_store_product(dmv_context *basis, KernelParams &p, int elt, const void *x_all, const uint32_t *pos,
+                        cudaStream_t stream, bool fill, dmv_context *timer);
 void do_generate(dmv_context *ctx, int elt, const void *x_dev, void *y_dev, const void *x_host_pending = nullptr, int64_t row_begin = 0, int64_t row_end = 0);
 void do_accumulate(dmv_context *ctx, int elt, int64_t count, const uint64_t *betas, const double *coeffs, void *y_dev);
 void collect_timings(dmv_context *ctx);

@@ -145,6 +145,36 @@ void launch_gather(const KernelParams &p, bool inversion, bool complex_values, b
 int launch_rows(const KernelParams &p, bool complex_elements, cudaStream_t stream);
 // side of the square-torus orbit minimum k_rows is compiled for (4 | 6), 0: the generic orbit walk
 int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas);
+
+// The term store of k_rows_stored (dmv_store.cu): every term k_rows accumulates, kept once per basis as a 32-bit entry
+// (index of its target within its column block) | (code of its coefficient << kStoreIndexBits).  The basis' states are
+// cut into `chunks` column blocks of block_states states; the entries are laid out block-major, and within a block by
+// tile of 32 rows, row and k_rows' term order.  counts[k * n_rows + r] = entries of row r in block k, tile_off[k * n_tiles
+// + t] = first entry of tile t in block k; row r's entries of block k follow those of the rows before it in its tile.
+constexpr int kStoreIndexBits = 28;
+constexpr int kStoreCodes = 16;          // 32 - kStoreIndexBits bits of coefficient code
+constexpr int kStoreMaxChunks = 64;
+struct RowsStoreView {
+  uint32_t *entries;
+  uint64_t *tile_off;
+  uint8_t *counts;
+  double *diag;                   // D(b) of every row (real operator), null without diagonal terms
+  int64_t n_rows, n_tiles, block_states;
+  int32_t chunks;
+  double coef[kStoreCodes];       // the coefficient of every code
+};
+// build passes over rows [0, s.n_rows) of p (p.row_states, or the basis itself): count (counts, diag; flags[0] terms
+// whose target is missing with c != 0, flags[1] a count past 255, flags[2] a coefficient without a code), then write
+// (entries, from counts and tile_off)
+void launch_store_build(const KernelParams &p, const RowsStoreView &s, bool write_pass, unsigned long long *flags,
+                        cudaStream_t stream);
+// tile sums of the counts (one per (block, tile), block-major) into tile_off[0 .. chunks * n_tiles); then the exclusive
+// prefix sum over them, in place, with the total in tile_off[chunks * n_tiles]
+void launch_store_offsets(const RowsStoreView &s, cudaStream_t stream);
+// one pass of k_rows_stored over blocks [k0, k1) of rows [p.row_begin, p.row_end): the first pass starts each row's
+// sum, the last one stores y as k_rows does; in between the sums wait in `partial` (one element per row)
+void launch_rows_stored(const KernelParams &p, const RowsStoreView &s, const void *xs, void *partial, int k0, int k1,
+                        bool complex_elements, cudaStream_t stream);
 // hash table of k_rows: insert every state (slot_of[i] = its slot), then per product table[slot_of[i]] = x[src(i)] * norm[i]
 // with src(i) = pos ? pos[i] : i
 void launch_table_insert(const uint64_t *reps, int64_t n, void *table, uint32_t n_buckets, int slots_per_bucket,
@@ -155,8 +185,11 @@ void launch_ordered_dir(const uint64_t *reps, int64_t n, OrderedDir ord, uint32_
 void launch_rows_batch(const KernelParams &p, cudaStream_t stream);
 void launch_table_fill_batch(int64_t n, int num_vectors, int elt, const void *x, int64_t stride, const double *norms,
                              const uint32_t *slot_of, const uint64_t *reps, void *table, cudaStream_t stream);
+// compact: the term store's scaled x instead (compact[i] = x[src(i)] * norm[i], 16 or 8 bytes in state order; slot_of,
+// reps, table and dense unused)
 void launch_table_fill(int64_t n, bool complex_elements, const void *x, const double *norms, const uint32_t *pos,
-                       const uint32_t *slot_of, const uint64_t *reps, void *table, void *dense, cudaStream_t stream);
+                       const uint32_t *slot_of, const uint64_t *reps, void *table, void *dense, cudaStream_t stream,
+                       void *compact = nullptr);
 // perfect-hash set-up (k_rows dense index): mark the positions of `n` states at a level in seen / collide bit arrays
 // (192 bits per block, 3 words each), and compact the states whose position collided into `next`
 void launch_mph_mark(const uint64_t *keys, int64_t n, int level, uint32_t n_blocks, unsigned long long *seen,

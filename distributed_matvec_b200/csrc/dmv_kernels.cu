@@ -1294,6 +1294,234 @@ __global__ void __launch_bounds__(kThreads, CTAS) k_rows(const KernelParams p) {
 }
 
 // -------------------------------------------------------------------------------------------------
+// The term store (RowsStoreView in dmv_host.h, built by dmv_store.cu).  Every term's target and coefficient depend on the
+// basis and the operator only, so they are found once: k_store_build walks the rows exactly as k_rows does (row_terms,
+// pop_term, the same orbit minimum) and finds each target's index in the sorted basis with `locate`.  The count pass
+// counts the entries of every (column block, row), evaluates the row's diagonal and reports what the store cannot hold;
+// the write pass puts each entry at its place.  k_rows_stored then needs no orbit minimum and no look-up: a pass over
+// adjacent column blocks gathers (n x) from the compact scaled x of those blocks only, which stays in L2 while the
+// pass runs, in place of one random HBM sector per term.
+// -------------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t warp_exclusive_sum(uint32_t v, unsigned lane) {
+  uint32_t s = v;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xffffffffu, s, d);
+    if (lane >= (unsigned)d) s += t;
+  }
+  return s - v;
+}
+
+template <int TK, bool WRITE>
+__global__ void __launch_bounds__(kThreads) k_store_build(const KernelParams p, const RowsStoreView s,
+                                                          unsigned long long *flags) {
+  extern __shared__ __align__(16) unsigned char smem[];
+  const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
+  const Tables<false> T = stage_tables<PROJ_GROUP, false>(p, smem, L);
+  const RowsSmem RS = rows_smem(p, L, false, TK);
+  uint64_t *sgxt = reinterpret_cast<uint64_t *>(smem + RS.gxt);
+  if constexpr (TK > 0)
+    for (int i = threadIdx.x; i < p.n_groups; i += blockDim.x) sgxt[i] = torus_sq_columns<TK>(p.groups[i].x);
+  __syncthreads();
+  const OrbitProgram &orbit = T.orbit;
+  const unsigned lane = threadIdx.x & 31u;
+  const unsigned warp = threadIdx.x >> 5;
+  const bool any_s_out = p.any_s_out != 0;
+  const uint64_t *__restrict__ row_states = p.row_states ? p.row_states : p.index.reps;
+  unsigned long long bad = 0, over = 0, uncoded = 0;
+  uint64_t cursor[WRITE ? kStoreMaxChunks : 1];   // write pass: next entry of the row in every block
+  uint32_t count[WRITE ? 1 : kStoreMaxChunks];    // count pass: entries of the row in every block
+  const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+  for (int64_t tile = (int64_t)blockIdx.x * kWarps + warp; tile < s.n_tiles; tile += warps_total) {
+    const int64_t i = tile * 32 + lane;
+    const bool valid = i < s.n_rows;
+    for (int k = 0; k < s.chunks; ++k) {
+      if constexpr (WRITE) {
+        const uint32_t c = valid ? s.counts[k * s.n_rows + i] : 0u;
+        cursor[k] = s.tile_off[k * s.n_tiles + tile] + warp_exclusive_sum(c, lane);
+      } else {
+        count[k] = 0;
+      }
+    }
+    const uint64_t b = valid ? row_states[i] : 0ull;
+    const uint64_t bt = TK > 0 ? torus_sq_columns<TK>(b) : 0ull;
+    int w = 0;
+    RowTerms rt = row_terms<false>(T, 0, 0, min(64, p.n_groups), b);
+    if (!valid) rt.mask = 0;
+    for (;;) {
+      while (valid && rt.mask == 0 && 64 * (w + 1) < p.n_groups) {
+        ++w;
+        rt = row_terms<false>(T, w, 64 * w, min(64 * w + 64, p.n_groups), b);
+      }
+      if (rt.mask == 0) break;
+      uint64_t flip;
+      const uint64_t flip_t = TK > 0 ? sgxt[64 * w + __ffsll((long long)rt.mask) - 1] : 0ull;
+      const double c = pop_term<false>(T, rt, 64 * w, b, any_s_out, flip);
+      const uint64_t raw = b ^ flip;
+      uint64_t want;
+      if constexpr (TK > 0) want = orbit_min_torus_sq_t<TK>(orbit, raw, bt ^ flip_t);
+      else want = orbit_representative(orbit, raw);
+      const int64_t idx = locate(p.index, want);
+      if (idx < 0) {   // not in the basis: k_rows skips it when c = 0 and reports it otherwise (DMV:115-118)
+        if (c != 0.0) ++bad;
+        continue;
+      }
+      const int k = (int)(idx / s.block_states);
+      int code = 0;
+      while (code < kStoreCodes && __double_as_longlong(s.coef[code]) != __double_as_longlong(c)) ++code;
+      if constexpr (WRITE) {
+        s.entries[cursor[k]++] = (uint32_t)(idx - (int64_t)k * s.block_states) | ((uint32_t)code << kStoreIndexBits);
+      } else {
+        if (code == kStoreCodes) ++uncoded;
+        ++count[k];
+      }
+    }
+    if constexpr (!WRITE) {
+      if (valid) {
+        for (int k = 0; k < s.chunks; ++k) {
+          if (count[k] > 255u) ++over;
+          s.counts[k * s.n_rows + i] = (uint8_t)min(count[k], 255u);
+        }
+        if (s.diag) {
+          double dre, dim;
+          diagonal<false>(T, p.n_diag, b, dre, dim);
+          s.diag[i] = dre;
+        }
+      }
+    }
+  }
+  if (bad) atomicAdd(flags, bad);
+  if (over) atomicAdd(flags + 1, over);
+  if (uncoded) atomicAdd(flags + 2, uncoded);
+}
+
+// per tile and block: the sum of its 32 rows' counts
+__global__ void k_store_tile_sums(const RowsStoreView s) {
+  const int64_t total = s.n_tiles * s.chunks;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < total; q += stride) {
+    const int64_t k = q / s.n_tiles, t = q - k * s.n_tiles;
+    const uint8_t *c = s.counts + k * s.n_rows + t * 32;
+    const int64_t rows = min((int64_t)32, s.n_rows - t * 32);
+    uint64_t sum = 0;
+    for (int64_t r = 0; r < rows; ++r) sum += c[r];
+    s.tile_off[q] = sum;
+  }
+}
+
+// exclusive prefix sum of a[0, n) in place, a[n] = the total: one CTA, deterministic (once per basis)
+__global__ void k_store_scan(uint64_t *a, int64_t n) {
+  __shared__ uint64_t part[1024];
+  const int64_t per = (n + blockDim.x - 1) / blockDim.x;
+  const int64_t lo = min(n, (int64_t)threadIdx.x * per), hi = min(n, lo + per);
+  uint64_t sum = 0;
+  for (int64_t q = lo; q < hi; ++q) sum += a[q];
+  part[threadIdx.x] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    uint64_t run = 0;
+    for (unsigned t = 0; t < blockDim.x; ++t) { const uint64_t v = part[t]; part[t] = run; run += v; }
+    a[n] = run;
+  }
+  __syncthreads();
+  uint64_t run = part[threadIdx.x];
+  for (int64_t q = lo; q < hi; ++q) { const uint64_t v = a[q]; a[q] = run; run += v; }
+}
+
+__device__ __forceinline__ uint32_t load_u8_hint(const uint8_t *q, uint64_t policy) {
+  uint32_t v;
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(q), "l"(policy));
+  return v;
+}
+// an entry: through L1 (a lane's next entries and its neighbours' share the line), evict_first in L2
+__device__ __forceinline__ uint32_t load_entry(const uint32_t *q, uint64_t policy) {
+  uint32_t v;
+  asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(q), "l"(policy));
+  return v;
+}
+// a gather from the current block of the compact x (an L2 hit): not allocated in L1
+__device__ __forceinline__ double gather_x(const double *q) {
+  double v;
+  asm volatile("ld.global.nc.L1::no_allocate.f64 %0, [%1];" : "=d"(v) : "l"(q));
+  return v;
+}
+__device__ __forceinline__ double2 gather_x(const double2 *q) {
+  double2 v;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.f64 {%0, %1}, [%2];" : "=d"(v.x), "=d"(v.y) : "l"(q));
+  return v;
+}
+
+// One lane per row, as k_rows.  A row's sum runs over blocks k0 .. k1 - 1 and within each block in k_rows' term order,
+// with k_rows' coefficients and (n x) products: over the whole basis at once (one block) y equals k_rows' bit for bit.
+// The entries, counts, row data and partial sums are read once per product (evict_first); four gathers per lane are in
+// flight at a time, nothing depends on a gather but its own multiply-add.
+template <bool CE>
+__global__ void __launch_bounds__(kThreads) k_rows_stored(const KernelParams p, const RowsStoreView s,
+                                                          const typename ValT<CE>::type *__restrict__ xs,
+                                                          typename ValT<CE>::type *partial, int k0, int k1) {
+  using E = typename ValT<CE>::type;
+  __shared__ double scoef[kStoreCodes];
+  if (threadIdx.x < kStoreCodes) scoef[threadIdx.x] = s.coef[threadIdx.x];
+  __syncthreads();
+  const unsigned lane = threadIdx.x & 31u;
+  const unsigned warp = threadIdx.x >> 5;
+  const bool first = k0 == 0, last = k1 == s.chunks;
+  const uint64_t stream = l2_policy(L2_FIRST);
+  const double *__restrict__ row_norms = p.row_norms ? p.row_norms : p.norms;
+  constexpr uint32_t kMask = (1u << kStoreIndexBits) - 1u;
+  const E zero = v_make(0.0, 0.0, (E *)nullptr);
+  const int64_t t0 = p.row_begin / 32, t1 = (p.row_end + 31) / 32;
+  const int64_t warps_total = (int64_t)gridDim.x * kWarps;
+  for (int64_t tile = t0 + (int64_t)blockIdx.x * kWarps + warp; tile < t1; tile += warps_total) {
+    const int64_t i = tile * 32 + lane;
+    const bool valid = i >= p.row_begin && i < p.row_end;
+    E acc = zero;
+#ifndef DMV_STORE_NO_PARTIAL   // measurement builds only: the partial sums neither read nor written, wrong results
+    if (!first && valid) acc = load_hint(partial + i, stream);
+#endif
+    for (int k = k0; k < k1; ++k) {
+      uint32_t cnt = i < s.n_rows ? load_u8_hint(s.counts + k * s.n_rows + i, stream) : 0u;
+      const uint64_t start = load64_hint(s.tile_off + k * s.n_tiles + tile, stream) + warp_exclusive_sum(cnt, lane);
+      if (!valid) cnt = 0;
+      const uint32_t *e = s.entries + start;
+#ifdef DMV_STORE_NO_GATHER   // measurement builds only: entries streamed, no gather, wrong results on purpose
+      auto gather_x = [](const E *q) { return v_make((double)(((uintptr_t)q >> 4) & 7u), 0.0, (E *)nullptr); };
+#endif
+      const E *xb = xs + (int64_t)k * s.block_states;
+      uint32_t j = 0;
+      for (; j + 4 <= cnt; j += 4) {
+        const uint32_t e0 = load_entry(e + j, stream), e1 = load_entry(e + j + 1, stream);
+        const uint32_t e2 = load_entry(e + j + 2, stream), e3 = load_entry(e + j + 3, stream);
+        const E v0 = gather_x(xb + (e0 & kMask)), v1 = gather_x(xb + (e1 & kMask));
+        const E v2 = gather_x(xb + (e2 & kMask)), v3 = gather_x(xb + (e3 & kMask));
+        axpy(acc, scoef[e0 >> kStoreIndexBits], v0);
+        axpy(acc, scoef[e1 >> kStoreIndexBits], v1);
+        axpy(acc, scoef[e2 >> kStoreIndexBits], v2);
+        axpy(acc, scoef[e3 >> kStoreIndexBits], v3);
+      }
+      for (; j < cnt; ++j) {
+        const uint32_t e0 = load_entry(e + j, stream);
+        axpy(acc, scoef[e0 >> kStoreIndexBits], gather_x(xb + (e0 & kMask)));
+      }
+    }
+    if (!valid) continue;
+    if (!last) {
+#ifndef DMV_STORE_NO_PARTIAL
+      store_hint(partial + i, acc, stream);
+#endif
+      continue;
+    }
+    // diagonal and the single store of y[i], as k_rows
+    const double inv_nb = 1.0 / load_hint(row_norms + i, stream);
+    E out;
+    if (s.diag) out = v_scale(load_hint(reinterpret_cast<const E *>(p.x) + p.x_row_offset + i, stream), load_hint(s.diag + i, stream));
+    else out = reinterpret_cast<const E *>(p.y)[i];
+    axpy(out, inv_nb, acc);
+    store_hint(reinterpret_cast<E *>(p.y) + i, out, stream);
+  }
+}
+
+// -------------------------------------------------------------------------------------------------
 // k_rows_batch: k_rows on up to six real (three complex) vectors at once -- the product the block eigensolver asks for
 // (reference src/Diagonalize.chpl:134-162: PRIMME hands `blockSize` vectors to one matvec call).  The orbit minimum and the
 // look-up of a term are shared by the vectors: one bucket = 64 bytes = { key, d[0..5], spare }, d = the scaled elements of
@@ -1445,11 +1673,21 @@ __global__ void k_ordered_dir(const uint64_t *__restrict__ reps, int64_t n, Orde
 template <bool CE>
 __global__ void k_table_fill(int64_t n, const void *__restrict__ x, const double *__restrict__ norms,
                              const uint32_t *__restrict__ pos, const uint32_t *__restrict__ slot_of,
-                             const uint64_t *__restrict__ reps, unsigned char *table, unsigned char *dense) {
+                             const uint64_t *__restrict__ reps, unsigned char *table, unsigned char *dense,
+                             unsigned char *compact) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
     const int64_t src = pos ? (int64_t)__ldg(pos + i) : i;
     const double nrm = __ldg(norms + i);
+    if (compact) {   // the term store's scaled x: the same products, in state order
+      if constexpr (CE) {
+        const double2 v = __ldg(reinterpret_cast<const double2 *>(x) + src);
+        reinterpret_cast<double2 *>(compact)[i] = make_double2(v.x * nrm, v.y * nrm);
+      } else {
+        reinterpret_cast<double *>(compact)[i] = __ldg(reinterpret_cast<const double *>(x) + src) * nrm;
+      }
+      continue;
+    }
     uint32_t s = __ldg(slot_of + i);
     const bool in_table = dense == nullptr || (s & 0x80000000u);
     s &= 0x7fffffffu;
@@ -1815,6 +2053,46 @@ int rows_torus_k(const OrbitProgram &o, bool dense, int rows_ctas) {
 }
 
 // p.batch vectors of p.batch_elt doubles per element (p.batch * p.batch_elt <= 6), p.table = the 64-byte-bucket table
+void launch_store_build(const KernelParams &p, const RowsStoreView &s, bool write_pass, unsigned long long *flags,
+                        cudaStream_t stream) {
+  if (s.n_rows <= 0) return;
+  if (s.chunks < 1 || s.chunks > kStoreMaxChunks) throw std::runtime_error("term store: 1 .. 64 column blocks");
+  const int k = rows_torus_k(p.orbit, false, 2);
+  const SmemLayout L = smem_layout(p, PROJ_GROUP, sizeof(double), false);
+  with_choice<6, 4, 0>(k, [&](auto tk) {
+    with_bool(write_pass, [&](auto wr) {
+      auto kernel = k_store_build<tk(), wr()>;
+      const size_t smem = rows_smem(p, L, false, tk()).total;
+      opt_in_smem(kernel, smem);
+      const int grid = one_wave(kernel, (s.n_tiles + kWarps - 1) / kWarps, smem);
+      kernel<<<grid, kThreads, smem, stream>>>(p, s, flags);
+      check_launch("k_store_build");
+    });
+  });
+}
+
+void launch_store_offsets(const RowsStoreView &s, cudaStream_t stream) {
+  const int64_t n = s.n_tiles * s.chunks;
+  k_store_tile_sums<<<capped_grid((n + 255) / 256, (int64_t)sm_count() * 8), 256, 0, stream>>>(s);
+  check_launch("k_store_tile_sums");
+  k_store_scan<<<1, 1024, 0, stream>>>(s.tile_off, n);
+  check_launch("k_store_scan");
+}
+
+void launch_rows_stored(const KernelParams &p, const RowsStoreView &s, const void *xs, void *partial, int k0, int k1,
+                        bool complex_elements, cudaStream_t stream) {
+  if (p.row_end <= p.row_begin) return;
+  const int64_t tiles = (p.row_end + 31) / 32 - p.row_begin / 32;
+  with_bool(complex_elements, [&](auto ce) {
+    using E = typename ValT<ce()>::type;
+    auto kernel = k_rows_stored<ce()>;
+    const int resident = resident_ctas(kernel, 0);
+    kernel<<<capped_grid((tiles + kWarps - 1) / kWarps, (int64_t)sm_count() * std::max(resident, 1)), kThreads, 0,
+             stream>>>(p, s, reinterpret_cast<const E *>(xs), reinterpret_cast<E *>(partial), k0, k1);
+    check_launch("k_rows_stored");
+  });
+}
+
 void launch_rows_batch(const KernelParams &p, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
   if (p.batch < 1 || (p.batch_elt != 1 && p.batch_elt != 2) || p.batch * p.batch_elt > 6)
@@ -1857,12 +2135,14 @@ void launch_ordered_dir(const uint64_t *reps, int64_t n, OrderedDir ord, uint32_
 }
 
 void launch_table_fill(int64_t n, bool complex_elements, const void *x, const double *norms, const uint32_t *pos,
-                       const uint32_t *slot_of, const uint64_t *reps, void *table, void *dense, cudaStream_t stream) {
+                       const uint32_t *slot_of, const uint64_t *reps, void *table, void *dense, cudaStream_t stream,
+                       void *compact) {
   if (n <= 0) return;
   const int blocks = capped_grid((n + 255) / 256, (int64_t)sm_count() * 16);
   unsigned char *t = reinterpret_cast<unsigned char *>(table), *d = reinterpret_cast<unsigned char *>(dense);
+  unsigned char *c = reinterpret_cast<unsigned char *>(compact);
   with_bool(complex_elements, [&](auto ce) {
-    k_table_fill<ce()><<<blocks, 256, 0, stream>>>(n, x, norms, pos, slot_of, reps, t, d);
+    k_table_fill<ce()><<<blocks, 256, 0, stream>>>(n, x, norms, pos, slot_of, reps, t, d, c);
   });
   check_launch("k_table_fill");
 }

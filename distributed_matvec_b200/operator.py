@@ -239,6 +239,12 @@ class Operator:
         nat.check(nat.lib().dmv_set_option(self._ctx, name.encode(), int(value)))
         return self
 
+    def debug_rows_store(self, mode: int, chunks: int = 0):
+        """dmv_debug_rows_store: the term store of the row kernel -1 auto, 0 never, 1 whenever it can be built; chunks
+        0 the cost model's column blocks, else 1 .. 64."""
+        nat.check(nat.lib().dmv_debug_rows_store(self._ctx, int(mode), int(chunks)))
+        return self
+
     def info(self, name: str) -> int:
         return int(nat.lib().dmv_get_info(self._ctx, name.encode()))
 

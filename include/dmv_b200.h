@@ -487,6 +487,23 @@ int dmv_debug_dense_order(const uint64_t *reps, int64_t n, int bits, uint32_t *b
                           int64_t *info);
 int dmv_debug_torus_sq_rows(const dmv_basis_desc *basis, int64_t count, const uint64_t *states, int64_t n_flips,
                             const uint64_t *flips, uint64_t *rows, uint64_t *single);
+/* The term store of the row kernel on bases with permutation symmetries (k_rows_stored, csrc/dmv_store.cu): the target
+ *   index and a coefficient code of every term, built once per basis and rows, read in column blocks whose scaled x
+ *   stays in L2.  It is chosen automatically; dmv_debug_rows_store overrides the choice for tests and measurements:
+ *   mode -1 auto, 0 never, 1 whenever the store can be built; chunks 0 the cost model's column blocks, else 1 .. 64.
+ *   The replicated-x product's whole-basis twin takes the same setting.  dmv_get_info keys: "rows_store" (1: the last
+ *   rows product ran on the store), "rows_store_chunks", "rows_store_mb", "rows_store_terms", "rows_store_builds".
+ * dmv_debug_rows_store_plan: the choice from sizes alone (no device): n_states targets, n_rows rows, about `terms`
+ *   terms, element type, L2 and free bytes, mode and chunks as above.  out[5] = {use, column blocks, blocks per pass,
+ *   states per block, bytes}; ms[2] = the model's milliseconds for the store and for k_rows.
+ * dmv_debug_rows_store_coefficients: the coefficient dictionary of the store from a real look-up table of n values
+ *   (and their negatives when any_s_out): *count codes written to coef (at most 16), or *count = -1 when the store
+ *   cannot encode them (more than 16 distinct values, or any_generic). */
+int dmv_debug_rows_store(dmv_context *ctx, int mode, int chunks);
+int dmv_debug_rows_store_plan(int64_t n_states, int64_t n_rows, int64_t terms, int elt, int64_t l2_bytes,
+                              int64_t free_bytes, int mode, int chunks, int64_t *out, double *ms);
+int dmv_debug_rows_store_coefficients(const double *lut, int64_t n, int any_s_out, int any_generic, double *coef,
+                                      int *count);
 /* dmv_debug_solver_kernel: runs one launcher of the solver vector kernels (csrc/dmv_solver.cu) on the current device
  *   and a private stream, on host data, for the tests (needs a device, unlike the entries above).  kernel: "dot",
  *   "lanczos_update", "scale", "fill", "block_dot", "block_combine", "block_gram", "block_update", "block_rotate",
