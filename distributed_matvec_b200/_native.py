@@ -88,6 +88,10 @@ _SIGNATURES = [
     ("dmv_pm_correlations", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     ("dmv_apply_spin", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                  C.c_void_p]),
+    ("dmv_reduced_density_matrix", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                             C.c_void_p]),
+    ("dmv_rdm_layout", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                 C.c_void_p]),
     ("dmv_lanczos_quadrature", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.POINTER(C.c_int)]),
     ("dmv_last_timings", C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.c_int]),

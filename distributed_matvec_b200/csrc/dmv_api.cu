@@ -1299,6 +1299,8 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (key == "eigsh_block_vectors") return ctx->eg_block_vectors;
   if (key == "eigsh_rotate_vectors") return ctx->eg_rotate_vectors;
   if (key == "quadrature_group") return ctx->qd_group;
+  if (key == "rdm_amplitudes") return ctx->rdm_amplitudes;
+  if (key == "rdm_gram_flops") return ctx->rdm_gram_flops;
   return -1;
 }
 

@@ -394,6 +394,8 @@ struct dmv_context {
   int64_t kr_dot_vectors = 0, kr_combine_vectors = 0;   // vector passes of dmv_expm_multiply's last block kernels
   int64_t eg_block_vectors = 0, eg_rotate_vectors = 0;  // vectors read or written by dmv_eigsh's last block kernels
   int qd_group = 0;   // G of the last dmv_lanczos_quadrature call
+  // dmv_reduced_density_matrix's last call on this rank: amplitudes filled, real FP64 multiply-adds its Gram ran
+  int64_t rdm_amplitudes = 0, rdm_gram_flops = 0;
 
   ~dmv_context() {
     delete global;

@@ -19,6 +19,9 @@ namespace {
 
 constexpr int kZzStates = 512;     // states staged in shared memory per tile
 
+// row tiles of 32 of a reduced density matrix block of dimension d (dmv_reduced_density_matrix, below)
+__host__ __device__ __forceinline__ int rdm_macro_dev(int d) { return (d + 31) / 32; }
+
 // row tiles of 16 (N sites + the constant row), column tiles of 8 (N sites)
 int zz_row_tiles(int n_sites) { return (n_sites + 1 + 15) / 16; }
 int zz_col_tiles(int n_sites) { return (n_sites + 7) / 8; }
@@ -440,6 +443,207 @@ void with_spin_kernel(int look, int tk, int walk, bool ce, F &&f) {
   });
 }
 
+// ---- reduced density matrices (dmv_reduced_density_matrix).  At a fixed Hamming weight W, ρ_A = Tr_B |ψ><ψ| is block
+// diagonal in the weight w of A; block w is Ψ Ψᴴ with Ψ[a, b] = ψ(embed_A(a) | embed_B(b)) over the configurations a of A
+// of weight w and b of B of weight W - w.  The columns b are cut into chunks; k_rdm_fill writes the amplitudes of a
+// chunk, row-major with `ld` columns (zeros past the chunk's last column), and k_rdm_gram adds Ψ Ψᴴ on the FP64 tensor
+// cores.
+struct RdmArgs {
+  PmArgs src;                  // the look-up of dmv_apply_spin; its rows / classes are unused
+  const uint64_t *embed_a;     // [d]: the states of A's rows, deposited on A's sites
+  const uint64_t *binom;       // [64][65]: C(n, k) (B's columns at a fixed weight)
+  uint64_t sites_b[64];        // site of bit j of a B configuration, as a one-bit mask
+  double scale;                // the source's src_scale (spin inversion alone: sqrt(1/2))
+  int64_t col0, cols, ld;      // first column (rank of b) of the chunk, its columns, row stride of psi
+  int d, n_b, k_b;             // rows, sites of B, ones of B (-1: free weight, b = the column itself)
+  double *psi;
+};
+
+constexpr int kRdmRowGroup = 16;   // rows of one column a lane fills (the column's configuration is unranked once)
+
+// b of column r: the r-th configuration of k ones on n_b sites in ascending numeric order (combinadic), on B's sites
+__device__ __forceinline__ uint64_t rdm_column_state(const RdmArgs &A, uint64_t r) {
+  uint64_t s = 0;
+  if (A.k_b < 0) {
+    for (uint64_t m = r; m; m &= m - 1) s |= A.sites_b[__ffsll((long long)m) - 1];
+    return s;
+  }
+  int k = A.k_b;
+  for (int pos = A.n_b - 1; pos >= 0 && k > 0; --pos) {
+    const uint64_t c = __ldg(A.binom + pos * 65 + k);
+    if (c <= r) { s |= A.sites_b[pos]; r -= c; --k; }
+  }
+  return s;
+}
+
+// psi[a * ld + c] = scale chi (n x)[rep(embed_A(a) | b_c)] for c < cols, 0 for cols <= c < ld.  A lane owns a column and
+// a group of kRdmRowGroup rows; a state outside the basis whose projection does not vanish goes to status.
+template <int LOOK, int TK, bool CE>
+__global__ void __launch_bounds__(256, 2) k_rdm_fill(const RdmArgs A) {
+  unsigned long long bad = 0;
+  uint64_t bad_state = 0;
+  const int64_t groups = (A.d + kRdmRowGroup - 1) / kRdmRowGroup, work = groups * A.ld;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < work; t += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t c = t % A.ld;
+    const int a0 = (int)(t / A.ld) * kRdmRowGroup, a1 = min(A.d, a0 + kRdmRowGroup);
+    const bool live = c < A.cols;
+    const uint64_t b = live ? rdm_column_state(A, (uint64_t)(A.col0 + c)) : 0;
+    for (int a = a0; a < a1; ++a) {
+      double2 v = make_double2(0.0, 0.0);
+      if (live) v = pm_target<LOOK, TK, CE>(A.src, __ldg(A.embed_a + a) | b, bad, bad_state);
+      if constexpr (CE) reinterpret_cast<double2 *>(A.psi)[a * A.ld + c] = make_double2(v.x * A.scale, v.y * A.scale);
+      else A.psi[a * A.ld + c] = v.x * A.scale;
+    }
+  }
+  if (bad && atomicAdd(A.src.status, bad) == 0) A.src.status[1] = bad_state;
+}
+
+constexpr int kRdmThreads = 256;
+
+// f(k_rdm_fill<LOOK, TK, CE>); TK (the square-torus orbit minimum) only for the orbit look-ups
+template <typename F>
+void with_rdm_fill(int look, int tk, bool ce, F &&f) {
+  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
+    with_bool(ce, [&](auto e) {
+      with_choice<6, 4, 0>(tk, [&](auto t) {
+        if constexpr (lk() >= PM_GROUP || t() == 0) f(k_rdm_fill<lk(), t(), e()>);
+        else throw std::logic_error("k_rdm_fill has no square-torus build without a group");
+      });
+    });
+  });
+}
+
+// Block tiles of 32 x 32 of ρ: a CTA per tile on or above the diagonal (I <= J) and per slice of the chunk's columns.
+constexpr int kRdmTile = 32;
+constexpr int kRdmTarget = 1024;   // CTAs a chunk is split into at most (tiles x slices), fixed so that sums never move
+
+int64_t rdm_tiles(int d) { const int64_t M = rdm_macro_dev(d); return M * (M + 1) / 2; }
+// slices of a chunk of `ld` columns, and the columns of one (a multiple of 32: the eight warps take four each)
+int rdm_slices(int d, int64_t ld) {
+  const int64_t by_tiles = (kRdmTarget + rdm_tiles(d) - 1) / rdm_tiles(d), by_cols = std::max<int64_t>(1, ld / 256);
+  return (int)std::max<int64_t>(1, std::min(by_tiles, by_cols));
+}
+int64_t rdm_slice_cols(int d, int64_t ld) {
+  const int S = rdm_slices(d, ld);
+  return (ld + 32 * S - 1) / (32 * S) * 32;
+}
+
+// partials[(s * tiles + t) * 1024 * (CE ? 2 : 1) + ...] = slice s's share of tile t = (I, J) of Ψ Ψᴴ: real parts
+// [32][32], then (CE) imaginary parts.  Warp w walks the groups of four columns w, w + 8, ... of the slice and holds
+// the 2 x 4 mma tiles of 16 x 8 in registers; the warps are summed in shared memory in warp order.  With Ψ = R + i I,
+// Re = R Rᵀ + I Iᵀ and Im = I Rᵀ - R Iᵀ (four real products per element); real elements take R Rᵀ alone.
+template <bool CE>
+__global__ void __launch_bounds__(256, 1) k_rdm_gram(const double *__restrict__ psi, int64_t ld, int d, int64_t cols,
+                                                   int64_t slice_cols, double *__restrict__ partials) {
+  __shared__ double s_blk[(CE ? 2 : 1) * kRdmTile * kRdmTile];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, q = lane & 3;
+  const int M = rdm_macro_dev(d);
+  int t = blockIdx.x, I = 0;
+  while (t >= M - I) { t -= M - I; ++I; }
+  const int J = I + t;
+  // rows of A (tile I) and of B (tile J) this lane reads: row tile rt rows rt * 16 + g, + 8; column tile ct row ct * 8 + g
+  int64_t ra[4], rb[4];
+  bool oka[4], okb[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int r = I * kRdmTile + (u >> 1) * 16 + (u & 1) * 8 + g, c = J * kRdmTile + u * 8 + g;
+    oka[u] = r < d; okb[u] = c < d;
+    ra[u] = (int64_t)(oka[u] ? r : 0) * ld; rb[u] = (int64_t)(okb[u] ? c : 0) * ld;
+  }
+  double re[2][4][4], im[2][4][4];
+#pragma unroll
+  for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+    for (int ct = 0; ct < 4; ++ct)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) re[rt][ct][e] = im[rt][ct][e] = 0.0;
+  const int64_t k0 = (int64_t)blockIdx.y * slice_cols, k1 = min(cols, k0 + slice_cols);
+#pragma unroll(CE ? 1 : 2)   // complex: 64 accumulators, no room for a second group's fragments
+  for (int64_t kw = k0 + 4 * warp; kw < k1; kw += 32) {   // warp-uniform: k1 - k0 is a multiple of 32
+    const int64_t k = kw + q;
+    double ar[4], ai[4], br[4], bi[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if constexpr (CE) {
+        const double2 va = oka[u] ? __ldg(reinterpret_cast<const double2 *>(psi) + ra[u] + k) : make_double2(0.0, 0.0);
+        const double2 vb = okb[u] ? __ldg(reinterpret_cast<const double2 *>(psi) + rb[u] + k) : make_double2(0.0, 0.0);
+        ar[u] = va.x; ai[u] = va.y; br[u] = vb.x; bi[u] = vb.y;
+      } else {
+        ar[u] = oka[u] ? __ldg(psi + ra[u] + k) : 0.0;
+        br[u] = okb[u] ? __ldg(psi + rb[u] + k) : 0.0;
+        ai[u] = bi[u] = 0.0;
+      }
+    }
+#pragma unroll
+    for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+      for (int ct = 0; ct < 4; ++ct) {
+        dmma_16x8x4(re[rt][ct], ar[2 * rt], ar[2 * rt + 1], br[ct]);
+        if constexpr (CE) {
+          dmma_16x8x4(re[rt][ct], ai[2 * rt], ai[2 * rt + 1], bi[ct]);
+          dmma_16x8x4(im[rt][ct], ai[2 * rt], ai[2 * rt + 1], br[ct]);
+          dmma_16x8x4(im[rt][ct], -ar[2 * rt], -ar[2 * rt + 1], bi[ct]);
+        }
+      }
+  }
+  for (int w = 0; w < 8; ++w) {   // the warps, in order
+    if (warp == w) {
+#pragma unroll
+      for (int rt = 0; rt < 2; ++rt)
+#pragma unroll
+        for (int ct = 0; ct < 4; ++ct)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int i = rt * 16 + g + (e >> 1) * 8, j = ct * 8 + 2 * q + (e & 1);
+            double *p = s_blk + i * kRdmTile + j;
+            if (w == 0) { p[0] = re[rt][ct][e]; if (CE) p[kRdmTile * kRdmTile] = im[rt][ct][e]; }
+            else { p[0] += re[rt][ct][e]; if (CE) p[kRdmTile * kRdmTile] += im[rt][ct][e]; }
+          }
+    }
+    __syncthreads();
+  }
+  constexpr int size = (CE ? 2 : 1) * kRdmTile * kRdmTile;
+  double *out = partials + ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * size;
+  for (int e = threadIdx.x; e < size; e += blockDim.x) out[e] = s_blk[e];
+}
+
+// acc[2 (i d + j) + {0, 1}] += sum over the slices s in order of partials (i <= j's tile, i, j < d): one thread per
+// element of the computed tiles
+template <bool CE>
+__global__ void __launch_bounds__(256) k_rdm_reduce(const double *__restrict__ partials, int slices, int64_t tiles,
+                                                    int d, double *__restrict__ acc) {
+  constexpr int size = (CE ? 2 : 1) * kRdmTile * kRdmTile;
+  const int M = rdm_macro_dev(d);
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < tiles * kRdmTile * kRdmTile;
+       e += (int64_t)gridDim.x * blockDim.x) {
+    int t = (int)(e / (kRdmTile * kRdmTile)), I = 0;
+    const int f = (int)(e % (kRdmTile * kRdmTile));
+    while (t >= M - I) { t -= M - I; ++I; }
+    const int i = I * kRdmTile + f / kRdmTile, j = (I + t) * kRdmTile + f % kRdmTile;
+    if (i >= d || j >= d) continue;
+    const int64_t base = (e / (kRdmTile * kRdmTile)) * size + f;
+    double re = 0.0, im = 0.0;
+    for (int s = 0; s < slices; ++s) {
+      re += partials[(int64_t)s * tiles * size + base];
+      if (CE) im += partials[(int64_t)s * tiles * size + base + kRdmTile * kRdmTile];
+    }
+    acc[2 * ((int64_t)i * d + j)] += re;
+    if (CE) acc[2 * ((int64_t)i * d + j) + 1] += im;
+  }
+}
+
+// out = scale ρ with the lower triangle mirrored from the upper one (conj) and a real diagonal
+__global__ void __launch_bounds__(256) k_rdm_finish(const double *__restrict__ acc, int d, double scale,
+                                                    double *__restrict__ out) {
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < (int64_t)d * d;
+       e += (int64_t)gridDim.x * blockDim.x) {
+    const int i = (int)(e / d), j = (int)(e % d);
+    const double *p = acc + 2 * (i <= j ? e : (int64_t)j * d + i);
+    out[2 * e] = p[0] * scale;
+    out[2 * e + 1] = i == j ? 0.0 : (i < j ? p[1] : -p[1]) * scale;
+  }
+}
+
 }  // namespace
 
 int zz_gram_columns(int n_sites) { return 8 * zz_col_tiles(n_sites); }
@@ -706,6 +910,75 @@ SpinPlan spin_plan(const SpinBasis &src, const SpinBasis &tgt, int elt, int kind
   return S;
 }
 
+// ---- host half of dmv_reduced_density_matrix: the blocks of ρ_A and the checks of A
+struct RdmLayout {
+  int w_first = -1;           // weight of A of the first block; -1 at free weight (one block, every configuration)
+  std::vector<int> dims;      // d_w of the blocks, in ascending w
+  std::vector<int> ones_b;    // ones of B of the blocks (-1 at free weight)
+  size_t entries = 0;         // sum of d_w^2
+};
+
+RdmLayout rdm_layout(int n_sites, int hamming_weight, int n_a) {
+  if (n_sites < 1 || n_sites > 64) throw std::runtime_error("number_sites must be between 1 and 64");
+  if (hamming_weight < -1 || hamming_weight > n_sites)
+    throw std::runtime_error("hamming_weight must be -1 (free) or between 0 and " + std::to_string(n_sites) +
+                             " (got " + std::to_string(hamming_weight) + ")");
+  if (n_a < 1 || n_a > 16) throw std::runtime_error("n_a must be between 1 and 16 (got " + std::to_string(n_a) + ")");
+  if (n_a > n_sites)
+    throw std::runtime_error("n_a = " + std::to_string(n_a) + " exceeds the " + std::to_string(n_sites) + " sites");
+  RdmLayout L;
+  if (hamming_weight < 0) {
+    L.dims = {1 << n_a};
+    L.ones_b = {-1};
+  } else {
+    L.w_first = std::max(0, hamming_weight - (n_sites - n_a));
+    for (int w = L.w_first; w <= std::min(n_a, hamming_weight); ++w) {
+      L.dims.push_back((int)binom().c[n_a][w]);
+      L.ones_b.push_back(hamming_weight - w);
+    }
+  }
+  for (int d : L.dims) L.entries += (size_t)d * d;
+  return L;
+}
+
+// A's sites as one-bit masks (bit k of a configuration of A is sites[k]); B's sites ascending
+void rdm_sites(int n_sites, int n_a, const int32_t *sites, std::vector<uint64_t> &a, std::vector<uint64_t> &b) {
+  if (!sites) throw std::runtime_error("sites_a must not be null");
+  uint64_t seen = 0;
+  for (int k = 0; k < n_a; ++k) {
+    const int32_t s = sites[k];
+    if (s < 0 || s >= n_sites)
+      throw std::runtime_error("site " + std::to_string(s) + " of sites_a is outside [0, " + std::to_string(n_sites) + ")");
+    if (seen >> s & 1ull) throw std::runtime_error("site " + std::to_string(s) + " appears twice in sites_a");
+    seen |= 1ull << s;
+    a.push_back(1ull << s);
+  }
+  for (int s = 0; s < n_sites; ++s)
+    if (!(seen >> s & 1ull)) b.push_back(1ull << s);
+}
+
+// embed_A of the rows of the block of weight w (w < 0: every configuration), ascending in the local configuration
+std::vector<uint64_t> rdm_rows(const std::vector<uint64_t> &a, int w) {
+  std::vector<uint64_t> rows;
+  const int n_a = (int)a.size();
+  for (uint32_t l = 0; l < (1u << n_a); ++l) {
+    if (w >= 0 && __builtin_popcount(l) != w) continue;
+    uint64_t s = 0;
+    for (int k = 0; k < n_a; ++k)
+      if (l >> k & 1u) s |= a[k];
+    rows.push_back(s);
+  }
+  return rows;
+}
+
+// The column chunks of a block: at most kRdmChunk amplitudes, the columns a multiple of 32 (a function of d_w and K
+// alone, so neither the sums nor their order depend on free memory)
+constexpr int64_t kRdmChunk = int64_t(1) << 24;
+int64_t rdm_chunk_cols(int d, uint64_t K) {
+  const int64_t by_size = std::max<int64_t>(32, kRdmChunk / d / 32 * 32);
+  return std::min<int64_t>(by_size, (int64_t)((K + 31) / 32 * 32));
+}
+
 }  // namespace
 
 extern "C" {
@@ -910,6 +1183,189 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
   }
   yout.finish(st);
   check_status(source);   // synchronises
+  API_END
+}
+
+// ---- reduced density matrices (DESIGN.md section 3, "dmv_reduced_density_matrix"): per vector and block w of ρ_A, the
+// columns of B are cut into chunks (every P-th chunk on each rank); per chunk one k_rdm_fill pass writes its amplitudes
+// through the look-up of dmv_apply_spin, k_rdm_gram adds Ψ Ψᴴ per slice of columns and k_rdm_reduce adds the slices,
+// in order, to the block.  The blocks are all-reduced over the ranks, mirrored and divided by <x|x>.
+int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, int n_a,
+                               const int32_t *sites_a, double *rho) {
+  API_BEGIN
+  SolverRun run(ctx, elt, "dmv_reduced_density_matrix", true);
+  if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
+  if (!x) throw std::runtime_error("x must not be null");
+  if (!rho) throw std::runtime_error("rho must not be null");
+  const int N = ctx->n_sites, P = run.P;
+  const RdmLayout L = rdm_layout(N, ctx->hamming_weight, n_a);
+  std::vector<uint64_t> site_a, site_b;
+  rdm_sites(N, n_a, sites_a, site_a, site_b);
+  const int n_b = (int)site_b.size();
+  const size_t cw = run.ce ? 2 : 1;
+  // every size follows from the layout alone: the blocks, the largest chunk, its slices' partials, a host staging copy
+  std::vector<uint64_t> cols_total(L.dims.size());
+  size_t psi_words = 0, part_words = 0;
+  int max_d = 0;
+  for (size_t i = 0; i < L.dims.size(); ++i) {
+    const int d = L.dims[i];
+    cols_total[i] = L.ones_b[i] < 0 ? 1ull << n_b : binom().c[n_b][L.ones_b[i]];
+    const int64_t ld = rdm_chunk_cols(d, cols_total[i]);
+    psi_words = std::max(psi_words, (size_t)d * ld * cw);
+    part_words = std::max(part_words, (size_t)rdm_slices(d, ld) * rdm_tiles(d) * kRdmTile * kRdmTile * cw);
+    max_d = std::max(max_d, d);
+  }
+  const size_t acc_words = 2 * L.entries;
+  const bool host_out = !is_device_pointer(rho);
+  {
+    size_t free_b = 0, total_b = 0;
+    CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    const double need = 8.0 * ((double)acc_words * (host_out ? 1.0 + num_vectors : 1.0) + (double)psi_words +
+                               (double)part_words);
+    if (need > (double)free_b)
+      throw std::runtime_error("dmv_reduced_density_matrix: ρ of " + std::to_string(n_a) + " sites (" +
+                               std::to_string(L.entries) + " entries per vector) with its work space needs " +
+                               std::to_string((uint64_t)need) + " bytes, but only " + std::to_string(free_b) +
+                               " bytes are free on the device");
+  }
+  cudaStream_t st = run.st;
+  dmv_context *basis = ctx;   // where the states are looked up
+  if (P > 1) {
+    if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
+    if (!ctx->replicated)
+      throw std::runtime_error("dmv_reduced_density_matrix on several ranks needs the whole basis on every rank (the "
+                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
+                               "fit in device memory");
+    basis = ctx->global;
+  }
+  // <x|x> of every vector first: a zero vector is refused before anything is written
+  const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
+  double *d_norm2 = run.scalars(2 * (size_t)num_vectors), *q_part = run.partials(quad_partials(1));
+  for (int v = 0; v < num_vectors; ++v)
+    launch_quad_dot(run.n, run.ce, 1, xin.ptr + (size_t)v * run.words, xin.ptr + (size_t)v * run.words, q_part,
+                    d_norm2 + 2 * v, st);
+  run.all_reduce(d_norm2, 2 * (size_t)num_vectors);
+  std::vector<double> norm2(2 * (size_t)num_vectors);
+  CUDA_CHECK(cudaMemcpyAsync(norm2.data(), d_norm2, norm2.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  for (int v = 0; v < num_vectors; ++v)
+    if (!(norm2[2 * v] > 0.0))
+      throw std::runtime_error("x is a zero vector: <x|x> = 0 (vector " + std::to_string(v) + ")");
+
+  const bool trivial = ctx->proj != PROJ_GROUP || ctx->orbit.trivial_characters;
+  const int look = ctx->proj == PROJ_NONE        ? PM_NONE
+                   : ctx->proj == PROJ_INVERSION ? PM_INVERSION
+                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
+                                                                     : PM_GROUP;
+  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
+                                                            basis->opt.rows_ctas) : 0;
+  RdmArgs A{};
+  A.src.index = base_params(basis).index;
+  A.src.orbit = basis->orbit;
+  A.src.norms = basis->d_norms.ptr;
+  A.src.pos = P > 1 ? ctx->d_pos.ptr : nullptr;
+  A.src.site_mask = ctx->site_mask;
+  A.src.inversion_character = (double)ctx->spin_inversion;
+  A.src.n_sites = N;
+  A.src.status = ctx->d_status.ptr;
+  A.scale = ctx->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
+  A.n_b = n_b;
+  std::copy(site_b.begin(), site_b.end(), A.sites_b);
+  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
+    cudaStream_t keep = basis->stream;
+    basis->stream = st;
+    ensure_table(basis, elt);
+    basis->stream = keep;
+    A.src.table = basis->d_table.ptr;
+    A.src.table_slots = basis->table_slots;
+    A.src.table_dir = basis->table_dir;
+    A.src.dord = basis->dord;
+    A.src.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
+  }
+  std::vector<uint64_t> h_binom(64 * 65);
+  for (int n = 0; n < 64; ++n)
+    for (int k = 0; k <= 64; ++k) h_binom[n * 65 + k] = binom().c[n][k];
+  DevBuf<uint64_t> d_binom, d_rows;
+  DevBuf<double> d_acc, d_psi, d_part;
+  d_binom.upload(h_binom, st);
+  d_rows.alloc(max_d);
+  d_acc.alloc(acc_words);
+  d_psi.alloc(psi_words);
+  d_part.alloc(part_words);
+  A.binom = d_binom.ptr;
+  A.embed_a = d_rows.ptr;
+  A.psi = d_psi.ptr;
+  OutArg<double> out(rho, (size_t)num_vectors * acc_words);
+  int64_t amplitudes = 0, flops = 0;
+  for (int v = 0; v < num_vectors; ++v) {
+    const double *xv = xin.ptr + (size_t)v * run.words;
+    A.src.x = P > 1 ? gather_x(ctx, elt, xv) : xv;
+    if (look == PM_TABLE)
+      launch_table_fill(basis->n_states, run.ce, A.src.x, basis->d_norms.ptr, A.src.pos, basis->d_slot_of.ptr,
+                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
+    CUDA_CHECK(cudaMemsetAsync(d_acc.ptr, 0, acc_words * sizeof(double), st));
+    size_t off = 0;
+    for (size_t bi = 0; bi < L.dims.size(); ++bi) {
+      const int d = L.dims[bi];
+      const uint64_t K = cols_total[bi];
+      const int64_t ld = rdm_chunk_cols(d, K), tiles = rdm_tiles(d), slice_cols = rdm_slice_cols(d, ld);
+      const int slices = rdm_slices(d, ld);
+      const std::vector<uint64_t> rows = rdm_rows(site_a, L.ones_b[bi] < 0 ? -1 : L.w_first + (int)bi);
+      CUDA_CHECK(cudaMemcpyAsync(d_rows.ptr, rows.data(), rows.size() * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+      A.d = d;
+      A.k_b = L.ones_b[bi];
+      A.ld = ld;
+      const uint64_t n_chunks = (K + ld - 1) / ld;
+      for (uint64_t c = P > 1 ? (uint64_t)ctx->rank : 0; c < n_chunks; c += P) {   // every P-th chunk
+        A.col0 = (int64_t)(c * ld);
+        A.cols = (int64_t)std::min<uint64_t>(ld, K - c * ld);
+        with_rdm_fill(look, tk, run.ce, [&](auto kernel) {
+          const int64_t work = (d + kRdmRowGroup - 1) / kRdmRowGroup * ld;
+          kernel<<<one_wave(kernel, (work + kRdmThreads - 1) / kRdmThreads, 0, kRdmThreads), kRdmThreads, 0, st>>>(A);
+          check_launch("k_rdm_fill");
+        });
+        with_bool(run.ce, [&](auto ce) {
+          k_rdm_gram<ce()><<<dim3((unsigned)tiles, (unsigned)slices), 256, 0, st>>>(d_psi.ptr, ld, d, ld, slice_cols,
+                                                                                   d_part.ptr);
+          check_launch("k_rdm_gram");
+          const int grid = one_wave(k_rdm_reduce<ce()>, (tiles * kRdmTile * kRdmTile + 255) / 256, 0, 256);
+          k_rdm_reduce<ce()><<<grid, 256, 0, st>>>(d_part.ptr, slices, tiles, d, d_acc.ptr + off);
+          check_launch("k_rdm_reduce");
+        });
+        amplitudes += (int64_t)d * A.cols;
+        flops += tiles * kRdmTile * kRdmTile * ld * (run.ce ? 4 : 1);
+      }
+      off += 2 * (size_t)d * d;
+    }
+    run.all_reduce(d_acc.ptr, acc_words);
+    off = 0;
+    for (const int d : L.dims) {
+      const int grid = one_wave(k_rdm_finish, ((int64_t)d * d + 255) / 256, 0, 256);
+      k_rdm_finish<<<grid, 256, 0, st>>>(d_acc.ptr + off, d, 1.0 / norm2[2 * v], out.ptr + (size_t)v * acc_words + off);
+      check_launch("k_rdm_finish");
+      off += 2 * (size_t)d * d;
+    }
+  }
+  out.finish(st);
+  check_status(ctx);   // synchronises
+  ctx->rdm_amplitudes = amplitudes;
+  ctx->rdm_gram_flops = flops;
+  API_END
+}
+
+// host-only layout of dmv_reduced_density_matrix (no device needed)
+int dmv_rdm_layout(int n_sites, int hamming_weight, int n_a, const int32_t *sites_a, int *num_blocks, int *w_first,
+                   int32_t *dims) {
+  API_BEGIN
+  if (!num_blocks) throw std::runtime_error("num_blocks must not be null");
+  const RdmLayout L = rdm_layout(n_sites, hamming_weight, n_a);
+  if (sites_a) {
+    std::vector<uint64_t> a, b;
+    rdm_sites(n_sites, n_a, sites_a, a, b);
+  }
+  *num_blocks = (int)L.dims.size();
+  if (w_first) *w_first = L.w_first;
+  if (dims) std::copy(L.dims.begin(), L.dims.end(), dims);
   API_END
 }
 

@@ -442,6 +442,52 @@ class Operator:
                                            _ptr(x), _ptr(y)))
         return y
 
+    def reduced_density_matrix(self, x, sites):
+        """ρ_A = Tr_B |ψ><ψ| of ψ = B x / ‖x‖ for the sites A = `sites` (1 to 16 distinct sites; bit k of a row of ρ_A is
+        site sites[k]) on the device (dmv_reduced_density_matrix).  x as for zz_correlations.  Collective when
+        num_ranks > 1.  -> {w: complex128 ndarray (d_w, d_w)} by the weight w of A (key None at free weight; see
+        entanglement.block_layout), or a list of such dicts for a batch."""
+        from .entanglement import block_layout
+        elt = _elt_of(x)
+        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        sites_a = np.ascontiguousarray(np.asarray(sites, dtype=np.int32).reshape(-1))
+        layout = block_layout(N, self.spec.basis.hamming_weight, int(sites_a.shape[0]))
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        if _is_torch(x):
+            self.use_torch_stream()
+            x = x.contiguous()
+        else:
+            x = np.ascontiguousarray(x)
+        out = np.zeros((k, sum(d * d for _, d in layout)), dtype=np.complex128)
+        nat.check(nat.lib().dmv_reduced_density_matrix(self._ctx, elt, k, _ptr(x), int(sites_a.shape[0]),
+                                                       sites_a.ctypes.data, out.ctypes.data))
+        result = []
+        for v in range(k):
+            blocks, off = {}, 0
+            for w, d in layout:
+                blocks[w] = out[v, off:off + d * d].reshape(d, d)
+                off += d * d
+            result.append(blocks)
+        return result[0] if x.ndim == 1 else result
+
+    def entanglement_entropy(self, x, sites, alpha=1):
+        """The Rényi entropy S_α(A) (α = 1: von Neumann, natural logarithm) of ψ = B x / ‖x‖ for the sites A, from
+        reduced_density_matrix and entanglement.renyi_entropy.  When A has more sites than its complement B, ρ_B is
+        computed instead: for a pure state ρ_A and ρ_B have the same non-zero spectrum, so S(A) = S(B).  -> float, or
+        an ndarray for a batch."""
+        from .entanglement import entanglement_spectrum, renyi_entropy
+        N = self.spec.basis.number_sites
+        sites = [int(s) for s in np.asarray(sites).reshape(-1)]
+        rest = [s for s in range(N) if s not in set(sites)]
+        if 0 < len(rest) < len(sites):
+            sites = rest
+        rho = self.reduced_density_matrix(x, sites)
+        if isinstance(rho, dict):
+            return renyi_entropy(entanglement_spectrum(rho), alpha)
+        return np.array([renyi_entropy(entanglement_spectrum(r), alpha) for r in rho])
+
     def lanczos_quadrature(self, num_vectors: int, steps: int, seed: int = 42, start=None,
                            complex_vectors: bool = False):
         """Finite-temperature Lanczos (stochastic Lanczos quadrature) on the device (dmv_lanczos_quadrature): for each

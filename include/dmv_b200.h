@@ -352,6 +352,35 @@ enum { DMV_SPIN_ONE = 0, DMV_SPIN_Z = 1, DMV_SPIN_PLUS = 2, DMV_SPIN_MINUS = 3 }
 int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
                    int num_vectors, const void *x, void *y);
 
+/* ---- bipartite entanglement on the device (row f9; not in the reference): the reduced density matrix
+ * ρ_A = Tr_B |ψ><ψ| of the normalised full-space state ψ = B x / ‖x‖ (B the basis of dmv_apply_spin, so
+ * ψ(s) = χ n x[rep(s)] / ‖x‖), for a set A of n_a sites (1 <= n_a <= 16, distinct, in [0, N)).  Bit k of a local
+ * configuration of A is site sites_a[k], so the order of the list matters; B is the complement, its sites ascending.
+ * At a fixed Hamming weight W, ρ_A is block diagonal in the weight w of A: blocks w = max(0, W - (N - n_a)) ...
+ * min(n_a, W), of dimension d_w = C(n_a, w), rows the local configurations of weight w in ascending numeric order.  At
+ * free weight one block of dimension 2^n_a, rows 0 ... 2^n_a - 1.  dmv_rdm_layout gives the blocks (no device needed):
+ * *num_blocks, *w_first (-1 at free weight; may be NULL) and dims (room for 17 entries; may be NULL), with the checks
+ * of n_a and, when sites_a is not NULL, of the sites.
+ * rho (host or device): num_vectors * Σ_w d_w² complex numbers, interleaved (re, im), every block row-major, one after
+ * another in ascending w, vector after vector.  Hermitian by construction (the lower triangle mirrors the upper one, the
+ * diagonal is real); real x with real characters gives imaginary parts of exactly 0.  Tr ρ = 1 to rounding (not
+ * imposed).  x: num_vectors vectors [num_vectors, n] of this rank's hashed block, host or device; elt = DMV_C128 always,
+ * DMV_F64 only when info "complex_coefficients" == 0.  Refused with a message, and nothing written: a zero vector,
+ * duplicate sites or sites out of range, n_a outside 1..16, and a ρ whose blocks, work space and (for host rho) staging
+ * copy do not fit in free device memory (the message names the bytes).
+ * Method: per block, the columns b of B (combinadic order at a fixed weight) are cut into chunks of at most 2^24
+ * amplitudes, a function of (N, W, A) alone.  k_rdm_fill writes Ψ[a, c] = ψ(embed_A(a) | embed_B(b_c)) of a chunk through
+ * the orbit minimum and look-up of dmv_apply_spin; k_rdm_gram adds Ψ Ψᴴ on the FP64 tensor cores (tiles of 32 x 32 on or
+ * above the diagonal, a fixed number of column slices summed in order, chunks added in order).  No floating-point
+ * atomics: a repeated call is bit-identical.  Collective when num_ranks > 1 (needs dmv_comm_init and the whole basis on
+ * every rank, as dmv_apply_spin): rank r takes chunks r, r + P, ...; the blocks are summed over the ranks and every rank
+ * returns the same ρ.  dmv_get_info: "rdm_amplitudes" (amplitudes this rank filled in the last call) and
+ * "rdm_gram_flops" (real FP64 multiply-adds its Gram ran, padded tiles included). */
+int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, int n_a,
+                               const int32_t *sites_a, double *rho);
+int dmv_rdm_layout(int n_sites, int hamming_weight, int n_a, const int32_t *sites_a, int *num_blocks, int *w_first,
+                   int32_t *dims);
+
 /* ---- finite-temperature Lanczos on the device (row f6; not in the reference): the random-vector quadrature of the
  * finite-temperature Lanczos method (Jaklič & Prelovšek 1994), also called stochastic Lanczos quadrature.  For each of
  * num_vectors start vectors r, `steps` steps of the three-term recurrence (no reorthogonalisation, no stored basis) give
