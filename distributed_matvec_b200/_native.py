@@ -35,7 +35,12 @@ class OperatorDesc(C.Structure):
     ]
 
 
+class ParticlesDesc(C.Structure):
+    _fields_ = [("particle_type", C.c_int32), ("number_particles", C.c_int32), ("number_up", C.c_int32)]
+
+
 DMV_F64, DMV_C128 = 1, 2
+DMV_SPIN, DMV_SPINLESS_FERMION, DMV_SPINFUL_FERMION = 0, 1, 2
 
 # every symbol include/dmv_b200.h declares: (name, restype, argtypes)
 _SIGNATURES = [
@@ -46,6 +51,8 @@ _SIGNATURES = [
     ("dmv_launch_count", C.c_int64, []),
     ("dmv_context_create", C.c_int, [C.POINTER(BasisDesc), C.POINTER(OperatorDesc), C.c_int, C.c_int, C.c_int,
                                      C.POINTER(C.c_void_p)]),
+    ("dmv_context_create_particles", C.c_int, [C.POINTER(BasisDesc), C.POINTER(ParticlesDesc), C.POINTER(OperatorDesc),
+                                                C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
     ("dmv_context_destroy", C.c_int, [C.c_void_p]),
     ("dmv_set_stream", C.c_int, [C.c_void_p, C.c_void_p, C.c_int]),
     ("dmv_synchronize", C.c_int, [C.c_void_p]),

@@ -6,6 +6,16 @@ by the third-party ``ls_hs_load_yaml_config`` in the reference.  The YAML schema
 
     basis: {number_spins, hamming_weight, spin_inversion, symmetries: [{permutation, sector}]}
     hamiltonian: {terms: [{expression | matrix, sites}]}
+
+plus the basis' particle type (``ls_hs_basis.particle_type``, reference src/FFI.chpl:85-99):
+
+    basis: {particle: spin-1/2 (default) | spinless-fermion | spinful-fermion,
+            number_sites, number_particles, number_up}
+
+A spinless-fermion basis has ``number_sites`` bits, bit i the occupation of site i; with ``number_particles`` it is the
+fixed-weight basis.  A spinful-fermion basis of N = ``number_sites`` <= 32 sites has 2N bits: bit i is the up occupation
+of site i and bit N + i its down occupation, so a state is ``(down << N) | up``; ``number_particles`` and ``number_up``
+are both required.  Fermionic bases take no symmetries, spin inversion or ``hamming_weight``.
 """
 from __future__ import annotations
 
@@ -15,18 +25,37 @@ from math import comb
 import numpy as np
 import yaml
 
-from .expr import TermTable, compile_terms, max_number_off_diag
+from .expr import FermionModes, TermTable, compile_terms, max_number_off_diag
 from .symmetry import SymmetryGroup, build_group
+
+
+SPIN, SPINLESS_FERMION, SPINFUL_FERMION = "spin-1/2", "spinless-fermion", "spinful-fermion"
+PARTICLE_TYPES = (SPIN, SPINLESS_FERMION, SPINFUL_FERMION)
 
 
 @dataclass
 class BasisSpec:
-    """Flat description of a spin basis (what ``ls_hs_basis`` carries, src/FFI.chpl:94-105)."""
+    """Flat description of a basis (what ``ls_hs_basis`` carries, src/FFI.chpl:85-105).  For fermions
+    ``hamming_weight`` is the particle number, the weight over all ``number_bits`` bits."""
     number_sites: int
     hamming_weight: int | None
     spin_inversion: int            # 0 = none
     generators: list[dict] = field(default_factory=list)
     _group: SymmetryGroup | None = None
+    particle_type: str = SPIN
+    number_particles: int | None = None
+    number_up: int | None = None   # spinful fermions only
+
+    @property
+    def number_bits(self) -> int:
+        """Bits of a basis state: 2N for spinful fermions on N sites, N otherwise."""
+        return 2 * self.number_sites if self.particle_type == SPINFUL_FERMION else self.number_sites
+
+    def is_fermionic(self) -> bool:
+        return self.particle_type != SPIN
+
+    def fermion_modes(self) -> FermionModes | None:
+        return FermionModes(self.number_sites, self.particle_type == SPINFUL_FERMION) if self.is_fermionic() else None
 
     # -- flags, named after the reference's Basis methods (src/ForeignTypes.chpl:82-100) --------
     def is_hamming_weight_fixed(self) -> bool:
@@ -54,6 +83,9 @@ class BasisSpec:
         """Smallest candidate state (mirror of ``ls_hs_min_state_estimate``, src/FFI.chpl:147)."""
         if self.hamming_weight is None:
             return 0
+        if self.particle_type == SPINFUL_FERMION:
+            n, up = self.number_sites, self.number_up
+            return (((1 << (self.hamming_weight - up)) - 1) << n) | ((1 << up) - 1)
         return (1 << self.hamming_weight) - 1
 
     def max_state_estimate(self) -> int:
@@ -61,7 +93,10 @@ class BasisSpec:
 
         With spin inversion every representative satisfies s <= s ^ mask, so the top site is
         never set (SURVEY.md App. A.2); the bound excludes it."""
-        n, w = self.number_sites, self.hamming_weight
+        n, w = self.number_bits, self.hamming_weight
+        if self.particle_type == SPINFUL_FERMION:
+            up, down, half = self.number_up, w - self.number_up, self.number_sites
+            return (((1 << down) - 1) << (n - down)) | (((1 << up) - 1) << (half - up))
         if w is None:
             hi = (1 << n) - 1
             if self.has_spin_inversion_symmetry():
@@ -74,8 +109,16 @@ class BasisSpec:
         return hi
 
     def number_candidates(self) -> int:
-        n, w = self.number_sites, self.hamming_weight
+        n, w = self.number_bits, self.hamming_weight
         return comb(n, w) if w is not None else 1 << n
+
+    def number_states(self) -> int | None:
+        """Dimension of a fermionic or symmetry-free basis: C(N, N_up) C(N, N_down) for spinful fermions."""
+        if self.particle_type == SPINFUL_FERMION:
+            return comb(self.number_sites, self.number_up) * comb(self.number_sites, self.hamming_weight - self.number_up)
+        if self.requires_projection():
+            return None
+        return self.number_candidates()
 
 
 @dataclass
@@ -96,7 +139,43 @@ class OperatorSpec:
         return self.off_diag.is_real() and self.diag.is_real()
 
 
+def _fermion_basis_from_dict(d: dict, particle: str) -> BasisSpec:
+    for key in ("symmetries", "spin_inversion", "hamming_weight", "number_spins"):
+        if d.get(key) is not None:
+            raise ValueError(f"{particle} basis: '{key}' is not supported (fermionic bases take number_sites, "
+                             "number_particles and, for spinful fermions, number_up)")
+    if "number_sites" not in d:
+        raise ValueError(f"{particle} basis needs number_sites")
+    n = int(d["number_sites"])
+    np_, nu = d.get("number_particles"), d.get("number_up")
+    if particle == SPINLESS_FERMION:
+        if not 0 < n <= 64:
+            raise ValueError(f"spinless-fermion basis: number_sites must be between 1 and 64 (got {n})")
+        if nu is not None:
+            raise ValueError("spinless-fermion basis: 'number_up' is for spinful fermions")
+        if np_ is not None and not 0 <= int(np_) <= n:
+            raise ValueError(f"spinless-fermion basis: number_particles must be between 0 and {n} (got {np_})")
+        w = None if np_ is None else int(np_)
+        return BasisSpec(number_sites=n, hamming_weight=w, spin_inversion=0, particle_type=particle,
+                         number_particles=w)
+    if not 0 < n <= 32:
+        raise ValueError(f"spinful-fermion basis: number_sites must be between 1 and 32 (got {n})")
+    if np_ is None or nu is None:
+        raise ValueError("spinful-fermion basis needs both number_particles and number_up")
+    np_, nu = int(np_), int(nu)
+    if not (0 <= nu <= n and 0 <= np_ - nu <= n):
+        raise ValueError(f"spinful-fermion basis: need 0 <= number_up <= {n} and 0 <= number_particles - number_up <= "
+                         f"{n} (got number_particles {np_}, number_up {nu})")
+    return BasisSpec(number_sites=n, hamming_weight=np_, spin_inversion=0, particle_type=particle,
+                     number_particles=np_, number_up=nu)
+
+
 def basis_from_dict(d: dict) -> BasisSpec:
+    particle = d.get("particle", SPIN)
+    if particle not in PARTICLE_TYPES:
+        raise ValueError(f"unknown particle type {particle!r}: expected one of {', '.join(PARTICLE_TYPES)}")
+    if particle != SPIN:
+        return _fermion_basis_from_dict(d, particle)
     n = int(d["number_spins"])
     if not 0 < n <= 64:
         raise ValueError("bases with more than 64 bits are not yet implemented")  # DMV:1099-1100
@@ -112,7 +191,7 @@ def basis_from_dict(d: dict) -> BasisSpec:
 
 
 def operator_from_dict(d: dict, basis: BasisSpec) -> OperatorSpec:
-    off, diag = compile_terms(d["terms"], basis.number_sites)
+    off, diag = compile_terms(d["terms"], basis.number_sites, basis.fermion_modes())
     return OperatorSpec(basis=basis, off_diag=off, diag=diag, name=str(d.get("name", "")))
 
 

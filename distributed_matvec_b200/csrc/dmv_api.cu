@@ -188,7 +188,7 @@ KernelParams base_params(dmv_context *ctx) {
   p.index.dir = ctx->d_dir.ptr;
   p.index.n_buckets = ctx->n_buckets;
   p.index.shift = ctx->dir_shift;
-  p.index.mode = ctx->index_mode;
+  p.index.mode = lin_tables(ctx->index_mode) ? INDEX_LIN : ctx->index_mode;
   p.index.binom = ctx->d_binom.ptr;
   p.index.stride = ctx->binom_stride;
   p.index.n_sites = ctx->n_sites;
@@ -346,6 +346,27 @@ void select_index_mode(dmv_context *ctx) {
   if (want == 0) return;
   const bool eligible = ctx->num_ranks == 1 && w >= 0 && ctx->proj != PROJ_GROUP;
   if (!eligible) return;
+  if (ctx->particle_type == DMV_SPINFUL_FERMION) {
+    // the Lin tables split at bit N (INDEX_LIN_SPLIT); the combinadic rank counts states of the wrong half weights
+    const int N = n / 2, n_up = ctx->number_up, n_dn = w - n_up;
+    const uint64_t per_hi = binom().c[N][n_up], total = binom().c[N][n_dn] * per_hi;
+    if (want == 2 || N > 20 || (uint64_t)ctx->n_states != total || total >= (1ull << 32)) return;
+    std::vector<uint32_t> ja((size_t)1 << N), jb((size_t)1 << N);
+    uint32_t r_hi = 0, r_lo = 0;
+    for (uint64_t h = 0; h < (1ull << N); ++h) {
+      ja[h] = __builtin_popcountll(h) == n_dn ? (uint32_t)(r_hi++ * per_hi) : 0xffffffffu;
+      jb[h] = __builtin_popcountll(h) == n_up ? r_lo++ : 0u;
+    }
+    ctx->d_lin_a.upload(ja, ctx->stream);
+    ctx->d_lin_b.upload(jb, ctx->stream);
+    ctx->lin_bits = N;
+    StateIndex ix{};
+    ix.reps = ctx->d_reps.ptr; ix.n = ctx->n_states; ix.n_sites = n; ix.weight = w; ix.site_mask = ctx->site_mask;
+    ix.mode = INDEX_LIN; ix.lin_a = ctx->d_lin_a.ptr; ix.lin_b = ctx->d_lin_b.ptr; ix.lin_bits = N;
+    ctx->rank_total = total;
+    if (index_verified(ctx, ix)) ctx->index_mode = INDEX_LIN_SPLIT;
+    return;
+  }
   const uint64_t total = binom().c[n][w];
   const uint64_t expect = (ctx->proj == PROJ_INVERSION) ? total / 2 : total;
   if ((uint64_t)ctx->n_states != expect || total >= (1ull << 32)) return;
@@ -899,7 +920,7 @@ void do_generate(dmv_context *ctx, int elt, const void *x_dev, void *y_dev,
       p.row_split = gather_row_split(ctx, ctx->n_states);
       p.uni_re = ctx->gather_uni[0]; p.uni_im = ctx->gather_uni[1];
       launch_gather(p, ctx->proj == PROJ_INVERSION, ctx->complex_coefficients, elt == DMV_C128,
-                    ctx->gather_narrow, ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);
+                    ctx->gather_narrow, lin_tables(ctx->index_mode), ctx->gather_uniform, ctx->stream);
       return;
     }
     if (use_rows(ctx)) {
@@ -1069,6 +1090,45 @@ void invalidate(dmv_context *c, unsigned stale) {
 
 }  // namespace
 
+const char *particle_name(int type) {
+  return type == DMV_SPINLESS_FERMION ? "spinless-fermion" : type == DMV_SPINFUL_FERMION ? "spinful-fermion" : "spin-1/2";
+}
+
+void require_spin(const dmv_context *ctx, const char *entry) {
+  if (ctx && ctx->particle_type != DMV_SPIN)
+    throw std::runtime_error(std::string(entry) + ": not defined on a " + particle_name(ctx->particle_type) +
+                             " basis (it assumes spin operators without Jordan-Wigner strings)");
+}
+
+// the particle numbers of a fermionic basis, checked before anything is allocated
+void check_particles(const dmv_basis_desc *basis, const dmv_particles_desc *pt) {
+  const int type = pt->particle_type, bits = basis->number_sites;
+  if (type != DMV_SPIN && type != DMV_SPINLESS_FERMION && type != DMV_SPINFUL_FERMION)
+    throw std::runtime_error("particle_type must be DMV_SPIN, DMV_SPINLESS_FERMION or DMV_SPINFUL_FERMION (got " +
+                             std::to_string(type) + ")");
+  if (type == DMV_SPIN) return;
+  const std::string what = particle_name(type);
+  if (basis->has_permutations || basis->spin_inversion != 0)
+    throw std::runtime_error(what + " basis: permutation symmetries and spin inversion are not supported for fermions");
+  if (basis->hamming_weight != pt->number_particles)
+    throw std::runtime_error(what + " basis: hamming_weight (" + std::to_string(basis->hamming_weight) +
+                             ") must equal number_particles (" + std::to_string(pt->number_particles) + ")");
+  if (type == DMV_SPINLESS_FERMION) {
+    if (pt->number_particles < -1 || pt->number_particles > bits)
+      throw std::runtime_error(what + " basis: number_particles must be -1 (free) or between 0 and " +
+                               std::to_string(bits) + " (got " + std::to_string(pt->number_particles) + ")");
+    return;
+  }
+  if (bits % 2 != 0)
+    throw std::runtime_error(what + " basis: number_sites counts bits and must be even, 2N for N sites (got " +
+                             std::to_string(bits) + ")");
+  const int N = bits / 2, up = pt->number_up, down = pt->number_particles - pt->number_up;
+  if (up < 0 || up > N || down < 0 || down > N)
+    throw std::runtime_error(what + " basis: need 0 <= number_up <= " + std::to_string(N) +
+                             " and 0 <= number_particles - number_up <= " + std::to_string(N) + " (got number_particles " +
+                             std::to_string(pt->number_particles) + ", number_up " + std::to_string(up) + ")");
+}
+
 } }  // namespace dmv::host
 
 extern "C" {
@@ -1080,10 +1140,17 @@ int64_t dmv_launch_count(void) { return launch_counter(); }
 
 int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op, int device, int rank,
                        int num_ranks, dmv_context **out) {
+  const dmv_particles_desc spin{DMV_SPIN, -1, -1};
+  return dmv_context_create_particles(basis, &spin, op, device, rank, num_ranks, out);
+}
+
+int dmv_context_create_particles(const dmv_basis_desc *basis, const dmv_particles_desc *particles,
+                                 const dmv_operator_desc *op, int device, int rank, int num_ranks, dmv_context **out) {
   API_BEGIN
-  if (!basis || !op || !out) throw std::runtime_error("null argument");
+  if (!basis || !particles || !op || !out) throw std::runtime_error("null argument");
   if (basis->number_sites <= 0 || basis->number_sites > 64)
     throw std::runtime_error("bases with more than 64 bits are not yet implemented");  // DMV:1099-1100
+  check_particles(basis, particles);
   if (num_ranks < 1 || num_ranks > 256 || rank < 0 || rank >= num_ranks)
     throw std::runtime_error("need 0 <= rank < num_ranks <= 256");                     // DMV:664: uint8 keys
   int n_dev = 0;
@@ -1103,6 +1170,9 @@ int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op,
   for (auto &e : ctx->ev_chunk) CUDA_CHECK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   ctx->n_sites = basis->number_sites;
   ctx->hamming_weight = basis->hamming_weight;
+  ctx->particle_type = particles->particle_type;
+  if (ctx->particle_type != DMV_SPIN) ctx->number_particles = particles->number_particles;
+  if (ctx->particle_type == DMV_SPINFUL_FERMION) ctx->number_up = particles->number_up;
   ctx->spin_inversion = basis->spin_inversion;
   ctx->has_permutations = basis->has_permutations != 0;
   ctx->site_mask = basis->number_sites == 64 ? ~0ull : ((1ull << basis->number_sites) - 1);
@@ -1152,7 +1222,11 @@ int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op,
     // bits only; it runs in 32-bit registers when sites and groups fit, and skips the LUT when every emitting
     // (group, support bits) pair carries the same coefficient (every Heisenberg-type operator)
     const HostTables &H = ctx->h_pull;
-    ctx->gather_ok = !H.bp.empty() && !H.any_s_out && !H.any_generic;
+    // (a group's sign mask lies outside its support, so k_gather applies it to the row state: see dmv_gather.cu.  With
+    // spin inversion the target is canonicalised, and k_gather has no build for both: such operators keep to k_pull /
+    // k_generate, as they did before sign masks reached k_gather)
+    ctx->gather_ok = !H.bp.empty() && !H.any_generic && !(H.any_s_out && ctx->proj == PROJ_INVERSION);
+    ctx->gather_signs = ctx->gather_ok && H.any_s_out;
     ctx->gather_narrow = basis->number_sites <= 32 && H.groups.size() <= 32;
     bool first = true, uniform = ctx->gather_ok;
     for (size_t g = 0; g < H.groups.size() && uniform; ++g)
@@ -1241,6 +1315,8 @@ int64_t dmv_get_info(const dmv_context *ctx, const char *name) {
   if (!ctx) return -1;
   if (key.compare(0, 7, "global.") == 0) return ctx->global ? dmv_get_info(ctx->global, key.c_str() + 7) : -1;
   if (key == "index_mode") return ctx->index_mode;
+  if (key == "particle_type") return ctx->particle_type;
+  if (key == "gather_signs") return ctx->gather_signs ? 1 : 0;
   if (key == "pull") return use_pull(ctx) ? 1 : 0;
   if (key == "gather")
     return ((use_pull(ctx) && use_gather(ctx)) || (ctx->replicated && ctx->global && use_gather(ctx->global))) ? 1 : 0;
@@ -1328,6 +1404,19 @@ int dmv_set_representatives(dmv_context *ctx, const uint64_t *representatives, i
   use_device(ctx);
   if (count < 0 || (count > 0 && !representatives)) throw std::runtime_error("bad representatives");
   if (count >= (1ll << 32)) throw std::runtime_error("more than 2^32 states per rank are not supported");
+  if (ctx->particle_type == DMV_SPINFUL_FERMION && count > 0) {
+    // every state needs number_up up and number_particles - number_up down particles, as the split index assumes
+    std::vector<uint64_t> h((size_t)count);
+    CUDA_CHECK(cudaMemcpy(h.data(), representatives, (size_t)count * 8, cudaMemcpyDefault));
+    const int N = ctx->n_sites / 2;
+    const uint64_t up_mask = (1ull << N) - 1;
+    for (uint64_t v : h)
+      if (__builtin_popcountll(v & up_mask) != ctx->number_up ||
+          __builtin_popcountll(v & ~up_mask) != ctx->number_particles - ctx->number_up || (v & ~ctx->site_mask) != 0)
+        throw std::runtime_error("spinful-fermion basis: state " + std::to_string(v) + " does not have " +
+                                 std::to_string(ctx->number_up) + " up and " +
+                                 std::to_string(ctx->number_particles - ctx->number_up) + " down particles");
+  }
   ctx->d_reps.alloc((size_t)count);
   if (count > 0)
     CUDA_CHECK(cudaMemcpyAsync(ctx->d_reps.ptr, representatives, (size_t)count * 8, cudaMemcpyDefault, ctx->stream));
@@ -1353,9 +1442,17 @@ int dmv_basis_build(dmv_context *ctx) {
   const bool fixed = w >= 0;
   // candidate range (mirror of ls_hs_min/max_state_estimate, reference src/ForeignTypes.chpl:102-109);
   // with spin inversion the top site is never set in a representative (SURVEY.md App. A.2)
-  uint64_t lo, hi;
+  uint64_t lo, hi, half_mask = 0;
   const bool inv = ctx->spin_inversion != 0;
-  if (fixed) {
+  if (ctx->particle_type == DMV_SPINFUL_FERMION) {
+    // (down << N) | up with both halves at fixed weight: the fixed-weight candidates over 2N bits between the smallest
+    // and the largest such state, filtered by the weight of the up half
+    const int N = n / 2, up = ctx->number_up, down = w - up;
+    auto low = [](int k) { return k == 0 ? 0ull : ((1ull << k) - 1); };
+    lo = (low(down) << N) | low(up);
+    hi = (down == 0 ? 0ull : low(down) << (n - down)) | (low(up) << (N - up));
+    half_mask = low(N);
+  } else if (fixed) {
     if (w > n) throw std::runtime_error("hamming weight exceeds the number of sites");
     lo = w == 0 ? 0 : ((w == 64) ? ~0ull : ((1ull << w) - 1));
     const int top = (inv && n - 1 >= w) ? n - 1 : n;
@@ -1390,8 +1487,8 @@ int dmv_basis_build(dmv_context *ctx) {
   d_last.upload(h_last, ctx->stream);
   d_count.alloc((size_t)n_chunks);
   d_offset.alloc((size_t)n_chunks);
-  launch_enumerate(ctx->orbit, ctx->proj, ctx->site_mask, fixed, ctx->rank, ctx->num_ranks, n_chunks,
-                   d_first.ptr, d_last.ptr, d_count.ptr, d_offset.ptr, nullptr, nullptr, false, ctx->stream);
+  launch_enumerate(ctx->orbit, ctx->proj, ctx->site_mask, fixed, half_mask, ctx->number_up, ctx->rank, ctx->num_ranks,
+                   n_chunks, d_first.ptr, d_last.ptr, d_count.ptr, d_offset.ptr, nullptr, nullptr, false, ctx->stream);
   std::vector<unsigned long long> h_count((size_t)n_chunks), h_offset((size_t)n_chunks);
   CUDA_CHECK(cudaMemcpyAsync(h_count.data(), d_count.ptr, sizeof(unsigned long long) * n_chunks,
                              cudaMemcpyDeviceToHost, ctx->stream));
@@ -1402,8 +1499,8 @@ int dmv_basis_build(dmv_context *ctx) {
   d_offset.upload(h_offset, ctx->stream);
   ctx->d_reps.alloc((size_t)acc);
   if (ctx->proj == PROJ_GROUP) ctx->d_norms.alloc((size_t)acc);
-  launch_enumerate(ctx->orbit, ctx->proj, ctx->site_mask, fixed, ctx->rank, ctx->num_ranks, n_chunks,
-                   d_first.ptr, d_last.ptr, d_count.ptr, d_offset.ptr, ctx->d_reps.ptr,
+  launch_enumerate(ctx->orbit, ctx->proj, ctx->site_mask, fixed, half_mask, ctx->number_up, ctx->rank, ctx->num_ranks,
+                   n_chunks, d_first.ptr, d_last.ptr, d_count.ptr, d_offset.ptr, ctx->d_reps.ptr,
                    ctx->proj == PROJ_GROUP ? ctx->d_norms.ptr : nullptr, true, ctx->stream);
   ctx->n_states = (int64_t)acc;
   install_directory(ctx);
@@ -1594,7 +1691,7 @@ int dmv_matvec_batch(dmv_context *ctx, int elt, int num_vectors, const void *x, 
       p.row_split = gather_row_split(ctx, ctx->n_states);
       p.uni_re = ctx->gather_uni[0]; p.uni_im = ctx->gather_uni[1];
       launch_gather(p, ctx->proj == PROJ_INVERSION, ctx->complex_coefficients, elt == DMV_C128, ctx->gather_narrow,
-                    ctx->index_mode == INDEX_LIN, ctx->gather_uniform, ctx->stream);
+                    lin_tables(ctx->index_mode), ctx->gather_uniform, ctx->stream);
     }
   }
   if (ctx->num_ranks == 1 && use_pull(ctx) && !use_gather(ctx) && use_rows_batch(ctx) &&

@@ -236,7 +236,9 @@ struct RowsStore {
 struct dmv_context {
   int device = 0, rank = 0, num_ranks = 1;
   // basis
-  int n_sites = 0, hamming_weight = -1, spin_inversion = 0;
+  int n_sites = 0, hamming_weight = -1, spin_inversion = 0;   // n_sites: bits of a state (2N for spinful fermions)
+  // DMV_SPIN / DMV_SPINLESS_FERMION / DMV_SPINFUL_FERMION (dmv_context_create_particles); number_up: spinful only
+  int particle_type = DMV_SPIN, number_particles = -1, number_up = -1;
   bool has_permutations = false;
   Projection proj = PROJ_NONE;
   bool identity_index = false;
@@ -268,6 +270,7 @@ struct dmv_context {
   Options opt;
   // k_gather applicability (set at context creation from the row-traversal tables)
   bool gather_ok = false, gather_narrow = false, gather_uniform = false;
+  bool gather_signs = false;   // the row tables carry sign masks outside the groups' supports (Jordan-Wigner strings)
   // k_rows applicability (bases with permutation symmetries, trivial characters, real bit-parallel operator) and its
   // hash table over this context's representatives (see table_slot in dmv_device.cuh)
   bool rows_ok = false;
@@ -451,6 +454,10 @@ struct Binomials {
 };
 const Binomials &binom();
 void select_index_mode(dmv_context *ctx);
+const char *particle_name(int particle_type);   // "spin-1/2", "spinless-fermion", "spinful-fermion"
+// the refusal of an observable that assumes spin operators without strings
+void require_spin(const dmv_context *ctx, const char *entry);
+inline bool lin_tables(int index_mode) { return index_mode == INDEX_LIN || index_mode == INDEX_LIN_SPLIT; }
 void install_directory(dmv_context *ctx);
 void upload_orbit(dmv_context *ctx);
 // lanes per row of a k_gather launch over `rows` rows with the tables of `g`: option "gather_split", else

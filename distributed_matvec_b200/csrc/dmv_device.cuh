@@ -170,7 +170,12 @@ __host__ __device__ __forceinline__ int locale_idx_of(uint64_t state, int num_ra
 // ---------------------------------------------------------------------------------------------
 //   INDEX_LIN       : same bases as INDEX_RANK: two-table (Lin) lookup  index = Ja[s >> h] + Jb[s & mask]:
 //                     two independent small-table loads, no dependent probe chain, bit-identical results.
-enum IndexMode { INDEX_DIRECTORY = 0, INDEX_IDENTITY = 1, INDEX_RANK = 2, INDEX_LIN = 3 };
+//   INDEX_LIN_SPLIT : spinful-fermion basis (hi = down half, lo = up half, both at fixed weight), ascending = (hi, lo)
+//                     lexicographic: Ja[hi] = rank of hi among the N_dn-weight words x C(N, N_up), Jb[lo] = rank of lo
+//                     among the N_up-weight words.  A wrong-weight hi has Ja = 0xffffffff and a wrong-weight lo Jb = 0:
+//                     at the right total weight both halves are wrong together, so the sum is >= n and never wraps.
+//                     The device runs it as INDEX_LIN (same look-up, other tables); only the host tells them apart.
+enum IndexMode { INDEX_DIRECTORY = 0, INDEX_IDENTITY = 1, INDEX_RANK = 2, INDEX_LIN = 3, INDEX_LIN_SPLIT = 4 };
 
 struct StateIndex {
   const uint64_t *reps;   // ascending, this rank's block

@@ -113,7 +113,10 @@ void setup_replicated(dmv_context *ctx) {
     o.diag_m = ctx->k_diag_m.data(); o.diag_r = ctx->k_diag_r.data(); o.diag_s = ctx->k_diag_s.data();
     // rough size check before enumerating: reps + directory + positions + gathered x
     double states = 1.0;
-    if (ctx->hamming_weight >= 0) states = (double)binom().c[ctx->n_sites][ctx->hamming_weight];
+    if (ctx->particle_type == DMV_SPINFUL_FERMION)
+      states = (double)binom().c[ctx->n_sites / 2][ctx->number_up] *
+               (double)binom().c[ctx->n_sites / 2][ctx->hamming_weight - ctx->number_up];
+    else if (ctx->hamming_weight >= 0) states = (double)binom().c[ctx->n_sites][ctx->hamming_weight];
     else states = std::ldexp(1.0, ctx->n_sites);
     if (ctx->spin_inversion != 0 && ctx->proj != PROJ_GROUP) states *= 0.5;
     if (ctx->proj == PROJ_GROUP) states = 1.5 * states / (double)std::max<int64_t>(1, ctx->k_group_order) + 1e4;
@@ -121,7 +124,8 @@ void setup_replicated(dmv_context *ctx) {
     CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
     if (states * 48.0 > 0.5 * (double)free_b) throw std::runtime_error("replicated-x product: the whole basis does not fit");
     dmv_context *g = nullptr;
-    if (dmv_context_create(&b, &o, ctx->device, 0, 1, &g) != 0) throw std::runtime_error(g_last_error);
+    const dmv_particles_desc pt{ctx->particle_type, ctx->number_particles, ctx->number_up};
+    if (dmv_context_create_particles(&b, &pt, &o, ctx->device, 0, 1, &g) != 0) throw std::runtime_error(g_last_error);
     ctx->global = g;
     // every option of the rank; "index" takes effect in the basis build.  ("mode", "exchange", "rounds", "peer_gather"
     // and "rows_batch*" steer single, collective and batched products, which nothing asks of the twin.)
@@ -176,7 +180,7 @@ void replicated_rows(dmv_context *ctx, int elt, const void *x_cat, void *y_dev) 
     p.row_split = gather_row_split(g, ctx->n_states);
     p.uni_re = g->gather_uni[0]; p.uni_im = g->gather_uni[1];
     launch_gather(p, g->proj == PROJ_INVERSION, g->complex_coefficients, elt == DMV_C128, g->gather_narrow,
-                  g->index_mode == INDEX_LIN, g->gather_uniform, ctx->stream);
+                  lin_tables(g->index_mode), g->gather_uniform, ctx->stream);
     return;
   }
   p.row_norms = ctx->d_norms.ptr;

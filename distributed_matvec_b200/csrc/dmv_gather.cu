@@ -13,6 +13,8 @@
 // in flight per lane.  With <= 32 sites and <= 32 groups the whole row runs in 32-bit registers (NARROW).
 // Only used when one rank owns the basis (the distributed product needs the scatter form: the owner of a
 // row does not hold the x of its neighbours).
+// SG: the groups carry sign masks s_out outside their flip supports (Jordan-Wigner strings of fermionic hops).  Row
+// state b and target b ^ x agree on those bits, so each emitted term is multiplied by (-1)^popc(b & s_out[g]).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -67,9 +69,9 @@ __device__ __forceinline__ double2 shfl_xor_v(double2 v, int m) {
 __device__ __forceinline__ void add_to(double &a, double b) { a += b; }
 __device__ __forceinline__ void add_to(double2 &a, double2 b) { a.x += b.x; a.y += b.y; }
 
-struct GatherLayout { size_t bp, dclass, diag, lut, gx, total; };
+struct GatherLayout { size_t bp, dclass, diag, lut, gx, sg, total; };
 __host__ __device__ inline GatherLayout gather_layout(const KernelParams &p, size_t word_bytes, size_t val_bytes,
-                                                      bool uniform) {
+                                                      bool uniform, bool signs) {
   GatherLayout L;
   size_t off = 0;
   L.bp = off; off += sizeof(BpWord) * (size_t)p.n_bp;
@@ -78,6 +80,7 @@ __host__ __device__ inline GatherLayout gather_layout(const KernelParams &p, siz
   off = (off + 15) / 16 * 16;
   L.lut = off; off += uniform ? 0 : val_bytes * (size_t)p.n_lut;
   L.gx = off; off += word_bytes * (size_t)p.n_groups;
+  L.sg = off; off += signs ? word_bytes * (size_t)p.n_groups : 0;
   L.total = (off + 15) / 16 * 16;
   return L;
 }
@@ -106,19 +109,20 @@ __device__ __forceinline__ uint32_t lin_index(const uint32_t *__restrict__ lin_a
   return r < n ? r : kNone;   // with spin inversion only the first half are representatives
 }
 
-template <bool INV, bool CV, bool CE, bool NARROW, bool LIN, bool UNI, int KB>
+template <bool INV, bool CV, bool CE, bool NARROW, bool LIN, bool UNI, bool SG, int KB>
 __global__ void __launch_bounds__(kThreads) k_gather(const KernelParams p) {
   using V = typename Val<CV>::type;            // coefficient type
   using E = typename Val<CE>::type;            // vector element type
   using A = typename Val<CV || CE>::type;      // row accumulator
   using W = typename std::conditional<NARROW, uint32_t, uint64_t>::type;
   extern __shared__ __align__(16) unsigned char smem[];
-  const GatherLayout L = gather_layout(p, sizeof(W), sizeof(V), UNI);
+  const GatherLayout L = gather_layout(p, sizeof(W), sizeof(V), UNI, SG);
   BpWord *s_bp = reinterpret_cast<BpWord *>(smem + L.bp);
   DiagClass *s_dclass = reinterpret_cast<DiagClass *>(smem + L.dclass);
   DiagTerm *s_diag = reinterpret_cast<DiagTerm *>(smem + L.diag);
   V *s_lut = reinterpret_cast<V *>(smem + L.lut);
   W *s_gx = reinterpret_cast<W *>(smem + L.gx);
+  W *s_sg = reinterpret_cast<W *>(smem + L.sg);
   {
     const uint64_t *src = reinterpret_cast<const uint64_t *>(p.bp);
     uint64_t *dst = reinterpret_cast<uint64_t *>(s_bp);
@@ -130,6 +134,8 @@ __global__ void __launch_bounds__(kThreads) k_gather(const KernelParams p) {
     if (!UNI)
       for (int i = threadIdx.x; i < p.n_lut; i += blockDim.x) s_lut[i] = reinterpret_cast<const V *>(p.lut)[i];
     for (int i = threadIdx.x; i < p.n_groups; i += blockDim.x) s_gx[i] = (W)p.groups[i].x;
+    if (SG)
+      for (int i = threadIdx.x; i < p.n_groups; i += blockDim.x) s_sg[i] = (W)p.groups[i].s_out;
   }
   __syncthreads();
 
@@ -207,6 +213,7 @@ __global__ void __launch_bounds__(kThreads) k_gather(const KernelParams p) {
         for (int j = 0; j < NB; ++j) {
           if (UNI) c[j] = uni;
           else c[j] = s_lut[4 * (g_base + g[j]) + ((unsigned)((a0 >> g[j]) & 1) | ((unsigned)((a1 >> g[j]) & 1) << 1))];
+          if (SG && (popc_w(b & s_sg[g_base + g[j]]) & 1)) c[j] = scale(c[j], -1.0);
           if (pos && idx[j] != kNone) idx[j] = __ldg(pos + idx[j]);
         }
         E xs[NB][KB];
@@ -499,14 +506,19 @@ void launch_gather(const KernelParams &p, bool inversion, bool complex_values, b
   with_bool(narrow, [&](auto nw) {
   with_bool(lin, [&](auto ln) {
   with_bool(uniform, [&](auto uni) {
+  with_bool(p.any_s_out != 0, [&](auto sg) {
   with_choice<1, 4>(p.batch == 4 ? 4 : 1, [&](auto kb) {
-    auto kernel = k_gather<inv(), cv(), ce(), nw(), ln(), uni(), kb()>;
-    const size_t smem = gather_layout(p, nw() ? 4 : 8, sizeof(typename Val<cv()>::type), uni()).total;
-    // whole waves of resident CTAs, grid-stride over the tiles
-    const int grid = one_wave(kernel, (tiles + kThreads / 32 - 1) / (kThreads / 32), smem);
-    kernel<<<grid, kThreads, smem, stream>>>(p);
-    check_launch("k_gather");
-  }); }); }); }); }); }); });
+    // sign masks come from fermionic bases, which have no spin inversion: those instances are not built
+    if constexpr (inv() && sg()) throw std::runtime_error("k_gather: sign masks with spin inversion");
+    else {
+      auto kernel = k_gather<inv(), cv(), ce(), nw(), ln(), uni(), sg(), kb()>;
+      const size_t smem = gather_layout(p, nw() ? 4 : 8, sizeof(typename Val<cv()>::type), uni(), sg()).total;
+      // whole waves of resident CTAs, grid-stride over the tiles
+      const int grid = one_wave(kernel, (tiles + kThreads / 32 - 1) / (kThreads / 32), smem);
+      kernel<<<grid, kThreads, smem, stream>>>(p);
+      check_launch("k_gather");
+    }
+  }); }); }); }); }); }); }); });
 }
 
 }  // namespace dmv

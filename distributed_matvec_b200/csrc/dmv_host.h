@@ -217,9 +217,11 @@ void launch_locale_idx(int64_t count, const uint64_t *states, int num_ranks, uin
 void launch_compute_norms(const OrbitProgram &P, int64_t count, const uint64_t *reps, double *norms,
                           cudaStream_t stream);
 // enumeration: chunk c covers candidates [chunk_first[c], chunk_first[c] + chunk_len[c]) in the
-// combinadic (fixed Hamming weight) or plain integer order; pass 0 counts, pass 1 writes.
+// combinadic (fixed Hamming weight) or plain integer order; pass 0 counts, pass 1 writes.  half_mask != 0 keeps only
+// the candidates with half_weight bits of half_mask set (the up half of a spinful-fermion basis).
 void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask, bool fixed_hamming,
-                      int rank, int num_ranks, int64_t n_chunks, const uint64_t *chunk_first,
+                      uint64_t half_mask, int half_weight, int rank, int num_ranks, int64_t n_chunks,
+                      const uint64_t *chunk_first,
                       const uint64_t *chunk_last, unsigned long long *chunk_count,
                       const unsigned long long *chunk_offset, uint64_t *out, double *out_norms,
                       bool write_pass, cudaStream_t stream);

@@ -1930,9 +1930,11 @@ __device__ __forceinline__ uint64_t next_state_fixed_hamming(uint64_t v) {
 // One thread per chunk of consecutive candidates [first, last]; keeps a candidate iff it is owned by
 // this rank, is the minimum of its orbit and has non-zero norm (reference
 // src/StatesEnumeration.chpl:158-224).  Pass 0 counts, pass 1 writes at chunk_offset[c].
+// half_mask != 0 (spinful fermions): only candidates with popcount(v & half_mask) == half_weight are kept.
 template <int PROJ, bool WRITE>
-__global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed_hamming, int rank,
-                            int num_ranks, int64_t n_chunks, const uint64_t *__restrict__ chunk_first,
+__global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed_hamming, uint64_t half_mask,
+                            int half_weight, int rank, int num_ranks, int64_t n_chunks,
+                            const uint64_t *__restrict__ chunk_first,
                             const uint64_t *__restrict__ chunk_last, unsigned long long *chunk_count,
                             const unsigned long long *__restrict__ chunk_offset, uint64_t *out,
                             double *out_norms) {
@@ -1943,7 +1945,8 @@ __global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed
   unsigned long long n = 0;
   unsigned long long base = WRITE ? chunk_offset[c] : 0ull;
   for (;;) {
-    bool keep = (num_ranks <= 1) || (locale_idx_of(v, num_ranks) == rank);
+    bool keep = (half_mask == 0 || __popcll(v & half_mask) == half_weight) &&
+                ((num_ranks <= 1) || (locale_idx_of(v, num_ranks) == rank));
     double norm = 1.0;
     if (keep) {
       if (PROJ == PROJ_INVERSION) {
@@ -2276,7 +2279,8 @@ void launch_compute_norms(const OrbitProgram &P, int64_t count, const uint64_t *
 }
 
 void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask, bool fixed_hamming,
-                      int rank, int num_ranks, int64_t n_chunks, const uint64_t *chunk_first,
+                      uint64_t half_mask, int half_weight, int rank, int num_ranks, int64_t n_chunks,
+                      const uint64_t *chunk_first,
                       const uint64_t *chunk_last, unsigned long long *chunk_count,
                       const unsigned long long *chunk_offset, uint64_t *out, double *out_norms,
                       bool write_pass, cudaStream_t stream) {
@@ -2284,7 +2288,8 @@ void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask
   const unsigned blocks = (unsigned)((n_chunks + 127) / 128);
   with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
     with_bool(write_pass, [&](auto write) {
-      k_enumerate<pj(), write()><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, rank, num_ranks, n_chunks,
+      k_enumerate<pj(), write()><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, half_mask, half_weight, rank,
+                                                             num_ranks, n_chunks,
                                                              chunk_first, chunk_last, chunk_count, chunk_offset, out,
                                                              out_norms);
     });

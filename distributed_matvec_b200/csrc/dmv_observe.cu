@@ -1016,6 +1016,7 @@ int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
 // host.  On several ranks the targets are looked up in the whole basis of the replicated-x form, against the gathered x.
 int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm) {
   API_BEGIN
+  require_spin(ctx, "dmv_pm_correlations");
   SolverRun run(ctx, elt, "dmv_pm_correlations", false);
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
@@ -1107,6 +1108,8 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
                    const void *x, void *y) {
   API_BEGIN
   if (!target || !source) throw std::runtime_error("target and source must not be null");
+  require_spin(source, "dmv_apply_spin");
+  require_spin(target, "dmv_apply_spin");
   SolverRun run(source, elt, "dmv_apply_spin", false);
   require_states(target);
   if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
@@ -1193,6 +1196,7 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
 int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, int n_a,
                                const int32_t *sites_a, double *rho) {
   API_BEGIN
+  require_spin(ctx, "dmv_reduced_density_matrix");
   SolverRun run(ctx, elt, "dmv_reduced_density_matrix", true);
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");

@@ -15,6 +15,17 @@ Conventions (ours; irrelevant for every Heisenberg input, see DESIGN.md):
   * site i is bit i of the uint64 basis state (LSB = site 0);
   * bit = 1 means spin up (sigma^z = +1), sigma^+ turns a 0 bit into a 1 bit;
   * a ``matrix:`` term on sites (i, j) is indexed by (bit_i << 1) | bit_j.
+
+Fermion operators (on a fermionic basis only, never mixed with σ / S in one expression):
+  * ``c†₀`` creation, ``c₀`` annihilation, ``n₀`` number on placeholder site 0 (ASCII digits work too);
+  * on a spinful basis each operator carries a spin arrow, before or after the index: ``c†₀↑ c₁↑``, ``n↑₀ n↓₀``;
+  * they combine with the coefficient, ``×`` / ``*``, ``+`` and ``−`` grammar of the spin operators, e.g.
+    ``-1.0 × c†₀↑ c₁↑ - 1.0 × c†₁↑ c₀↑`` or ``4 × n₀↑ n₀↓``.
+The mode of a factor is its concrete site i (spinless; spinful up) or N + i (spinful down), and bit k of a state is the
+occupation of mode k.  Modes are ordered by bit: c_k = Z_0 ... Z_{k-1} σ⁻_k (Jordan-Wigner).  Every monomial is compiled
+per concrete instance: with T the set of modes it touches, its 2^|T| local matrix carries the signs of the modes inside
+T, and the string of the modes outside T becomes the term's sign mask s = XOR over its c / c† factors on mode k of
+(bits below k) & ~T.  A hop and its conjugate get the same x and s.
 """
 from __future__ import annotations
 
@@ -41,9 +52,26 @@ _SIGMA = {
 }
 
 
+_FERMION_KINDS = ("c+", "c", "n")
+_ARROWS = {"↑": "up", "↓": "down"}
+
+
+@dataclass(frozen=True)
+class FermionModes:
+    """Bit layout of a fermionic basis: mode of (site, spin) = site, or site + number_sites for spin down."""
+    number_sites: int
+    spinful: bool
+
+    def mode(self, site: int, spin: str) -> int:
+        if self.spinful != (spin != ""):
+            raise ValueError("fermion operators need a spin arrow (↑ or ↓) on a spinful basis and none on a spinless one")
+        return site + (self.number_sites if spin == "down" else 0)
+
+
 @dataclass(frozen=True)
 class Factor:
-    """One primitive operator: kind in {'sigma','S'}, comp in x,y,z,+,-, placeholder site index."""
+    """One primitive operator: kind in {'sigma','S'}, comp in x,y,z,+,-, placeholder site index; or a fermion
+    operator: kind in {'c+','c','n'}, comp the spin ('up', 'down' or '' on a spinless basis)."""
     kind: str
     comp: str
     site: int
@@ -102,6 +130,24 @@ def _tokenize(text: str):
         elif ch == "I":
             yield ("num", 1.0 + 0j)
             i += 1
+        elif ch in "cn":
+            kind = "n" if ch == "n" else "c"
+            i += 1
+            if kind == "c" and text[i:i + 1] == "†":
+                kind = "c+"
+                i += 1
+            spin, digits = "", ""
+            while i < n and (text[i] in _SUBSCRIPT_DIGITS or text[i].isdigit() or text[i] in _ARROWS):
+                if text[i] in _ARROWS:
+                    if spin:
+                        raise ValueError(f"two spin arrows on one operator in {text!r}")
+                    spin = _ARROWS[text[i]]
+                else:
+                    digits += _SUBSCRIPT_DIGITS.get(text[i], text[i])
+                i += 1
+            if not digits:
+                raise ValueError(f"missing site index in {text!r}")
+            yield ("op", Factor(kind, spin, int(digits)))
         else:
             raise ValueError(f"unexpected character {ch!r} in expression {text!r}")
 
@@ -135,7 +181,14 @@ def parse_expression(text: str) -> list[Product]:
         products.append(cur)
     if not products:
         raise ValueError(f"empty expression {text!r}")
+    kinds = {f.kind in _FERMION_KINDS for p in products for f in p.factors}
+    if len(kinds) > 1:
+        raise ValueError(f"spin (σ, S) and fermion (c†, c, n) operators are mixed in {text!r}")
     return products
+
+
+def is_fermionic(products: list[Product]) -> bool:
+    return any(f.kind in _FERMION_KINDS for p in products for f in p.factors)
 
 
 def local_matrix(products: list[Product]) -> tuple[int, np.ndarray]:
@@ -179,11 +232,15 @@ class TermTable:
         return bool(np.all(self.v.imag == 0))
 
 
-def _accumulate_instance(acc: dict, k: int, mat: np.ndarray, sites: tuple[int, ...]):
+def _check_sites(k: int, sites: tuple[int, ...]):
     if len(set(sites)) != len(sites):
         raise ValueError(f"repeated site in {sites}")
     if len(sites) != k:
         raise ValueError(f"expression acts on {k} sites but got index tuple {sites}")
+
+
+def _accumulate_instance(acc: dict, k: int, mat: np.ndarray, sites: tuple[int, ...]):
+    _check_sites(k, sites)
     mask = 0
     for st in sites:
         mask |= 1 << st
@@ -201,24 +258,92 @@ def _accumulate_instance(acc: dict, k: int, mat: np.ndarray, sites: tuple[int, .
             continue
         r = spread(in_idx)
         x = r ^ spread(out_idx)
-        key = (mask, r, x)
+        key = (mask, r, x, 0)
         acc[key] = acc.get(key, 0j) + complex(val)
 
 
-def compile_terms(term_specs: list[dict], number_sites: int) -> tuple[TermTable, TermTable]:
+def fermion_monomial_terms(coeff: complex, ops: list[tuple[str, int]]):
+    """Terms (v, m, r, x, s) of coeff * op_1 op_2 ... op_n on concrete modes, ops = [(kind, mode)] with kind in
+    'c+', 'c', 'n' (the rightmost acts first).  m is the set T of touched modes, the local matrix carries the signs of
+    the modes inside T, and s = XOR over the c / c† factors on mode k of (bits below k) & ~T."""
+    T = sorted({mode for _, mode in ops})
+    m = 0
+    for mode in T:
+        m |= 1 << mode
+    s = 0
+    for kind, mode in ops:
+        if kind != "n":
+            s ^= ((1 << mode) - 1) & ~m
+    pos = {mode: b for b, mode in enumerate(T)}
+
+    def spread(local: int) -> int:
+        return sum(1 << T[b] for b in range(len(T)) if (local >> b) & 1)
+
+    out = []
+    for local_in in range(1 << len(T)):
+        st, amp = local_in, complex(coeff)
+        for kind, mode in reversed(ops):
+            b = pos[mode]
+            occ = (st >> b) & 1
+            if kind == "n":
+                if not occ:
+                    amp = 0j
+                    break
+                continue
+            if occ != (kind == "c"):   # c needs the mode occupied, c† needs it empty
+                amp = 0j
+                break
+            if bin(st & ((1 << b) - 1)).count("1") & 1:
+                amp = -amp
+            st ^= 1 << b
+        if amp != 0:
+            r = spread(local_in)
+            out.append((amp, m, r, r ^ spread(st), s))
+    return out
+
+
+def _accumulate_fermion_instance(acc: dict, products: list[Product], k: int, sites: tuple[int, ...],
+                                 modes: FermionModes):
+    _check_sites(k, sites)
+    for p in products:
+        ops = [(f.kind, modes.mode(sites[f.site], f.comp)) for f in p.factors]
+        if not ops:
+            raise ValueError("a constant term needs at least one operator on a fermionic basis")
+        for v, m, r, x, s in fermion_monomial_terms(p.coeff, ops):
+            key = (m, r, x, s)
+            acc[key] = acc.get(key, 0j) + v
+
+
+def compile_terms(term_specs: list[dict], number_sites: int,
+                  fermions: FermionModes | None = None) -> tuple[TermTable, TermTable]:
     """Compile the ``hamiltonian.terms`` list of a YAML config into (off_diag, diag) tables.
 
     Each spec has ``sites`` (list of index tuples) and either ``expression`` (string) or
     ``matrix`` (2^k x 2^k nested list, data/old/*.yaml form).
-    Equal (m, r, x) contributions from different expressions are summed and exact zeros
+    Equal (m, r, x, s) contributions from different expressions are summed and exact zeros
     dropped (sigma^x sigma^x + sigma^y sigma^y cancels on parallel spins), which is the
-    operator-compile-time merge SURVEY.md App. A.4(2) refers to.
+    operator-compile-time merge SURVEY.md App. A.4(2) refers to.  ``fermions``: the mode layout of a fermionic
+    basis, whose expressions are compiled instance by instance (module docstring); spin terms have s = 0.
     """
-    acc: dict[tuple[int, int, int], complex] = {}
+    acc: dict[tuple[int, int, int, int], complex] = {}
     for spec in term_specs:
         if "expression" in spec:
-            k, mat = local_matrix(parse_expression(spec["expression"]))
+            products = parse_expression(spec["expression"])
+            if is_fermionic(products) != (fermions is not None):
+                raise ValueError(f"{spec['expression']!r}: fermion operators (c†, c, n) need a fermionic basis, and "
+                                 "a fermionic basis takes fermion operators only")
+            k = 1 + max((f.site for p in products for f in p.factors), default=0)
+            if fermions is not None:
+                for sites in spec["sites"]:
+                    sites = tuple(int(s) for s in sites)
+                    if any(s < 0 or s >= number_sites for s in sites):
+                        raise ValueError(f"site index out of range in {sites}")
+                    _accumulate_fermion_instance(acc, products, k, sites, fermions)
+                continue
+            k, mat = local_matrix(products)
         elif "matrix" in spec:
+            if fermions is not None:
+                raise ValueError("matrix terms are not supported on a fermionic basis: use c†, c and n expressions")
             mat = np.array(spec["matrix"], dtype=np.complex128)
             k = int(mat.shape[0]).bit_length() - 1
             if mat.shape != (1 << k, 1 << k):
@@ -232,13 +357,14 @@ def compile_terms(term_specs: list[dict], number_sites: int) -> tuple[TermTable,
             _accumulate_instance(acc, k, mat, sites)
 
     off, diag_groups = [], {}
-    for (m, r, x), v in sorted(acc.items()):
+    for (m, r, x, s), v in sorted(acc.items()):
         if abs(v) == 0:
             continue
         if x == 0:
+            assert s == 0, "a diagonal monomial has an even number of c / c† factors on every mode, so no string"
             diag_groups.setdefault(m, {})[r] = v
         else:
-            off.append((v, m, r, x, 0))
+            off.append((v, m, r, x, s))
 
     # Diagonal part: Walsh-expand each function f(r) over the bits of m so that e.g.
     # the four (m, r) entries of sigma^z sigma^z collapse into ONE term (v, m=0, r=0, s=m).

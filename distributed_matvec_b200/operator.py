@@ -18,7 +18,7 @@ import ctypes as C
 import numpy as np
 
 from . import _native as nat
-from .config import BasisSpec, OperatorSpec
+from .config import SPINFUL_FERMION, SPINLESS_FERMION, BasisSpec, OperatorSpec
 
 
 def _is_torch(a) -> bool:
@@ -68,6 +68,12 @@ class Basis:
     def numberSites(self): return self.spec.number_sites
     @property
     def spinInversion(self): return self.spec.spin_inversion
+    # particle type (src/ForeignTypes.chpl:79-98)
+    def isSpinBasis(self): return not self.spec.is_fermionic()
+    def isSpinfulFermionicBasis(self): return self.spec.particle_type == SPINFUL_FERMION
+    def isSpinlessFermionicBasis(self): return self.spec.particle_type == SPINLESS_FERMION
+    def numberParticles(self): return self.spec.number_particles
+    def numberUp(self): return self.spec.number_up
 
     def build(self):
         """``Basis.build()`` (FT:72): enumerate this rank's representatives on the GPU."""
@@ -134,7 +140,7 @@ class Operator:
         b = spec.basis
         self._keep = []
         bd = nat.BasisDesc()
-        bd.number_sites = b.number_sites
+        bd.number_sites = b.number_bits
         bd.hamming_weight = -1 if b.hamming_weight is None else b.hamming_weight
         bd.spin_inversion = b.spin_inversion
         bd.has_permutations = int(b.has_permutation_symmetries())
@@ -156,8 +162,14 @@ class Operator:
         od.off_v, od.off_m, od.off_r, od.off_x, od.off_s = (a.ctypes.data for a in arrs[:5])
         od.n_diag = len(diag)
         od.diag_v, od.diag_m, od.diag_r, od.diag_s = (a.ctypes.data for a in arrs[5:])
+        pd = nat.ParticlesDesc()
+        pd.particle_type = {SPINLESS_FERMION: nat.DMV_SPINLESS_FERMION,
+                            SPINFUL_FERMION: nat.DMV_SPINFUL_FERMION}.get(b.particle_type, nat.DMV_SPIN)
+        pd.number_particles = -1 if b.number_particles is None else b.number_particles
+        pd.number_up = -1 if b.number_up is None else b.number_up
         handle = C.c_void_p()
-        nat.check(nat.lib().dmv_context_create(C.byref(bd), C.byref(od), device, rank, num_ranks, C.byref(handle)))
+        nat.check(nat.lib().dmv_context_create_particles(C.byref(bd), C.byref(pd), C.byref(od), device, rank, num_ranks,
+                                                         C.byref(handle)))
         self._ctx = handle
         self.basis = Basis(b, self)
 
@@ -365,9 +377,10 @@ class Operator:
         """Spin-spin correlations C[i, j] = <x|σᶻᵢσᶻⱼ|x> / <x|x> and magnetisation m[i] = <x|σᶻᵢ> / <x|x> on the device
         (dmv_zz_correlations), with σᶻ = +1 on a set bit.  x: shape (n,) or (k, n), float64 or complex128, a numpy
         array or a torch CUDA tensor (used in place on torch's current stream).  Collective when num_ranks > 1.
-        -> numpy (C, m) of shapes (N, N), (N,), or (k, N, N), (k, N) for a batch."""
+        On a fermionic basis i, j run over the bits (modes) and σᶻᵢ = 2nᵢ - 1.
+        -> numpy (C, m) of shapes (N, N), (N,), or (k, N, N), (k, N) for a batch, N the number of bits."""
         elt = _elt_of(x)
-        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        n, N = self.basis.numberStates(), self.spec.basis.number_bits
         if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
             raise ValueError(f"x must have shape ({n},) or (k, {n})")
         k = 1 if x.ndim == 1 else int(x.shape[0])
@@ -383,7 +396,7 @@ class Operator:
         """Flip-flop correlations T[i, j] = <x|σ⁺ᵢσ⁻ⱼ|x> / <x|x> on the device (dmv_pm_correlations), with σ⁺ turning a
         0 bit into a 1 bit.  x as for zz_correlations.  -> numpy complex128 of shape (N, N), or (k, N, N) for a batch."""
         elt = _elt_of(x)
-        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        n, N = self.basis.numberStates(), self.spec.basis.number_bits
         if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
             raise ValueError(f"x must have shape ({n},) or (k, {n})")
         k = 1 if x.ndim == 1 else int(x.shape[0])
@@ -418,7 +431,7 @@ class Operator:
         if kind not in self._SPIN_KINDS:
             raise ValueError(f"kind must be one of {sorted(self._SPIN_KINDS)}, got {kind!r}")
         elt = _elt_of(x)
-        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        n, N = self.basis.numberStates(), self.spec.basis.number_bits
         if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
             raise ValueError(f"x must have shape ({n},) or (k, {n})")
         w = np.ascontiguousarray(np.asarray(weights, dtype=np.complex128).reshape(-1))
@@ -449,7 +462,7 @@ class Operator:
         entanglement.block_layout), or a list of such dicts for a batch."""
         from .entanglement import block_layout
         elt = _elt_of(x)
-        n, N = self.basis.numberStates(), self.spec.basis.number_sites
+        n, N = self.basis.numberStates(), self.spec.basis.number_bits
         if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
             raise ValueError(f"x must have shape ({n},) or (k, {n})")
         sites_a = np.ascontiguousarray(np.asarray(sites, dtype=np.int32).reshape(-1))
@@ -478,7 +491,7 @@ class Operator:
         computed instead: for a pure state ρ_A and ρ_B have the same non-zero spectrum, so S(A) = S(B).  -> float, or
         an ndarray for a batch."""
         from .entanglement import entanglement_spectrum, renyi_entropy
-        N = self.spec.basis.number_sites
+        N = self.spec.basis.number_bits
         sites = [int(s) for s in np.asarray(sites).reshape(-1)]
         rest = [s for s in range(N) if s not in set(sites)]
         if 0 < len(rest) < len(sites):

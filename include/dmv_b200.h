@@ -67,6 +67,28 @@ int64_t dmv_launch_count(void);
  * partition  owner(s) = hash64_01(s) % num_ranks  (reference src/StatesEnumeration.chpl:122-136). */
 int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op, int device, int rank,
                        int num_ranks, dmv_context **out);
+
+/* ---- fermionic bases (the particle type of `ls_hs_basis`, reference src/FFI.chpl:85-99).  A state is a word of
+ * basis->number_sites BITS, one per fermionic mode, and a term's sign mask s carries the Jordan-Wigner string:
+ *   DMV_SPIN               spin-1/2; dmv_context_create is this case (number_particles, number_up unused)
+ *   DMV_SPINLESS_FERMION   bit i = occupation of site i; number_particles = -1 (free) or the particle number
+ *   DMV_SPINFUL_FERMION    N = number_sites / 2 sites: bit i = up occupation of site i, bit N + i = down occupation, so a
+ *                          state is (down << N) | up; number_particles and number_up are both fixed, and the basis is
+ *                          every state with number_up up and number_particles - number_up down particles
+ * For fermions basis->hamming_weight must equal number_particles (the weight over all bits).  Refused before anything
+ * is allocated: permutations or spin inversion with fermions; an odd bit count for spinful fermions; number_up outside
+ * 0..N or number_particles - number_up outside 0..N; a spinless number_particles outside -1..number_sites.
+ * On a fermionic context dmv_pm_correlations, dmv_apply_spin and dmv_reduced_density_matrix refuse (they assume spin
+ * operators without strings); dmv_zz_correlations gives <(2n_a - 1)(2n_b - 1)> over the bits.
+ * Info "particle_type" answers the constant below. */
+enum { DMV_SPIN = 0, DMV_SPINLESS_FERMION = 1, DMV_SPINFUL_FERMION = 2 };
+typedef struct {
+  int32_t particle_type;
+  int32_t number_particles;
+  int32_t number_up;
+} dmv_particles_desc;
+int dmv_context_create_particles(const dmv_basis_desc *basis, const dmv_particles_desc *particles,
+                                 const dmv_operator_desc *op, int device, int rank, int num_ranks, dmv_context **out);
 int dmv_context_destroy(dmv_context *ctx);
 /* launch on `cuda_stream` (a cudaStream_t; NULL is the legacy default stream), or on the context's own
  * non-blocking stream when use_own_stream != 0 (the initial state) */
@@ -120,7 +142,8 @@ int dmv_synchronize(dmv_context *ctx);
  *                        to the scatter product and its counting pass (dmv_plan); a change re-plans.  The overlapped
  *                        rounds of the record exchange always run S = 1
  *          "index"    = -1 auto (identity / Lin tables / directory) | 0 directory + binary search | 2 combinadic rank
- *                        | 3 Lin tables (full fixed-Hamming bases)
+ *                        | 3 Lin tables (full fixed-Hamming bases).  On a spinful-fermion basis (one rank, N <= 20) auto
+ *                        and 3 take the Lin tables split at bit N (index_mode 4), 2 the directory
  *          "bitparallel" = 1 | 0 walk the flip-mask groups one by one
  *          "canon"    = -1 auto (orbit minima through canonical forms: full space group of a torus, rotations x mirror x
  *                        flip of a chain) | 1 the round-1 forms (block rotations + coset chain; four run searches)
@@ -135,7 +158,9 @@ int dmv_synchronize(dmv_context *ctx);
  *               "global_states", "complex_coefficients", "quadrature_group", "rows_tk" (side of the square-torus orbit minimum k_rows is
  *               compiled for with the current options: 4 | 6, 0 the generic walk), "gather_split" (lanes per row the next
  *               single-rank k_gather launch uses), "push_split" (lanes per source state the next k_generate launch and
- *               its plan use), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
+ *               its plan use), "index_mode" (0 directory, 1 identity, 2 combinadic rank, 3 Lin tables, 4 Lin tables
+ *               split at bit N of a spinful-fermion basis), "particle_type", "gather_signs" (1: the operator's row
+ *               tables carry sign masks and k_gather applies them), ... (-1: unknown); "global.<key>" answers <key> for the whole-basis
  *               context of the replicated-x product (-1 while there is none) */
 int dmv_set_option(dmv_context *ctx, const char *name, int64_t value);
 int64_t dmv_get_info(const dmv_context *ctx, const char *name);

@@ -9,6 +9,11 @@ content and re-emits it in a normalised layout (no anchors, no comments, no solv
 re-checks semantic equality against the stored copies.
 
 Usage:  python tools/gen_models.py REFERENCE_DATA_DIR [data]
+        python tools/gen_models.py --fermions [data]
+
+--fermions writes the fermionic models, which the reference's data directory does not have: hubbard_chain_8 (periodic
+chain of 8 sites) and hubbard_square_4x4 (4 x 4 torus), H = -t sum_<ij>,s (c+_is c_js + h.c.) + U sum_i n_i,up n_i,down
+with t = 1, U = 4 at half filling; and spinless_ring_28, H = -t sum_i (c+_i c_i+1 + h.c.) with t = 1 at 14 particles.
 """
 import glob
 import os
@@ -51,9 +56,56 @@ def normalise(conf: dict) -> dict:
     return {"basis": basis, "hamiltonian": {"name": conf["hamiltonian"].get("name", ""), "terms": terms}}
 
 
+def _bonds_ring(n):
+    return [[i, (i + 1) % n] for i in range(n)]
+
+
+def _bonds_torus(lx, ly):
+    out = []
+    for y in range(ly):
+        for x in range(lx):
+            i = x + lx * y
+            out += [[i, (x + 1) % lx + lx * y], [i, x + lx * ((y + 1) % ly)]]
+    return out
+
+
+def hubbard(n_sites, bonds, t=1.0, u=4.0, number_up=None, number_down=None, name="Hubbard model"):
+    up = n_sites // 2 if number_up is None else number_up
+    down = n_sites // 2 if number_down is None else number_down
+    hop = f"-{t} × c†₀↑ c₁↑ - {t} × c†₁↑ c₀↑ - {t} × c†₀↓ c₁↓ - {t} × c†₁↓ c₀↓"
+    return {"basis": {"particle": "spinful-fermion", "number_sites": n_sites, "number_particles": up + down,
+                      "number_up": up},
+            "hamiltonian": {"name": name, "terms": [
+                {"expression": hop, "sites": _Flow(_Flow(b) for b in bonds)},
+                {"expression": f"{u} × n₀↑ n₀↓", "sites": _Flow(_Flow([i]) for i in range(n_sites))}]}}
+
+
+def spinless_ring(n_sites, number_particles, t=1.0, name="spinless fermions on a ring"):
+    return {"basis": {"particle": "spinless-fermion", "number_sites": n_sites, "number_particles": number_particles},
+            "hamiltonian": {"name": name, "terms": [
+                {"expression": f"-{t} × c†₀ c₁ - {t} × c†₁ c₀", "sites": _Flow(_Flow(b) for b in _bonds_ring(n_sites))}]}}
+
+
+def fermion_models() -> dict:
+    return {"hubbard_chain_8": hubbard(8, _bonds_ring(8)),
+            "hubbard_square_4x4": hubbard(16, _bonds_torus(4, 4)),
+            "spinless_ring_28": spinless_ring(28, 14)}
+
+
+def write_fermion_models(dst):
+    for name, conf in fermion_models().items():
+        with open(os.path.join(dst, name + ".yaml"), "w", encoding="utf-8") as f:
+            f.write(f"# model input '{name}.yaml': written by tools/gen_models.py --fermions\n")
+            yaml.safe_dump(conf, f, allow_unicode=True, sort_keys=False, width=120)
+        print("wrote", name)
+
+
 def main():
     if len(sys.argv) < 2:
         raise SystemExit(__doc__)
+    if sys.argv[1] == "--fermions":
+        write_fermion_models(sys.argv[2] if len(sys.argv) > 2 else os.path.join(os.path.dirname(__file__), "..", "data"))
+        return
     src = sys.argv[1]
     dst = sys.argv[2] if len(sys.argv) > 2 else os.path.join(os.path.dirname(__file__), "..", "data")
     os.makedirs(dst, exist_ok=True)
