@@ -23,7 +23,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 WORLDS = (2, 3, 4)
 CASES = ("nccl", "oneshot", "rounds2", "rounds3", "rounds5", "rounds64", "repl_peer", "repl_nccl")
 AT_SIZE = "heisenberg_chain_24"            # 2.7 million states: at least 2^18 per rank
-PORTS = {2: 29611, 3: 29621, 4: 29631}     # (test_multi_gpu.py and the solver tests use 29511 .. 29599)
 # the exchange each case must report it ran
 RAN = {"nccl": "records/nccl", "oneshot": "records/peer-direct", "rounds2": "records/peer-direct in 2 rounds",
        "rounds3": "records/peer-direct in 3 rounds", "rounds5": "records/peer-direct in 5 rounds",
@@ -33,10 +32,10 @@ RAN = {"nccl": "records/nccl", "oneshot": "records/peer-direct", "rounds2": "rec
 _runs = {}
 
 
-def _run(world, args, key):
+def _run(world, args):
+    # --standalone: the launcher binds its rendezvous store to a free port, so no fixed port can be taken already
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
-           "--master-addr", "127.0.0.1", "--master-port", str(PORTS[world] + key),
-           os.path.join(ROOT, "tools", "exchange_check.py"), *args]
+           "--standalone", os.path.join(ROOT, "tools", "exchange_check.py"), *args]
     out = subprocess.run(cmd, cwd=ROOT, env=dict(os.environ), capture_output=True, text=True, timeout=1200)
     lines = [l.rstrip() for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     return out.returncode, lines, out.stdout[-4000:] + out.stderr[-3000:]
@@ -46,9 +45,9 @@ def _world(world):
     if world not in _runs:
         if not torch.cuda.is_available():
             pytest.fail("this test needs a CUDA device (no CPU fallback exists)")
-        runs = [_run(world, ["--cases", ",".join(CASES)], 0)]
+        runs = [_run(world, ["--cases", ",".join(CASES)])]
         if world <= 3:
-            runs.append(_run(world, ["--cases", "rounds_auto,nccl", "--parts", "mixed", AT_SIZE], 1))
+            runs.append(_run(world, ["--cases", "rounds_auto,nccl", "--parts", "mixed", AT_SIZE]))
         _runs[world] = runs
     return _runs[world]
 

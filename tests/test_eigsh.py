@@ -363,8 +363,8 @@ def test_errors(need_cuda):
 @pytest.mark.gpu
 def test_collective_eigsh_two_ranks(need_cuda):
     """Two ranks: chain_10, square_4x4, momentum_sector and chain_24 against one rank (tools/eigsh_check.py)."""
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", "29553", os.path.join(ROOT, "tools", "eigsh_check.py")]
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--standalone",
+           os.path.join(ROOT, "tools", "eigsh_check.py")]
     out = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=1500)
     lines = [l for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     assert out.returncode == 0 and len(lines) >= 4 and not any(l.rstrip().endswith("FAIL") for l in lines), \

@@ -489,8 +489,8 @@ def test_errors_write_nothing(need_cuda):
 @pytest.mark.gpu
 def test_two_ranks_against_one(need_cuda):
     """Two ranks on one device against one rank (tools/entanglement_check.py)."""
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", "29563", os.path.join(ROOT, "tools", "entanglement_check.py")]
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--standalone",
+           os.path.join(ROOT, "tools", "entanglement_check.py")]
     out = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=900)
     lines = [l for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     assert out.returncode == 0 and len(lines) >= 4 and not any(l.rstrip().endswith("FAIL") for l in lines), \

@@ -347,8 +347,8 @@ def test_errors(need_cuda):
 def test_collective_expm_two_ranks(need_cuda):
     """Two ranks (on two GPUs, or both on one): chain_10, square_4x4, chain_24_symm, momentum_sector and chain_24, the
     hashed y back in block order against the one-rank result to 1e-10 (tools/expm_check.py)."""
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", "29547", os.path.join(ROOT, "tools", "expm_check.py")]
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--standalone",
+           os.path.join(ROOT, "tools", "expm_check.py")]
     out = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=1500)
     lines = [l for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     assert out.returncode == 0 and len(lines) >= 13 and not any(l.rstrip().endswith("FAIL") for l in lines), \

@@ -19,10 +19,10 @@ SMALL = ["heisenberg_chain_10", "heisenberg_chain_16", "heisenberg_square_4x4", 
 AT_SIZE = ["heisenberg_chain_24", "heisenberg_chain_32_symm", "heisenberg_square_6x6"]   # >= 10^6 states per rank
 
 
-def _run(world, env, names, port):
+def _run(world, env, names):
+    # --standalone: the launcher binds its rendezvous store to a free port, so no fixed port can be taken already
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
-           "--master-addr", "127.0.0.1", "--master-port", str(port), os.path.join(ROOT, "tools", "multi_gpu_check.py"),
-           *names]
+           "--standalone", os.path.join(ROOT, "tools", "multi_gpu_check.py"), *names]
     out = subprocess.run(cmd, cwd=ROOT, env={**os.environ, **env}, capture_output=True, text=True, timeout=1500)
     lines = [l for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     assert out.returncode == 0 and lines and not any(l.rstrip().endswith("FAIL") for l in lines), \
@@ -38,7 +38,7 @@ def test_collective_product_two_gpus(exchange, peer_gather):
     if not torch.cuda.is_available():
         pytest.fail("this test needs a CUDA device (no CPU fallback exists)")
     names = SMALL + (AT_SIZE if exchange in ("-1", "1") else AT_SIZE[:1])
-    lines = _run(2, {"DMV_EXCHANGE": exchange, "DMV_PEER_GATHER": peer_gather}, names, 29531 + int(exchange) + 2)
+    lines = _run(2, {"DMV_EXCHANGE": exchange, "DMV_PEER_GATHER": peer_gather}, names)
     text = "\n".join(lines)
     if exchange == "-1":
         assert "replicated-x/peer-direct gather" in text

@@ -811,8 +811,8 @@ def test_errors_change_nothing(need_cuda):
 @pytest.mark.gpu
 def test_collective_apply_spin_two_ranks(need_cuda):
     """Two ranks against one rank (tools/spin_check.py)."""
-    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr",
-           "127.0.0.1", "--master-port", "29561", os.path.join(ROOT, "tools", "spin_check.py")]
+    cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--standalone",
+           os.path.join(ROOT, "tools", "spin_check.py")]
     out = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=900)
     lines = [l for l in out.stdout.splitlines() if l.rstrip().endswith(("OK", "FAIL"))]
     assert out.returncode == 0 and len(lines) >= 6 and not any(l.rstrip().endswith("FAIL") for l in lines), \
