@@ -1433,10 +1433,10 @@ __device__ __forceinline__ uint32_t load_u8_hint(const uint8_t *q, uint64_t poli
   asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u8 %0, [%1], %2;" : "=r"(v) : "l"(q), "l"(policy));
   return v;
 }
-// an entry: through L1 (a lane's next entries and its neighbours' share the line), evict_first in L2
+// an entry: the warp reads whole lines of a run (read once: not allocated in L1, evict_first in L2)
 __device__ __forceinline__ uint32_t load_entry(const uint32_t *q, uint64_t policy) {
   uint32_t v;
-  asm volatile("ld.global.nc.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(q), "l"(policy));
+  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(q), "l"(policy));
   return v;
 }
 // a gather from the current block of the compact x (an L2 hit): not allocated in L1
@@ -1451,20 +1451,36 @@ __device__ __forceinline__ double2 gather_x(const double2 *q) {
   return v;
 }
 
-// One lane per row, as k_rows.  A row's sum runs over blocks k0 .. k1 - 1 and within each block in k_rows' term order,
-// with k_rows' coefficients and (n x) products: over the whole basis at once (one block) y equals k_rows' bit for bit.
-// The entries, counts, row data and partial sums are read once per product (evict_first); four gathers per lane are in
-// flight at a time, nothing depends on a gather but its own multiply-add.
+// Entries of a tile's run that its warp gathers at once (kStoreWindow / 32 per lane), and the shared memory of their
+// values and codes: one window per warp.
+constexpr int kStoreWindow = 128;
+template <bool CE>
+constexpr size_t rows_stored_smem() {
+  return (size_t)kWarps * kStoreWindow * (sizeof(typename ValT<CE>::type) + 1);
+}
+
+// One warp per tile of 32 rows, one lane per row for the sums, as k_rows.  In every block the tile's entries are one run
+// in lane order (k_store_build).  The warp reads the run of its valid lanes in windows of kStoreWindow entries: lane l
+// loads the entries at positions l, l + 32, ... of the window (one line per warp instruction), issues their gathers back
+// to back and puts each value and code at its position in the warp's window, whichever row it belongs to.  Then each
+// lane sums the part of its own row's range that lies in the window, in order.  So a row's sum runs over blocks
+// k0 .. k1 - 1 and within each block in k_rows' term order, with k_rows' coefficients and (n x) products: over the whole
+// basis at once (one block) y equals k_rows' bit for bit.  The entries, counts, row data and partial sums are read once
+// per product (evict_first).
 template <bool CE>
 __global__ void __launch_bounds__(kThreads) k_rows_stored(const KernelParams p, const RowsStoreView s,
                                                           const typename ValT<CE>::type *__restrict__ xs,
                                                           typename ValT<CE>::type *partial, int k0, int k1) {
   using E = typename ValT<CE>::type;
+  constexpr int kPer = kStoreWindow / 32;
+  extern __shared__ __align__(16) unsigned char smem[];
   __shared__ double scoef[kStoreCodes];
   if (threadIdx.x < kStoreCodes) scoef[threadIdx.x] = s.coef[threadIdx.x];
   __syncthreads();
   const unsigned lane = threadIdx.x & 31u;
   const unsigned warp = threadIdx.x >> 5;
+  E *const sval = reinterpret_cast<E *>(smem) + warp * kStoreWindow;
+  uint8_t *const scode = smem + kWarps * kStoreWindow * sizeof(E) + warp * kStoreWindow;
   const bool first = k0 == 0, last = k1 == s.chunks;
   const uint64_t stream = l2_policy(L2_FIRST);
   const double *__restrict__ row_norms = p.row_norms ? p.row_norms : p.norms;
@@ -1475,33 +1491,45 @@ __global__ void __launch_bounds__(kThreads) k_rows_stored(const KernelParams p, 
   for (int64_t tile = t0 + (int64_t)blockIdx.x * kWarps + warp; tile < t1; tile += warps_total) {
     const int64_t i = tile * 32 + lane;
     const bool valid = i >= p.row_begin && i < p.row_end;
+    // the valid lanes are contiguous: lane_lo .. lane_hi
+    const int lane_lo = (int)max(p.row_begin - tile * 32, (int64_t)0);
+    const int lane_hi = (int)min(p.row_end - tile * 32, (int64_t)32) - 1;
     E acc = zero;
 #ifndef DMV_STORE_NO_PARTIAL   // measurement builds only: the partial sums neither read nor written, wrong results
     if (!first && valid) acc = load_hint(partial + i, stream);
 #endif
     for (int k = k0; k < k1; ++k) {
       uint32_t cnt = i < s.n_rows ? load_u8_hint(s.counts + k * s.n_rows + i, stream) : 0u;
-      const uint64_t start = load64_hint(s.tile_off + k * s.n_tiles + tile, stream) + warp_exclusive_sum(cnt, lane);
+      const uint32_t excl = warp_exclusive_sum(cnt, lane);
       if (!valid) cnt = 0;
-      const uint32_t *e = s.entries + start;
+      // the run of the valid lanes, [run_lo, run_lo + run_n) from the tile's first entry in the block; this row's
+      // entries are [lo, lo + cnt) of it
+      const uint32_t run_lo = __shfl_sync(0xffffffffu, excl, lane_lo);
+      const uint32_t run_n = __shfl_sync(0xffffffffu, excl + cnt, lane_hi) - run_lo;
+      const uint32_t lo = valid ? excl - run_lo : 0u, hi = lo + cnt;
+      const uint32_t *e = s.entries + load64_hint(s.tile_off + k * s.n_tiles + tile, stream) + run_lo;
 #ifdef DMV_STORE_NO_GATHER   // measurement builds only: entries streamed, no gather, wrong results on purpose
       auto gather_x = [](const E *q) { return v_make((double)(((uintptr_t)q >> 4) & 7u), 0.0, (E *)nullptr); };
 #endif
       const E *xb = xs + (int64_t)k * s.block_states;
-      uint32_t j = 0;
-      for (; j + 4 <= cnt; j += 4) {
-        const uint32_t e0 = load_entry(e + j, stream), e1 = load_entry(e + j + 1, stream);
-        const uint32_t e2 = load_entry(e + j + 2, stream), e3 = load_entry(e + j + 3, stream);
-        const E v0 = gather_x(xb + (e0 & kMask)), v1 = gather_x(xb + (e1 & kMask));
-        const E v2 = gather_x(xb + (e2 & kMask)), v3 = gather_x(xb + (e3 & kMask));
-        axpy(acc, scoef[e0 >> kStoreIndexBits], v0);
-        axpy(acc, scoef[e1 >> kStoreIndexBits], v1);
-        axpy(acc, scoef[e2 >> kStoreIndexBits], v2);
-        axpy(acc, scoef[e3 >> kStoreIndexBits], v3);
-      }
-      for (; j < cnt; ++j) {
-        const uint32_t e0 = load_entry(e + j, stream);
-        axpy(acc, scoef[e0 >> kStoreIndexBits], gather_x(xb + (e0 & kMask)));
+      for (uint32_t w0 = 0; w0 < run_n; w0 += kStoreWindow) {
+        uint32_t ent[kPer];
+#pragma unroll
+        for (int q = 0; q < kPer; ++q)
+          ent[q] = w0 + lane + 32 * q < run_n ? load_entry(e + w0 + lane + 32 * q, stream) : 0u;
+        E v[kPer];
+#pragma unroll
+        for (int q = 0; q < kPer; ++q)
+          v[q] = w0 + lane + 32 * q < run_n ? gather_x(xb + (ent[q] & kMask)) : zero;
+#pragma unroll
+        for (int q = 0; q < kPer; ++q) {
+          sval[lane + 32 * q] = v[q];
+          scode[lane + 32 * q] = (uint8_t)(ent[q] >> kStoreIndexBits);
+        }
+        __syncwarp();
+        const uint32_t end = min(hi, w0 + kStoreWindow);
+        for (uint32_t j = max(lo, w0); j < end; ++j) axpy(acc, scoef[scode[j - w0]], sval[j - w0]);
+        __syncwarp();
       }
     }
     if (!valid) continue;
@@ -2089,9 +2117,10 @@ void launch_rows_stored(const KernelParams &p, const RowsStoreView &s, const voi
   with_bool(complex_elements, [&](auto ce) {
     using E = typename ValT<ce()>::type;
     auto kernel = k_rows_stored<ce()>;
-    const int resident = resident_ctas(kernel, 0);
-    kernel<<<capped_grid((tiles + kWarps - 1) / kWarps, (int64_t)sm_count() * std::max(resident, 1)), kThreads, 0,
-             stream>>>(p, s, reinterpret_cast<const E *>(xs), reinterpret_cast<E *>(partial), k0, k1);
+    constexpr size_t smem = rows_stored_smem<ce()>();
+    const int grid = one_wave(kernel, (tiles + kWarps - 1) / kWarps, smem);
+    kernel<<<grid, kThreads, smem, stream>>>(p, s, reinterpret_cast<const E *>(xs), reinterpret_cast<E *>(partial), k0,
+                                             k1);
     check_launch("k_rows_stored");
   });
 }

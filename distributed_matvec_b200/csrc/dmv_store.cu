@@ -21,17 +21,18 @@ namespace dmv { namespace host {
 namespace {
 
 // Rates of the cost model: the least-squares fit (in log time) to the sweep of one H100 SXM at 700 W
-// (profiles/h100_rows_store_sweep.log: 6x6 square, chain_32_symm, chain_36_symm, complex128 and float64, C = 1 .. 64).
-// They are effective rates, not hardware ones, and one set cannot fit every workload: the gathers of the chains have
-// more locality than the torus' (chain_36_symm at C = 1, all misses: 76 G/s; the 6x6 square: 34 G/s, the rate of random
-// HBM sectors), so the model is off by up to 41 % on the 6x6 square at C = 1 and 51 % on chain_36_symm in float64.
-// Near each workload's best C it is within 20 %, and its choice is within 10 % of the best C measured.
+// (profiles/h100_rows_store_window_sweep.log: 6x6 square, chain_32_symm, chain_36_symm, complex128 and float64,
+// C = 1 .. 64, one block per pass).  They are effective rates, not hardware ones, and one set cannot fit every
+// workload: the model puts the 6x6 square up to 32 % too fast (C = 1) and the chains' float64 products up to 27 % too
+// slow.  Near each workload's best C it is within 20 %.  It chooses C = 9 on the 6x6 square (best measured: C = 8,
+// C = 12 is 2 % slower), 3 on chain_32_symm (about 5 % slower than C = 1) and 1 on chain_36_symm (the best in
+// complex128).
 constexpr double kRowsTermsPerS = 30.0e9;    // k_rows: measured 32.5 G terms/s on the 6x6 square, 25 on chain_32 and
                                              // 20 on chain_36 (there the model puts k_rows 37 % too fast)
-constexpr double kL2GatherPerS = 125.0e9;    // random gathers that hit L2
-constexpr double kMissGatherPerS = 60.0e9;   // gathers that miss L2, between the torus' 34 and the chains' 76 G/s
-constexpr double kStreamBytesPerS = 3.0e12;  // entries, counts, row data and partial sums
-constexpr double kL2Share = 0.25;            // share of L2 a pass's block of x keeps resident beside the streams
+constexpr double kL2GatherPerS = 167.0e9;    // random gathers that hit L2
+constexpr double kMissGatherPerS = 94.0e9;   // gathers that miss L2
+constexpr double kStreamBytesPerS = 2.5e12;  // entries, counts, row data and partial sums
+constexpr double kL2Share = 0.5;             // share of L2 a pass's block of x keeps resident beside the streams
 constexpr int64_t kStoreMinRows = 1 << 20;   // below this a product takes well under a millisecond: k_rows
 
 int64_t store_bytes(int64_t n_states, int64_t n_rows, int64_t terms, int chunks) {
