@@ -95,6 +95,9 @@ _SIGNATURES = [
     ("dmv_pm_correlations", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     ("dmv_apply_spin", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                  C.c_void_p]),
+    ("dmv_one_body_density_matrix", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    ("dmv_apply_fermion", C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                    C.c_void_p]),
     ("dmv_reduced_density_matrix", C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
                                              C.c_void_p]),
     ("dmv_rdm_layout", C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_int),

@@ -1100,6 +1100,12 @@ void require_spin(const dmv_context *ctx, const char *entry) {
                              " basis (it assumes spin operators without Jordan-Wigner strings)");
 }
 
+void require_fermion(const dmv_context *ctx, const char *entry) {
+  if (ctx && ctx->particle_type == DMV_SPIN)
+    throw std::runtime_error(std::string(entry) + ": not defined on a spin-1/2 basis (it applies fermionic operators "
+                             "with Jordan-Wigner strings)");
+}
+
 // the particle numbers of a fermionic basis, checked before anything is allocated
 void check_particles(const dmv_basis_desc *basis, const dmv_particles_desc *pt) {
   const int type = pt->particle_type, bits = basis->number_sites;

@@ -457,6 +457,8 @@ void select_index_mode(dmv_context *ctx);
 const char *particle_name(int particle_type);   // "spin-1/2", "spinless-fermion", "spinful-fermion"
 // the refusal of an observable that assumes spin operators without strings
 void require_spin(const dmv_context *ctx, const char *entry);
+// the refusal of an observable of fermionic operators on a spin basis
+void require_fermion(const dmv_context *ctx, const char *entry);
 inline bool lin_tables(int index_mode) { return index_mode == INDEX_LIN || index_mode == INDEX_LIN_SPLIT; }
 void install_directory(dmv_context *ctx);
 void upload_orbit(dmv_context *ctx);

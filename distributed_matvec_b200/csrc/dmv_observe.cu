@@ -289,7 +289,9 @@ __global__ void __launch_bounds__(256, 2) k_pm_rows(const PmArgs A) {
 // The CTA's warps share a tile of 32 rows, one per lane; warp w takes the unordered pairs w, w + warps, ..., every lane
 // adds its row's term and the warp sums them by shuffles in a fixed order, one sum per direction of the pair.  The
 // classes of an unordered pair belong to one warp only, so lane 0 owns their slots in shared memory.
-template <int LOOK, bool CE>
+// JW (fermionic bases, PM_NONE only): the term of c†ᵢcⱼ carries the Jordan-Wigner sign (-1)^popc(b & between(i, j)),
+// the bits strictly between the two modes; b and its target agree there, so both directions of a pair take one sign.
+template <int LOOK, bool CE, bool JW>
 __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
   extern __shared__ double s_cls[];   // [classes] real parts, then imaginary parts
   const int C = A.c_hi, N = A.n_sites, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
@@ -309,6 +311,10 @@ __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
       if (valid && bi != bj) {
         const double2 v = pm_target<LOOK, 0, CE>(A, b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
         c = make_double2(xb.x * v.x - xb.y * v.y, xb.x * v.y + xb.y * v.x);
+        if constexpr (JW) {   // pairs are stored with si < sj
+          const uint64_t between = ((1ull << sj) - 1) & ~((2ull << si) - 1);
+          if (__popcll(b & between) & 1) c = make_double2(-c.x, -c.y);
+        }
       }
       double s[4] = {bi ? c.x : 0.0, bi ? c.y : 0.0, bi ? 0.0 : c.x, bi ? 0.0 : c.y};   // (i, j), then (j, i)
 #pragma unroll
@@ -333,15 +339,19 @@ __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
 constexpr size_t kPmSmem = 96 * 1024;   // shared memory of one CTA: two CTAs per SM
 constexpr int kPmThreads = 256;
 
-// f(kernel) for the walk the basis asks for: k_pm_pairs<LOOK, CE> without permutations, else k_pm_rows<LOOK, TK, CE,
-// CPLX> (TK only with trivial characters).  The class sums are complex (CPLX) with complex vectors or characters;
-// PM_TABLE runs on trivial characters only, so there CPLX == CE.
+// f(kernel) for the walk the basis asks for: k_pm_pairs<LOOK, CE, JW> without permutations, else k_pm_rows<LOOK, TK,
+// CE, CPLX> (TK only with trivial characters).  The class sums are complex (CPLX) with complex vectors or characters;
+// PM_TABLE runs on trivial characters only, so there CPLX == CE.  JW (fermionic bases) only with PM_NONE.
 template <typename F>
-void with_pm_kernel(int look, int tk, bool ce, bool cplx, F &&f) {
+void with_pm_kernel(int look, int tk, bool ce, bool cplx, bool jw, F &&f) {
   with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
     with_bool(ce, [&](auto e) {
-      if constexpr (lk() <= PM_INVERSION) {
-        f(k_pm_pairs<lk(), e()>);
+      if constexpr (lk() == PM_NONE) {
+        with_bool(jw, [&](auto j) { f(k_pm_pairs<PM_NONE, e(), j()>); });
+      } else if (jw) {
+        throw std::logic_error("k_pm_pairs has Jordan-Wigner builds only without symmetries");
+      } else if constexpr (lk() == PM_INVERSION) {
+        f(k_pm_pairs<lk(), e(), false>);
       } else {
         with_bool(cplx, [&](auto cx) {
           with_choice<6, 4, 0>(tk, [&](auto t) {
@@ -380,7 +390,10 @@ struct SpinArgs {
 };
 
 // One lane owns one row of the target basis and walks its sites; one store of y per row, no atomics.
-template <int LOOK, int TK, int WALK, bool CE>
+// JW (dmv_apply_fermion, PM_NONE with SPIN_SET / SPIN_CLEAR only): the walk is c†_k on the set bits or c_k on the clear
+// bits of the row, each term with the Jordan-Wigner sign (-1)^popc(r & ((1 << k) - 1)); src.site_mask holds the modes
+// the walk visits (one spin half of a spinful basis).
+template <int LOOK, int TK, int WALK, bool CE, bool JW>
 __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
   __shared__ double2 s_k[128];   // k_set [0, N), k_clear [N, 2 N)
   const int N = A.src.n_sites;
@@ -395,6 +408,11 @@ __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
     auto add = [&](double2 k, double2 v) {
       acc.x += k.x * v.x - (CE ? k.y * v.y : 0.0);
       if constexpr (CE) acc.y += k.x * v.y + k.y * v.x;
+    };
+    auto string_sign = [&](double2 k, int mode) {   // k times the Jordan-Wigner sign of `mode` on r
+      if constexpr (JW)
+        if (__popcll(r & ((1ull << mode) - 1)) & 1) return make_double2(-k.x, -k.y);
+      return k;
     };
     if constexpr (WALK == SPIN_SELF) {
       double2 c = A.c0;
@@ -411,12 +429,12 @@ __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
       if constexpr (WALK & SPIN_SET)
         for (uint64_t m = r & mask; m; m &= m - 1) {
           const int k = __ffsll((long long)m) - 1;
-          add(s_k[k], pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+          add(string_sign(s_k[k], k), pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
         }
       if constexpr (WALK & SPIN_CLEAR)
         for (uint64_t m = ~r & mask; m; m &= m - 1) {
           const int k = __ffsll((long long)m) - 1;
-          add(s_k[N + k], pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+          add(string_sign(s_k[N + k], k), pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
         }
     }
     const double s = A.src_scale / (A.row_norms ? __ldg(A.row_norms + i) : A.row_norm);
@@ -428,15 +446,24 @@ __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
 
 constexpr int kSpinThreads = 256;
 
-// f(k_spin_rows<LOOK, TK, WALK, CE>); TK (the square-torus orbit minimum) only for the orbit look-ups
+// f(k_spin_rows<LOOK, TK, WALK, CE, JW>); TK (the square-torus orbit minimum) only for the orbit look-ups, JW only for
+// PM_NONE with the set-bit or clear-bit walk
 template <typename F>
-void with_spin_kernel(int look, int tk, int walk, bool ce, F &&f) {
+void with_spin_kernel(int look, int tk, int walk, bool ce, bool jw, F &&f) {
   with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
     with_choice<SPIN_SELF, SPIN_CLEAR, SPIN_SET, SPIN_BOTH>(walk, [&](auto wk) {
       with_bool(ce, [&](auto e) {
         with_choice<6, 4, 0>(tk, [&](auto t) {
-          if constexpr (lk() >= PM_GROUP || t() == 0) f(k_spin_rows<lk(), t(), wk(), e()>);
-          else throw std::logic_error("k_spin_rows has no square-torus build without a group");
+          if constexpr (lk() == PM_NONE && t() == 0 && (wk() == SPIN_SET || wk() == SPIN_CLEAR)) {
+            with_bool(jw, [&](auto j) { f(k_spin_rows<lk(), t(), wk(), e(), j()>); });
+          } else if (jw) {
+            throw std::logic_error("k_spin_rows has Jordan-Wigner builds only for the set-bit and clear-bit walks "
+                                   "without symmetries");
+          } else if constexpr (lk() >= PM_GROUP || t() == 0) {
+            f(k_spin_rows<lk(), t(), wk(), e(), false>);
+          } else {
+            throw std::logic_error("k_spin_rows has no square-torus build without a group");
+          }
         });
       });
     });
@@ -774,8 +801,8 @@ void pm_finish(int N, const PmClasses &K, const double *sums, double W, const do
 }
 
 // sums[2 c + {0, 1}] = class sum c of the vector A.x over this rank's rows (classes < count).  The lane-major walk runs
-// once per group of classes whose slots fit in shared memory.
-void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, double *sums) {
+// once per group of classes whose slots fit in shared memory.  jw: the Jordan-Wigner walk of fermionic bases.
+void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, bool jw, double *sums) {
   const bool pairs = look <= PM_INVERSION;
   const int per_pass = pairs ? count : (int)(kPmSmem / ((size_t)kPmThreads * (cplx ? 16 : 8)));
   for (int c0 = 0; c0 < count; c0 += per_pass) {
@@ -785,7 +812,7 @@ void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, d
     // thread
     const size_t smem = pairs ? (size_t)A.c_hi * 16 : (size_t)kPmThreads * (A.c_hi - A.c_lo) * (cplx ? 16 : 8);
     const int64_t work = pairs ? (A.n_rows + 31) / 32 : (A.n_rows + kPmThreads - 1) / kPmThreads;
-    with_pm_kernel(look, tk, run.ce, cplx, [&](auto kernel) {
+    with_pm_kernel(look, tk, run.ce, cplx, jw, [&](auto kernel) {
       const int grid = one_wave(kernel, work, smem, kPmThreads);
       A.partials = run.partials((size_t)grid * (A.c_hi - A.c_lo) * 2);
       kernel<<<grid, kPmThreads, smem, run.st>>>(A);
@@ -910,6 +937,56 @@ SpinPlan spin_plan(const SpinBasis &src, const SpinBasis &tgt, int elt, int kind
   return S;
 }
 
+// ---- host half of dmv_apply_fermion: the particle numbers of the two bases.  Returns the modes the walk visits: every
+// mode of a spinless basis; for a spinful one the spin half the non-zero weights lie in (number_up is fixed, so the
+// other half's neighbours of a row are outside the source basis).  The weights themselves go through spin_plan.
+uint64_t fermion_walk(const dmv_context *src, const dmv_context *tgt, int kind, const double *w) {
+  if (kind != DMV_FERMION_CREATE && kind != DMV_FERMION_ANNIHILATE)
+    throw std::runtime_error("kind must be DMV_FERMION_CREATE or DMV_FERMION_ANNIHILATE (got " + std::to_string(kind) +
+                             ")");
+  if (!w) throw std::runtime_error("weights must not be null");
+  if (tgt->particle_type != src->particle_type)
+    throw std::runtime_error(std::string("the target is a ") + particle_name(tgt->particle_type) +
+                             " basis and the source a " + particle_name(src->particle_type) +
+                             " basis: both need the same particle type");
+  const int M = src->n_sites;
+  if (tgt->n_sites != M)
+    throw std::runtime_error("the target has " + std::to_string(tgt->n_sites) + " modes and the source " +
+                             std::to_string(M) + ": both bases need the same number of modes");
+  const int d = kind == DMV_FERMION_CREATE ? 1 : -1;
+  const std::string op = kind == DMV_FERMION_CREATE ? "c†" : "c", sd = d > 0 ? " + 1" : " - 1";
+  if (src->particle_type == DMV_SPINLESS_FERMION) {
+    const int ns = src->number_particles, nt = tgt->number_particles;
+    if (!((ns < 0 && nt < 0) || (ns >= 0 && nt == ns + d)))
+      throw std::runtime_error("particle numbers: " + op + " needs target = source" + sd + " or both free, got source " +
+                               std::to_string(ns) + " and target " + std::to_string(nt));
+    return src->site_mask;
+  }
+  const int N = M / 2;
+  const uint64_t up = (1ull << N) - 1;   // N <= 32
+  bool w_up = false, w_down = false;
+  for (int j = 0; j < M; ++j)
+    if (w[2 * j] != 0.0 || w[2 * j + 1] != 0.0) (j < N ? w_up : w_down) = true;
+  const int su = src->number_up, sdn = src->number_particles - su;
+  const int tu = tgt->number_up, tdn = tgt->number_particles - tu;
+  auto sector = [](int u, int dn) {
+    return "(number_up " + std::to_string(u) + ", number_down " + std::to_string(dn) + ")";
+  };
+  if (w_up && w_down)
+    throw std::runtime_error("the weights are non-zero in both spin halves: " + op + " would reach the sectors " +
+                             sector(su + d, sdn) + " and " + sector(su, sdn + d) +
+                             " at once; apply the up and the down modes separately");
+  const bool to_up = tu == su + d && tdn == sdn, to_down = tu == su && tdn == sdn + d;
+  if (w_up ? !to_up : w_down ? !to_down : !(to_up || to_down))
+    throw std::runtime_error("particle numbers: " + op + " on the " +
+                             (w_up ? "up modes needs the target " + sector(su + d, sdn)
+                              : w_down ? "down modes needs the target " + sector(su, sdn + d)
+                                       : "up or down modes needs the target " + sector(su + d, sdn) + " or " +
+                                             sector(su, sdn + d)) +
+                             " from the source " + sector(su, sdn) + ", got " + sector(tu, tdn));
+  return w_up || (!w_down && to_up) ? up : up << N;
+}
+
 // ---- host half of dmv_reduced_density_matrix: the blocks of ρ_A and the checks of A
 struct RdmLayout {
   int w_first = -1;           // weight of A of the first block; -1 at free weight (one block, every configuration)
@@ -979,49 +1056,17 @@ int64_t rdm_chunk_cols(int d, uint64_t K) {
   return std::min<int64_t>(by_size, (int64_t)((K + 31) / 32 * 32));
 }
 
-}  // namespace
-
-extern "C" {
-
-// ---- spin-spin correlations (DESIGN.md section 3, "dmv_zz_correlations"): one k_zz_gram pass per vector, the
-// (N + 1) x N block all-reduced over the ranks, the group average on the host.
-int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
-                        double *magnetization) {
-  API_BEGIN
-  SolverRun run(ctx, elt, "dmv_zz_correlations", false);
+// The walk of dmv_pm_correlations (spin bases: <σ⁺ᵢσ⁻ⱼ>) and dmv_one_body_density_matrix (fermionic bases: <c†ᵢcⱼ>,
+// with the Jordan-Wigner sign).  A spinful basis fixes number_up, so a pair with one mode in each spin half leaves the
+// basis: such pairs are not walked, and their entries stay exactly 0.  entry / out_name: for the messages.
+void pair_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm, const char *entry,
+                       const char *out_name) {
+  SolverRun run(ctx, elt, entry, false);
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
-  if (!correlations) throw std::runtime_error("correlations must not be null");
-  const int N = ctx->n_sites;
-  const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
-                             ctx->spin_inversion);
-  const size_t words = run.words;
-  cudaStream_t st = run.st;
-  double *partials = run.partials(zz_gram_partials(run.n, N)), *d_gram = run.scalars(zz_gram_size(N));
-  const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * words, st);
-  std::vector<double> C((size_t)num_vectors * N * N), m((size_t)num_vectors * N);
-  for (int v = 0; v < num_vectors; ++v)
-    zz_moments(run, G, xin.ptr + (size_t)v * words, partials, d_gram, C.data() + (size_t)v * N * N,
-               m.data() + (size_t)v * N);
-  CUDA_CHECK(cudaMemcpyAsync(correlations, C.data(), C.size() * sizeof(double), cudaMemcpyDefault, st));
-  if (magnetization)
-    CUDA_CHECK(cudaMemcpyAsync(magnetization, m.data(), m.size() * sizeof(double), cudaMemcpyDefault, st));
-  CUDA_CHECK(cudaStreamSynchronize(st));
-  API_END
-}
-
-// ---- flip-flop correlations (DESIGN.md section 3, "dmv_pm_correlations"): per vector one k_zz_gram pass (W and the
-// magnetisation for the diagonal), one walk over this rank's rows and their antiparallel pairs (k_pm_rows with
-// permutations, k_pm_pairs without) into one sum per class of site pairs, all-reduced over the ranks, finished on the
-// host.  On several ranks the targets are looked up in the whole basis of the replicated-x form, against the gathered x.
-int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm) {
-  API_BEGIN
-  require_spin(ctx, "dmv_pm_correlations");
-  SolverRun run(ctx, elt, "dmv_pm_correlations", false);
-  if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
-  if (!x) throw std::runtime_error("x must not be null");
-  if (!pm) throw std::runtime_error("pm must not be null");
+  if (!pm) throw std::runtime_error(std::string(out_name) + " must not be null");
   const int N = ctx->n_sites, P = run.P;
+  const bool jw = ctx->particle_type != DMV_SPIN;
   const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
                              ctx->spin_inversion);
   const PmClasses K = pm_classes(N, G);
@@ -1031,7 +1076,7 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
   if (P > 1) {
     if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
     if (!ctx->replicated)
-      throw std::runtime_error("dmv_pm_correlations on several ranks needs the whole basis on every rank (the "
+      throw std::runtime_error(std::string(entry) + " on several ranks needs the whole basis on every rank (the "
                                "replicated-x form), and it is switched off by the exchange / mode options or does not "
                                "fit in device memory");
     basis = ctx->global;
@@ -1047,7 +1092,8 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
   std::vector<int16_t> class_of(K.of.begin(), K.of.end());
   std::vector<uint16_t> pairs;
   for (int i = 0; i < N; ++i)
-    for (int j = i + 1; j < N; ++j) pairs.push_back((uint16_t)(i | j << 8));
+    for (int j = i + 1; j < N; ++j)
+      if (ctx->particle_type != DMV_SPINFUL_FERMION || (i < N / 2) == (j < N / 2)) pairs.push_back((uint16_t)(i | j << 8));
   DevBuf<int16_t> d_class_of;
   DevBuf<uint16_t> d_pairs;
   d_class_of.upload(class_of, st);
@@ -1090,7 +1136,7 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
     if (look == PM_TABLE)
       launch_table_fill(basis->n_states, run.ce, A.x, basis->d_norms.ptr, A.pos, basis->d_slot_of.ptr,
                         basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
-    pm_sums(run, A, count, look, tk, cplx, d_sums);
+    pm_sums(run, A, count, look, tk, cplx, jw, d_sums);
     run.all_reduce(d_sums, 2 * (size_t)count);
     CUDA_CHECK(cudaMemcpyAsync(sums.data(), d_sums, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
     check_status(ctx);   // synchronises
@@ -1098,24 +1144,12 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
   }
   CUDA_CHECK(cudaMemcpyAsync(pm, out.data(), out.size() * sizeof(double), cudaMemcpyDefault, st));
   CUDA_CHECK(cudaStreamSynchronize(st));
-  API_END
 }
 
-// ---- one-site operators between bases (DESIGN.md section 3, "dmv_apply_spin"): per vector one k_spin_rows pass over
-// the target's rows of this rank, the source's states found as dmv_pm_correlations finds its targets.  On several ranks
-// in the source's whole-basis twin against the gathered x.
-int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights, int num_vectors,
-                   const void *x, void *y) {
-  API_BEGIN
-  if (!target || !source) throw std::runtime_error("target and source must not be null");
-  require_spin(source, "dmv_apply_spin");
-  require_spin(target, "dmv_apply_spin");
-  SolverRun run(source, elt, "dmv_apply_spin", false);
-  require_states(target);
-  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
-  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
-    throw std::runtime_error("target and source must have the same rank and number of ranks");
-  const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt, kind, weights);
+// The launch half of dmv_apply_spin and dmv_apply_fermion: per vector one k_spin_rows pass over the target's rows of
+// this rank.  walk_mask: the modes the set-bit / clear-bit walks visit; jw: Jordan-Wigner signs (fermionic bases).
+void apply_one_site(SolverRun &run, dmv_context *target, dmv_context *source, int elt, const SpinPlan &S, bool jw,
+                    uint64_t walk_mask, int num_vectors, const void *x, void *y, const char *entry) {
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
   if (!y) throw std::runtime_error("y must not be null");
@@ -1125,7 +1159,7 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
   if (P > 1) {
     if (!source->exchange_decided) decide_exchange(source);   // collective: every rank reaches the same decision
     if (!source->replicated)
-      throw std::runtime_error("dmv_apply_spin on several ranks needs the source's whole basis on every rank (the "
+      throw std::runtime_error(std::string(entry) + " on several ranks needs the source's whole basis on every rank (the "
                                "replicated-x form), and it is switched off by the exchange / mode options or does not "
                                "fit in device memory");
     basis = source->global;
@@ -1144,7 +1178,7 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
   A.src.orbit = basis->orbit;
   A.src.norms = basis->d_norms.ptr;
   A.src.pos = P > 1 ? source->d_pos.ptr : nullptr;
-  A.src.site_mask = source->site_mask;
+  A.src.site_mask = walk_mask;
   A.src.inversion_character = (double)source->spin_inversion;
   A.src.n_sites = N;
   A.src.status = source->d_status.ptr;
@@ -1178,7 +1212,7 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
       launch_table_fill(basis->n_states, run.ce, A.src.x, basis->d_norms.ptr, A.src.pos, basis->d_slot_of.ptr,
                         basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
     if (A.n_rows > 0)
-      with_spin_kernel(look, tk, S.walk, run.ce, [&](auto kernel) {
+      with_spin_kernel(look, tk, S.walk, run.ce, jw, [&](auto kernel) {
         const int grid = one_wave(kernel, (A.n_rows + kSpinThreads - 1) / kSpinThreads, 0, kSpinThreads);
         kernel<<<grid, kSpinThreads, 0, st>>>(A);
         check_launch("k_spin_rows");
@@ -1186,6 +1220,95 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
   }
   yout.finish(st);
   check_status(source);   // synchronises
+  }
+
+}  // namespace
+
+extern "C" {
+
+// ---- spin-spin correlations (DESIGN.md section 3, "dmv_zz_correlations"): one k_zz_gram pass per vector, the
+// (N + 1) x N block all-reduced over the ranks, the group average on the host.
+int dmv_zz_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *correlations,
+                        double *magnetization) {
+  API_BEGIN
+  SolverRun run(ctx, elt, "dmv_zz_correlations", false);
+  if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
+  if (!x) throw std::runtime_error("x must not be null");
+  if (!correlations) throw std::runtime_error("correlations must not be null");
+  const int N = ctx->n_sites;
+  const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
+                             ctx->spin_inversion);
+  const size_t words = run.words;
+  cudaStream_t st = run.st;
+  double *partials = run.partials(zz_gram_partials(run.n, N)), *d_gram = run.scalars(zz_gram_size(N));
+  const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * words, st);
+  std::vector<double> C((size_t)num_vectors * N * N), m((size_t)num_vectors * N);
+  for (int v = 0; v < num_vectors; ++v)
+    zz_moments(run, G, xin.ptr + (size_t)v * words, partials, d_gram, C.data() + (size_t)v * N * N,
+               m.data() + (size_t)v * N);
+  CUDA_CHECK(cudaMemcpyAsync(correlations, C.data(), C.size() * sizeof(double), cudaMemcpyDefault, st));
+  if (magnetization)
+    CUDA_CHECK(cudaMemcpyAsync(magnetization, m.data(), m.size() * sizeof(double), cudaMemcpyDefault, st));
+  CUDA_CHECK(cudaStreamSynchronize(st));
+  API_END
+}
+
+// ---- flip-flop correlations (DESIGN.md section 3, "dmv_pm_correlations"): per vector one k_zz_gram pass (W and the
+// magnetisation for the diagonal), one walk over this rank's rows and their antiparallel pairs (k_pm_rows with
+// permutations, k_pm_pairs without) into one sum per class of site pairs, all-reduced over the ranks, finished on the
+// host.  On several ranks the targets are looked up in the whole basis of the replicated-x form, against the gathered x.
+int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x, double *pm) {
+  API_BEGIN
+  require_spin(ctx, "dmv_pm_correlations");
+  pair_correlations(ctx, elt, num_vectors, x, pm, "dmv_pm_correlations", "pm");
+  API_END
+}
+
+// ---- the one-body density matrix of a fermionic basis (DESIGN.md section 3, "dmv_one_body_density_matrix"): the walk
+// of dmv_pm_correlations with a Jordan-Wigner sign on each term, over the pairs of modes that stay in the basis.
+int dmv_one_body_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, double *out) {
+  API_BEGIN
+  require_fermion(ctx, "dmv_one_body_density_matrix");
+  pair_correlations(ctx, elt, num_vectors, x, out, "dmv_one_body_density_matrix", "out");
+  API_END
+}
+
+// ---- one-site operators between bases (DESIGN.md section 3, "dmv_apply_spin"): per vector one k_spin_rows pass over
+// the target's rows of this rank, the source's states found as dmv_pm_correlations finds its targets.  On several ranks
+// in the source's whole-basis twin against the gathered x.
+int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights, int num_vectors,
+                   const void *x, void *y) {
+  API_BEGIN
+  if (!target || !source) throw std::runtime_error("target and source must not be null");
+  require_spin(source, "dmv_apply_spin");
+  require_spin(target, "dmv_apply_spin");
+  SolverRun run(source, elt, "dmv_apply_spin", false);
+  require_states(target);
+  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
+  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
+    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt, kind, weights);
+  apply_one_site(run, target, source, elt, S, false, source->site_mask, num_vectors, x, y, "dmv_apply_spin");
+  API_END
+}
+
+// ---- c† and c between particle sectors (DESIGN.md section 3, "dmv_apply_fermion"): the walk of dmv_apply_spin with a
+// Jordan-Wigner sign on each term, over the modes of the spin half the weights live in.
+int dmv_apply_fermion(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
+                      int num_vectors, const void *x, void *y) {
+  API_BEGIN
+  if (!target || !source) throw std::runtime_error("target and source must not be null");
+  require_fermion(source, "dmv_apply_fermion");
+  require_fermion(target, "dmv_apply_fermion");
+  SolverRun run(source, elt, "dmv_apply_fermion", false);
+  require_states(target);
+  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
+  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
+    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  const uint64_t walk_mask = fermion_walk(source, target, kind, weights);
+  const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt,
+                               kind == DMV_FERMION_CREATE ? DMV_SPIN_PLUS : DMV_SPIN_MINUS, weights);
+  apply_one_site(run, target, source, elt, S, true, walk_mask, num_vectors, x, y, "dmv_apply_fermion");
   API_END
 }
 

@@ -455,6 +455,59 @@ class Operator:
                                            _ptr(x), _ptr(y)))
         return y
 
+    def one_body_density_matrix(self, x):
+        """The one-body density matrix G[i, j] = <x|c†ᵢ cⱼ|x> / <x|x> of a fermionic basis on the device
+        (dmv_one_body_density_matrix), i, j over the modes (spinful: site, then site + N for down).  A spinful basis
+        fixes number_up, so its cross-spin block is exactly 0.  x as for zz_correlations.
+        -> numpy complex128 of shape (M, M), or (k, M, M) for a batch, M the number of modes."""
+        elt = _elt_of(x)
+        n, M = self.basis.numberStates(), self.spec.basis.number_bits
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        if _is_torch(x):
+            self.use_torch_stream()
+        else:
+            x = np.ascontiguousarray(x)
+        out = np.zeros((k, M, M), dtype=np.complex128)
+        nat.check(nat.lib().dmv_one_body_density_matrix(self._ctx, elt, k, _ptr(x), out.ctypes.data))
+        return out[0] if x.ndim == 1 else out
+
+    _FERMION_KINDS = {"c+": 0, "c†": 0, "c": 1}
+
+    def apply_fermion(self, kind: str, weights, x, target: "Operator"):
+        """y = O x with O = sum_j weights[j] c†_j (kind "c+" or "c†") or sum_j weights[j] c_j (kind "c") on the device
+        (dmv_apply_fermion), from this fermionic basis into `target`'s particle sector (one particle more for c†, one
+        fewer for c; on a spinful basis the non-zero weights lie in one spin half, whose count changes).  x, weights
+        and y as for apply_spin, with one weight per mode.  Collective when num_ranks > 1.
+        -> y of shape (n_target,) or (k, n_target), of x's kind and type."""
+        if kind not in self._FERMION_KINDS:
+            raise ValueError(f"kind must be one of {sorted(self._FERMION_KINDS)}, got {kind!r}")
+        elt = _elt_of(x)
+        n, M = self.basis.numberStates(), self.spec.basis.number_bits
+        if x.ndim not in (1, 2) or int(x.shape[-1]) != n:
+            raise ValueError(f"x must have shape ({n},) or (k, {n})")
+        w = np.ascontiguousarray(np.asarray(weights, dtype=np.complex128).reshape(-1))
+        if w.shape[0] != M:
+            raise ValueError(f"weights must have {M} entries")
+        k = 1 if x.ndim == 1 else int(x.shape[0])
+        m = target.basis.numberStates()
+        shape = (m,) if x.ndim == 1 else (k, m)
+        if _is_torch(x):
+            import torch
+            if not x.is_cuda:
+                raise ValueError("a torch x must be a CUDA tensor")
+            self.use_torch_stream()
+            target.use_torch_stream()
+            x = x.contiguous()
+            y = torch.empty(shape, dtype=x.dtype, device=x.device)
+        else:
+            x = np.ascontiguousarray(x)
+            y = np.empty(shape, dtype=x.dtype)
+        nat.check(nat.lib().dmv_apply_fermion(target._ctx, self._ctx, elt, self._FERMION_KINDS[kind], w.ctypes.data, k,
+                                              _ptr(x), _ptr(y)))
+        return y
+
     def reduced_density_matrix(self, x, sites):
         """ρ_A = Tr_B |ψ><ψ| of ψ = B x / ‖x‖ for the sites A = `sites` (1 to 16 distinct sites; bit k of a row of ρ_A is
         site sites[k]) on the device (dmv_reduced_density_matrix).  x as for zz_correlations.  Collective when

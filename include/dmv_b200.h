@@ -79,7 +79,8 @@ int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op,
  * is allocated: permutations or spin inversion with fermions; an odd bit count for spinful fermions; number_up outside
  * 0..N or number_particles - number_up outside 0..N; a spinless number_particles outside -1..number_sites.
  * On a fermionic context dmv_pm_correlations, dmv_apply_spin and dmv_reduced_density_matrix refuse (they assume spin
- * operators without strings); dmv_zz_correlations gives <(2n_a - 1)(2n_b - 1)> over the bits.
+ * operators without strings); dmv_zz_correlations gives <(2n_a - 1)(2n_b - 1)> over the bits; dmv_one_body_density_matrix
+ * and dmv_apply_fermion (below) are the single-particle observables, and refuse a spin context.
  * Info "particle_type" answers the constant below. */
 enum { DMV_SPIN = 0, DMV_SPINLESS_FERMION = 1, DMV_SPINFUL_FERMION = 2 };
 typedef struct {
@@ -376,6 +377,38 @@ int dmv_pm_correlations(dmv_context *ctx, int elt, int num_vectors, const void *
 enum { DMV_SPIN_ONE = 0, DMV_SPIN_Z = 1, DMV_SPIN_PLUS = 2, DMV_SPIN_MINUS = 3 };
 int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
                    int num_vectors, const void *x, void *y);
+
+/* ---- single-particle observables of fermionic bases on the device (row f11; not in the reference).  Conventions: the
+ * M = number_sites bits are the modes; spinful mode = site for up and site + N for down (N = M / 2).  c_k carries the
+ * Jordan-Wigner string of every mode below it: c_k|s> = (-1)^popc(s & ((1 << k) - 1)) |s ^ (1 << k)> for bit k set, so
+ * the string of a down mode runs over every up mode (the convention of the fermionic operator expressions).
+ *
+ * dmv_one_body_density_matrix: G[i, j] = <x|c†ᵢ cⱼ|x> / <x|x> for num_vectors vectors of a fermionic context (layout of
+ * x as dmv_zz_correlations).  out: num_vectors * M * M complex numbers (vector, i, j), interleaved (re, im), host or
+ * device, as dmv_pm_correlations.  G is Hermitian; G[i, i] = <nᵢ> = (1 + mᵢ) / 2 with m from dmv_zz_correlations.  A
+ * spinful basis fixes number_up, so its cross-spin block (i and j in different halves) is exactly 0 and is never walked.
+ * Method: the pair-major walk of dmv_pm_correlations (k_pm_pairs) over the rows b with bit i set and bit j clear, each
+ * term conj(x_b) x[b ^ (1 << i | 1 << j)] (-1)^popc(b & between(i, j)), between(i, j) the bits strictly between i and j.
+ * elt = DMV_F64 or DMV_C128.  Refused, with nothing written: a spin-1/2 context, a zero vector, null pointers,
+ * num_vectors < 1, and several ranks without dmv_comm_init.  Collective when num_ranks > 1 (the whole basis on every
+ * rank, as dmv_pm_correlations); every rank returns the same matrices.  A repeated call is bit-identical.
+ *
+ * dmv_apply_fermion: y = O x from the source's particle sector into the target's, O = Σⱼ wⱼ c†ⱼ (DMV_FERMION_CREATE) or
+ * Σⱼ wⱼ cⱼ (DMV_FERMION_ANNIHILATE); weights: M complex numbers, interleaved (re, im).  Row r of the target:
+ *     c†: Σ over the set bits k of r of   w_k (-1)^popc(r & ((1 << k) - 1)) x[r ^ (1 << k)],
+ *     c:  Σ over the clear bits k of r of w_k (-1)^popc(r & ((1 << k) - 1)) x[r | (1 << k)].
+ * Accepted: two fermionic contexts of one particle type, with the same number of modes, device, rank and number of
+ * ranks.  Spinless: target number_particles = source ± 1 (c† / c), or both free.  Spinful: the non-zero weights lie in
+ * one spin half and that half's count changes by ± 1 while the other stays (all-zero weights: either half); weights
+ * non-zero in both halves are refused, the message naming the two sectors they would reach.  DMV_F64 needs real
+ * weights.  x, y: [num_vectors, n] of each context, host or device.  Refused, with nothing written: anything else, as
+ * dmv_apply_spin.  Method: k_spin_rows, one lane per target row walking the modes of its half, one store per row, no
+ * atomics: a repeated call is bit-identical.  Collective when num_ranks > 1 (needs dmv_comm_init on the source and its
+ * whole basis on every rank, as dmv_apply_spin). */
+int dmv_one_body_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, double *out);
+enum { DMV_FERMION_CREATE = 0, DMV_FERMION_ANNIHILATE = 1 };
+int dmv_apply_fermion(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
+                      int num_vectors, const void *x, void *y);
 
 /* ---- bipartite entanglement on the device (row f9; not in the reference): the reduced density matrix
  * ρ_A = Tr_B |ψ><ψ| of the normalised full-space state ψ = B x / ‖x‖ (B the basis of dmv_apply_spin, so
