@@ -704,11 +704,11 @@ uint32_t dord_build(const uint64_t *reps, int64_t n, OrderedDir &D, std::vector<
   return (uint32_t)placed;
 }
 
-// hash table of k_rows over ctx's representatives: keys once per basis and element type, values once per product
-void ensure_table(dmv_context *ctx, int elt) {
+// hash table of k_rows over ctx's representatives: keys once per basis and element type (built on st), values once per
+// product (fill_table)
+void ensure_table(dmv_context *ctx, int elt, cudaStream_t st) {
   if (ctx->table_elt == elt) return;
   const int64_t n = ctx->n_states;
-  cudaStream_t st = ctx->stream;
   const bool ce = elt == DMV_C128;
   ctx->dense_order = dense_order_wanted(ctx) && n >= 1;
   ctx->dord = DenseOrder{};
@@ -836,6 +836,12 @@ void ensure_table(dmv_context *ctx, int elt) {
   ctx->table_elt = elt;
 }
 
+// the values of ctx's table (ensure_table) from x, indexed like ctx's states (through pos when given)
+void fill_table(dmv_context *ctx, int elt, const void *x, const uint32_t *pos, cudaStream_t st) {
+  launch_table_fill(ctx->n_states, elt == DMV_C128, x, ctx->d_norms.ptr, pos, ctx->d_slot_of.ptr, ctx->d_reps.ptr,
+                    ctx->d_table.ptr, ctx->dense_index || ctx->dense_order ? ctx->d_dense.ptr : nullptr, st);
+}
+
 // y[rows] <- rows of H through k_rows.  `basis` owns the table (this rank's context, or the twin holding the whole
 // basis in the replicated-x product), x_all is indexed like basis' states (through pos when given), p names the rows.
 void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_all, const uint32_t *pos,
@@ -845,15 +851,10 @@ void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_al
   p.uni_re = basis->gather_uni[0]; p.uni_im = basis->gather_uni[1];
   // the term store when it applies (dmv_store.cu): no orbit minimum and no table look-up per product
   if (rows_store_product(basis, p, elt, x_all, pos, stream, fill, timer)) return;
-  cudaStream_t keep = basis->stream;
-  basis->stream = stream;
-  ensure_table(basis, elt);
-  basis->stream = keep;
+  ensure_table(basis, elt, stream);
   if (fill) {   // (a product cut into row chunks refreshes the values once, with its first chunk)
     CUDA_CHECK(cudaEventRecord(timer->ev_fill[0], stream));
-    launch_table_fill(basis->n_states, elt == DMV_C128, x_all, basis->d_norms.ptr, pos, basis->d_slot_of.ptr,
-                      basis->d_reps.ptr, basis->d_table.ptr,
-                      basis->dense_index || basis->dense_order ? basis->d_dense.ptr : nullptr, stream);
+    fill_table(basis, elt, x_all, pos, stream);
     CUDA_CHECK(cudaEventRecord(timer->ev_fill[1], stream));
     timer->fill_timed = true;
   }

@@ -479,7 +479,8 @@ VecStage stage_vectors(dmv_context *ctx, int elt, const void *x, void *y);
 void finish_vectors(dmv_context *ctx, const VecStage &v);
 void upload_out_pointers(dmv_context *ctx);
 void do_plan(dmv_context *ctx);
-void ensure_table(dmv_context *ctx, int elt);
+void ensure_table(dmv_context *ctx, int elt, cudaStream_t st);
+void fill_table(dmv_context *ctx, int elt, const void *x, const uint32_t *pos, cudaStream_t st);
 void rows_product_batch(dmv_context *ctx, int elt, int nv, const void *x, void *y, int64_t stride);
 void rows_product(dmv_context *basis, KernelParams &p, int elt, const void *x_all, const uint32_t *pos, cudaStream_t stream, bool fill = true, dmv_context *timer = nullptr);
 // the term store (dmv_store.cu): the plan of a store from sizes alone, and the product on it (false: the product is

@@ -132,37 +132,13 @@ auto with_zz_gram(bool complex_elements, int n_sites, F &&f) {
   });
 }
 
-// ---- flip-flop correlations (dmv_pm_correlations).  A row b and an antiparallel pair (i, j) with bit i of b set and
-// bit j clear give the term conj(x_b) / n_b chi (n x)[rep(b ^ (1 << i | 1 << j))] of the class of the ordered pair
-// (i, j); the host turns the class sums into <σ⁺ᵢσ⁻ⱼ>.  How the target's (n x) is found:
-enum PmLook {
-  PM_NONE = 0,        // no symmetry: the index of the basis
-  PM_INVERSION = 1,   // spin inversion alone: min(a, flip a), the character when flipped
-  PM_GROUP = 2,       // permutations: orbit minimum (orbit_scan and its character when they are not trivial), the index
-  PM_TABLE = 3,       // permutations, trivial characters: orbit minimum, then k_rows' hash table (x n in the slot)
-};
-
-struct PmArgs {
-  StateIndex index;          // the basis the targets are looked up in: this rank's, or the whole basis on several ranks
-  OrbitProgram orbit;
-  const double *norms;       // of index's states
-  const uint32_t *pos;       // several ranks: global index g lives at x[pos[g]]; null on one rank
-  const double *x;           // the vector (the gathered one on several ranks)
-  const uint64_t *rows;      // this rank's representatives and their norms
-  const double *row_norms;
-  int64_t n_rows, x_row_offset;
-  uint64_t site_mask;
-  double inversion_character;
-  const unsigned char *table;   // PM_TABLE: k_rows' table (table_slot / ordered layout), filled from x
-  uint32_t table_slots;
-  OrderedDir table_dir;
-  DenseOrder dord;              // ... or the dense ordered table (blocks not null), its slots in `dense`
-  const unsigned char *dense;
-  const int16_t *class_of;   // [N * N]: class of the ordered pair (i, j), -1 on the diagonal
-  const uint16_t *pairs;     // pair-major walk: the unordered pairs i | j << 8
-  int n_sites, n_pairs, c_lo, c_hi;   // classes [c_lo, c_hi) of this pass
-  double *partials;          // [grid][c_hi - c_lo][2]
-  unsigned long long *status;
+// ---- the look-up of the observables (k_pm_*, k_spin_rows, k_rdm_fill): chi (n x)[rep(a)] at any state a of a basis's
+// sector, through StateLookup::at.  The host half (ObservableLookup, below) picks the build and fills the struct.
+enum LookupKind {
+  LOOK_NONE = 0,        // no symmetry: the index of the basis
+  LOOK_INVERSION = 1,   // spin inversion alone: min(a, flip a), the character when flipped
+  LOOK_GROUP = 2,       // permutations: orbit minimum (orbit_scan and its character when they are not trivial), the index
+  LOOK_TABLE = 3,       // permutations, trivial characters: orbit minimum, then k_rows' hash table (x n in the slot)
 };
 
 template <bool CE>
@@ -171,78 +147,127 @@ __device__ __forceinline__ double2 pm_load(const double *x, int64_t i) {
   else return make_double2(__ldg(x + i), 0.0);
 }
 
-// chi (n x)[rep(a)]; a target outside the basis is counted in bad / bad_state unless its projection vanishes (a
-// stabiliser sum of zero under non-trivial characters), which contributes nothing
-template <int LOOK, int TK, bool CE>
-__device__ __forceinline__ double2 pm_target(const PmArgs &A, uint64_t a, unsigned long long &bad, uint64_t &bad_state) {
-  double2 chi = make_double2(1.0, 0.0);
-  uint64_t key = a;
-  if constexpr (LOOK == PM_INVERSION) {
-    const uint64_t inv = a ^ A.site_mask;
-    if (inv < a) { key = inv; chi.x = A.inversion_character; }
-  } else if constexpr (LOOK == PM_GROUP || LOOK == PM_TABLE) {
-    if (LOOK == PM_TABLE || A.orbit.trivial_characters) {
-      if constexpr (TK > 0) key = orbit_min_torus_sq<TK>(A.orbit, a);
-      else key = orbit_representative(A.orbit, a);
-    } else {
-      const OrbitResult r = orbit_scan<false, false>(A.orbit, a);
-      key = r.rep;
-      chi = __ldg(A.orbit.characters + r.arg);   // chi(g), not conjugated: the convention of k_pull
+struct StateLookup {
+  StateIndex index;          // the basis the states are looked up in: this rank's, or the whole basis on several ranks
+  OrbitProgram orbit;
+  const double *norms;       // of index's states
+  const uint32_t *pos;       // several ranks: global index g lives at x[pos[g]]; null on one rank
+  const double *x;           // the vector (the gathered one on several ranks)
+  uint64_t site_mask;        // the basis's sites, all flipped by spin inversion
+  double inversion_character;
+  const unsigned char *table;   // LOOK_TABLE: k_rows' table (table_slot / ordered layout), filled from x
+  uint32_t table_slots;
+  OrderedDir table_dir;
+  DenseOrder dord;              // ... or the dense ordered table (blocks not null), its slots in `dense`
+  const unsigned char *dense;
+  unsigned long long *status;
+
+  // chi (n x)[rep(a)]; a state outside the basis is counted in bad / bad_state unless its projection vanishes (a
+  // stabiliser sum of zero under non-trivial characters), which contributes nothing
+  template <int LOOK, int TK, bool CE>
+  __device__ __forceinline__ double2 at(uint64_t a, unsigned long long &bad, uint64_t &bad_state) const {
+    double2 chi = make_double2(1.0, 0.0);
+    uint64_t key = a;
+    if constexpr (LOOK == LOOK_INVERSION) {
+      const uint64_t inv = a ^ site_mask;
+      if (inv < a) { key = inv; chi.x = inversion_character; }
+    } else if constexpr (LOOK == LOOK_GROUP || LOOK == LOOK_TABLE) {
+      if (LOOK == LOOK_TABLE || orbit.trivial_characters) {
+        if constexpr (TK > 0) key = orbit_min_torus_sq<TK>(orbit, a);
+        else key = orbit_representative(orbit, a);
+      } else {
+        const OrbitResult r = orbit_scan<false, false>(orbit, a);
+        key = r.rep;
+        chi = __ldg(orbit.characters + r.arg);   // chi(g), not conjugated: the convention of k_pull
+      }
     }
-  }
-  if constexpr (LOOK == PM_TABLE) {
-    if (A.dord.blocks != nullptr) {   // dense ordered table: the rank block, then the slot (or the block's leftovers)
-      const uint64_t h = dord_hash(key);
-      const uint32_t p = ordered_block(key, A.table_dir.k_lo, A.table_dir.shift, A.table_dir.last);
-      const uint64_t *w = A.dord.blocks + 4 * (size_t)dord_block(h, __ldg(A.table_dir.dir + p), __ldg(A.table_dir.dir + p + 1));
-      uint32_t end = 0;
-      for (uint32_t s = dord_slot(__ldg(w), __ldg(w + 1), __ldg(w + 2), __ldg(w + 3), dord_bits(h), end); s < end; ++s) {
-        const size_t width = CE ? 32 : 16;
-        const ulonglong2 kv = __ldg(reinterpret_cast<const ulonglong2 *>(A.dense + s * width));
-        if (kv.x != key) continue;
-        if (CE) return __ldg(reinterpret_cast<const double2 *>(A.dense + s * width + 16));
-        return make_double2(__longlong_as_double((long long)kv.y), 0.0);
+    if constexpr (LOOK == LOOK_TABLE) {
+      if (dord.blocks != nullptr) {   // dense ordered table: the rank block, then the slot (or the block's leftovers)
+        const uint64_t h = dord_hash(key);
+        const uint32_t p = ordered_block(key, table_dir.k_lo, table_dir.shift, table_dir.last);
+        const uint64_t *w = dord.blocks + 4 * (size_t)dord_block(h, __ldg(table_dir.dir + p), __ldg(table_dir.dir + p + 1));
+        uint32_t end = 0;
+        for (uint32_t s = dord_slot(__ldg(w), __ldg(w + 1), __ldg(w + 2), __ldg(w + 3), dord_bits(h), end); s < end; ++s) {
+          const size_t width = CE ? 32 : 16;
+          const ulonglong2 kv = __ldg(reinterpret_cast<const ulonglong2 *>(dense + s * width));
+          if (kv.x != key) continue;
+          if (CE) return __ldg(reinterpret_cast<const double2 *>(dense + s * width + 16));
+          return make_double2(__longlong_as_double((long long)kv.y), 0.0);
+        }
+        ++bad; bad_state = key;
+        return make_double2(0.0, 0.0);
+      }
+      uint32_t bk = table_home(key, table_slots, table_dir);
+      for (;;) {
+        const ulonglong2 k = __ldg(reinterpret_cast<const ulonglong2 *>(table + (size_t)bk * 32));
+        const double2 v = __ldg(reinterpret_cast<const double2 *>(table + (size_t)bk * 32 + 16));
+        if (CE) {   // { key, spare, re, im }
+          if (k.x == key) return v;
+          if (k.x == kEmptyKey) break;
+        } else {    // { key0, key1, value0, value1 }
+          if (k.x == key) return make_double2(v.x, 0.0);
+          if (k.y == key) return make_double2(v.y, 0.0);
+          if (k.x == kEmptyKey || k.y == kEmptyKey) break;
+        }
+        bk = bk + 1 == table_slots ? 0 : bk + 1;
       }
       ++bad; bad_state = key;
       return make_double2(0.0, 0.0);
-    }
-    uint32_t bk = table_home(key, A.table_slots, A.table_dir);
-    for (;;) {
-      const ulonglong2 k = __ldg(reinterpret_cast<const ulonglong2 *>(A.table + (size_t)bk * 32));
-      const double2 v = __ldg(reinterpret_cast<const double2 *>(A.table + (size_t)bk * 32 + 16));
-      if (CE) {   // { key, spare, re, im }
-        if (k.x == key) return v;
-        if (k.x == kEmptyKey) break;
-      } else {    // { key0, key1, value0, value1 }
-        if (k.x == key) return make_double2(v.x, 0.0);
-        if (k.y == key) return make_double2(v.y, 0.0);
-        if (k.x == kEmptyKey || k.y == kEmptyKey) break;
+    } else {
+      const int64_t idx = locate(index, key);
+      if (idx < 0) {
+        if (LOOK != LOOK_GROUP || orbit.trivial_characters ||
+            orbit_stabiliser_sum(orbit, key) > 1e-12 * (double)orbit.group_order) { ++bad; bad_state = key; }
+        return make_double2(0.0, 0.0);
       }
-      bk = bk + 1 == A.table_slots ? 0 : bk + 1;
+      double2 v = pm_load<CE>(x, pos ? (int64_t)__ldg(pos + idx) : idx);
+      if constexpr (LOOK == LOOK_GROUP) {
+        const double nrm = __ldg(norms + idx);
+        v = make_double2(v.x * nrm, v.y * nrm);
+      }
+      return make_double2(chi.x * v.x - chi.y * v.y, chi.x * v.y + chi.y * v.x);
     }
-    ++bad; bad_state = key;
-    return make_double2(0.0, 0.0);
-  } else {
-    const int64_t idx = locate(A.index, key);
-    if (idx < 0) {
-      if (LOOK != PM_GROUP || A.orbit.trivial_characters ||
-          orbit_stabiliser_sum(A.orbit, key) > 1e-12 * (double)A.orbit.group_order) { ++bad; bad_state = key; }
-      return make_double2(0.0, 0.0);
-    }
-    double2 v = pm_load<CE>(A.x, A.pos ? (int64_t)__ldg(A.pos + idx) : idx);
-    if constexpr (LOOK == PM_GROUP) {
-      const double nrm = __ldg(A.norms + idx);
-      v = make_double2(v.x * nrm, v.y * nrm);
-    }
-    return make_double2(chi.x * v.x - chi.y * v.y, chi.x * v.y + chi.y * v.x);
   }
+};
+
+// the states a kernel found outside the basis: status[0] counts them, status[1] holds one of them
+__device__ __forceinline__ void report_bad(unsigned long long *status, unsigned long long bad, uint64_t bad_state) {
+  if (bad && atomicAdd(status, bad) == 0) status[1] = bad_state;
 }
+
+// f(lk, tk, ce): the look-up builds (LOOK, TK, CE) as compile-time constants.  TK, the square-torus orbit minimum
+// (rows_torus_k: 6, 4 or 0), exists only for the orbit look-ups, LOOK >= LOOK_GROUP.
+template <typename F>
+void with_lookup(const char *kernel, int look, int tk, bool ce, F &&f) {
+  with_choice<LOOK_NONE, LOOK_INVERSION, LOOK_GROUP, LOOK_TABLE>(look, [&](auto lk) {
+    with_bool(ce, [&](auto e) {
+      with_choice<6, 4, 0>(tk, [&](auto t) {
+        if constexpr (lk() >= LOOK_GROUP || t() == 0) f(lk, t, e);
+        else throw std::logic_error(std::string(kernel) + " has no square-torus build without a group");
+      });
+    });
+  });
+}
+
+// ---- flip-flop correlations (dmv_pm_correlations).  A row b and an antiparallel pair (i, j) with bit i of b set and
+// bit j clear give the term conj(x_b) / n_b chi (n x)[rep(b ^ (1 << i | 1 << j))] of the class of the ordered pair
+// (i, j); the host turns the class sums into <σ⁺ᵢσ⁻ⱼ>.  The rows are the looked-up basis's own (this rank's share).
+struct PmArgs {
+  StateLookup look;
+  const uint64_t *rows;      // this rank's representatives and their norms
+  const double *row_norms;
+  int64_t n_rows, x_row_offset;
+  const int16_t *class_of;   // [N * N]: class of the ordered pair (i, j), -1 on the diagonal
+  const uint16_t *pairs;     // pair-major walk: the unordered pairs i | j << 8
+  int n_sites, n_pairs, c_lo, c_hi;   // classes [c_lo, c_hi) of this pass
+  double *partials;          // [grid][c_hi - c_lo][2]
+};
 
 // conj(x_b) / n_b of row i
 template <int LOOK, bool CE>
 __device__ __forceinline__ double2 pm_row_factor(const PmArgs &A, int64_t i) {
-  const double2 v = pm_load<CE>(A.x, A.x_row_offset + i);
-  const double s = LOOK >= PM_GROUP ? 1.0 / __ldg(A.row_norms + i) : 1.0;
+  const double2 v = pm_load<CE>(A.look.x, A.x_row_offset + i);
+  const double s = LOOK >= LOOK_GROUP ? 1.0 / __ldg(A.row_norms + i) : 1.0;
   return make_double2(v.x * s, -v.y * s);
 }
 
@@ -259,14 +284,14 @@ __global__ void __launch_bounds__(256, 2) k_pm_rows(const PmArgs A) {
   for (int64_t i = (int64_t)blockIdx.x * T + t; i < A.n_rows; i += (int64_t)gridDim.x * T) {
     const uint64_t b = __ldg(A.rows + i);
     const double2 xb = pm_row_factor<LOOK, CE>(A, i);
-    for (uint64_t up = b & A.site_mask; up; up &= up - 1) {
+    for (uint64_t up = b & A.look.site_mask; up; up &= up - 1) {
       const int si = __ffsll((long long)up) - 1;
       const int16_t *cls = A.class_of + si * N;
-      for (uint64_t dn = ~b & A.site_mask; dn; dn &= dn - 1) {
+      for (uint64_t dn = ~b & A.look.site_mask; dn; dn &= dn - 1) {
         const int sj = __ffsll((long long)dn) - 1;
         const int c = (int)__ldg(cls + sj) - A.c_lo;
         if ((unsigned)c >= (unsigned)C) continue;
-        const double2 v = pm_target<LOOK, TK, CE>(A, b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
+        const double2 v = A.look.at<LOOK, TK, CE>(b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
         s_slot[c * T + t] += xb.x * v.x - xb.y * v.y;
         if constexpr (CPLX) s_slot[(C + c) * T + t] += xb.x * v.y + xb.y * v.x;
       }
@@ -282,14 +307,14 @@ __global__ void __launch_bounds__(256, 2) k_pm_rows(const PmArgs A) {
     A.partials[((int64_t)blockIdx.x * C + c) * 2] = re;
     A.partials[((int64_t)blockIdx.x * C + c) * 2 + 1] = im;
   }
-  if (bad && atomicAdd(A.status, bad) == 0) A.status[1] = bad_state;
+  report_bad(A.look.status, bad, bad_state);
 }
 
 // Pair-major walk (bases without permutations: a class per ordered pair, or per {(i, j), (j, i)} with spin inversion).
 // The CTA's warps share a tile of 32 rows, one per lane; warp w takes the unordered pairs w, w + warps, ..., every lane
 // adds its row's term and the warp sums them by shuffles in a fixed order, one sum per direction of the pair.  The
 // classes of an unordered pair belong to one warp only, so lane 0 owns their slots in shared memory.
-// JW (fermionic bases, PM_NONE only): the term of c†ᵢcⱼ carries the Jordan-Wigner sign (-1)^popc(b & between(i, j)),
+// JW (fermionic bases, LOOK_NONE only): the term of c†ᵢcⱼ carries the Jordan-Wigner sign (-1)^popc(b & between(i, j)),
 // the bits strictly between the two modes; b and its target agree there, so both directions of a pair take one sign.
 template <int LOOK, bool CE, bool JW>
 __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
@@ -309,7 +334,7 @@ __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
       const bool bi = (b >> si) & 1ull, bj = (b >> sj) & 1ull;
       double2 c = make_double2(0.0, 0.0);
       if (valid && bi != bj) {
-        const double2 v = pm_target<LOOK, 0, CE>(A, b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
+        const double2 v = A.look.at<LOOK, 0, CE>(b ^ (1ull << si) ^ (1ull << sj), bad, bad_state);
         c = make_double2(xb.x * v.x - xb.y * v.y, xb.x * v.y + xb.y * v.x);
         if constexpr (JW) {   // pairs are stored with si < sj
           const uint64_t between = ((1ull << sj) - 1) & ~((2ull << si) - 1);
@@ -333,43 +358,39 @@ __global__ void __launch_bounds__(256) k_pm_pairs(const PmArgs A) {
     A.partials[((int64_t)blockIdx.x * C + c) * 2] = s_cls[c];
     A.partials[((int64_t)blockIdx.x * C + c) * 2 + 1] = s_cls[C + c];
   }
-  if (bad && atomicAdd(A.status, bad) == 0) A.status[1] = bad_state;
+  report_bad(A.look.status, bad, bad_state);
 }
 
 constexpr size_t kPmSmem = 96 * 1024;   // shared memory of one CTA: two CTAs per SM
 constexpr int kPmThreads = 256;
 
 // f(kernel) for the walk the basis asks for: k_pm_pairs<LOOK, CE, JW> without permutations, else k_pm_rows<LOOK, TK,
-// CE, CPLX> (TK only with trivial characters).  The class sums are complex (CPLX) with complex vectors or characters;
-// PM_TABLE runs on trivial characters only, so there CPLX == CE.  JW (fermionic bases) only with PM_NONE.
+// CE, CPLX>.  The class sums are complex (CPLX) with complex vectors or characters; LOOK_TABLE runs on trivial
+// characters only, so there CPLX == CE.  JW (fermionic bases) only with LOOK_NONE.
 template <typename F>
 void with_pm_kernel(int look, int tk, bool ce, bool cplx, bool jw, F &&f) {
-  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
-    with_bool(ce, [&](auto e) {
-      if constexpr (lk() == PM_NONE) {
-        with_bool(jw, [&](auto j) { f(k_pm_pairs<PM_NONE, e(), j()>); });
-      } else if (jw) {
-        throw std::logic_error("k_pm_pairs has Jordan-Wigner builds only without symmetries");
-      } else if constexpr (lk() == PM_INVERSION) {
-        f(k_pm_pairs<lk(), e(), false>);
-      } else {
-        with_bool(cplx, [&](auto cx) {
-          with_choice<6, 4, 0>(tk, [&](auto t) {
-            if constexpr (lk() == PM_TABLE ? cx() == e() : cx() || !e()) f(k_pm_rows<lk(), t(), e(), cx()>);
-            else throw std::logic_error("k_pm_rows has no build for these sums");
-          });
-        });
-      }
-    });
+  with_lookup("k_pm_rows", look, tk, ce, [&](auto lk, auto t, auto e) {
+    if (jw && lk() != LOOK_NONE) throw std::logic_error("k_pm_pairs has Jordan-Wigner builds only without symmetries");
+    if constexpr (lk() == LOOK_NONE) {
+      with_bool(jw, [&](auto j) { f(k_pm_pairs<LOOK_NONE, e(), j()>); });
+    } else if constexpr (lk() == LOOK_INVERSION) {
+      f(k_pm_pairs<LOOK_INVERSION, e(), false>);
+    } else {
+      with_bool(cplx, [&](auto cx) {
+        if constexpr (lk() == LOOK_TABLE ? cx() == e() : cx() || !e()) f(k_pm_rows<lk(), t(), e(), cx()>);
+        else throw std::logic_error("k_pm_rows has no build for these sums");
+      });
+    }
   });
 }
 
 // ---- one-site operators between two bases (dmv_apply_spin).  Row r of the target basis is
 //     y_r = 1 / n_t(r) sum_k K_k <r| o_k |psi>,   psi = B_s x,
 // with o_k = σ⁺_k on the set bits of r and σ⁻_k on its clear bits (the source state r ^ (1 << k)), or the diagonal
-// factor sum_k K_k s_k(r) (σᶻ) or sum_k K_k (1).  pm_target gives psi at any state of the source's sector: chi (n x)[rep]
-// with the orbit minimum and character of the source (PM_GROUP, PM_TABLE), x[index] without a group (PM_NONE), chi
-// x[index] with spin inversion alone, whose norm sqrt(1/2) is src_scale.  The host forms K (spin_weights below).
+// factor sum_k K_k s_k(r) (σᶻ) or sum_k K_k (1).  StateLookup::at gives psi at any state of the source's sector: chi
+// (n x)[rep] with the orbit minimum and character of the source (LOOK_GROUP, LOOK_TABLE), x[index] without a group
+// (LOOK_NONE), chi x[index] with spin inversion alone, whose norm sqrt(1/2) is src_scale.  The host forms K
+// (spin_weights below).
 enum SpinWalk {
   SPIN_SELF = 0,    // σᶻ / 1: the row's own state, times c0 + sum over its set bits of k_set + over its clear bits of k_clear
   SPIN_CLEAR = 1,   // σ⁻: the clear bits of the row (k_clear)
@@ -378,30 +399,32 @@ enum SpinWalk {
 };
 
 struct SpinArgs {
-  PmArgs src;                 // the source's look-up; its rows / classes are unused
+  StateLookup src;            // the source's look-up
   const uint64_t *rows;       // this rank's rows of the target basis and their norms (null: row_norm for every row)
   const double *row_norms;
   double row_norm, src_scale;
   const double *k;            // [2][N] complex: k_set, then k_clear
   double2 c0;
+  uint64_t walk_mask;         // SPIN_SET / SPIN_CLEAR / SPIN_BOTH: the sites (modes) the walk visits
   uint64_t diag_mask;         // SPIN_SELF: the sites whose k_set / k_clear enter the row factor (0 for the identity)
   int64_t n_rows;
+  int n_sites;
   double *y;
 };
 
 // One lane owns one row of the target basis and walks its sites; one store of y per row, no atomics.
-// JW (dmv_apply_fermion, PM_NONE with SPIN_SET / SPIN_CLEAR only): the walk is c†_k on the set bits or c_k on the clear
-// bits of the row, each term with the Jordan-Wigner sign (-1)^popc(r & ((1 << k) - 1)); src.site_mask holds the modes
+// JW (dmv_apply_fermion, LOOK_NONE with SPIN_SET / SPIN_CLEAR only): the walk is c†_k on the set bits or c_k on the
+// clear bits of the row, each term with the Jordan-Wigner sign (-1)^popc(r & ((1 << k) - 1)); walk_mask holds the modes
 // the walk visits (one spin half of a spinful basis).
 template <int LOOK, int TK, int WALK, bool CE, bool JW>
 __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
   __shared__ double2 s_k[128];   // k_set [0, N), k_clear [N, 2 N)
-  const int N = A.src.n_sites;
+  const int N = A.n_sites;
   for (int t = threadIdx.x; t < 2 * N; t += blockDim.x) s_k[t] = __ldg(reinterpret_cast<const double2 *>(A.k) + t);
   __syncthreads();
   unsigned long long bad = 0;
   uint64_t bad_state = 0;
-  const uint64_t mask = A.src.site_mask;
+  const uint64_t mask = A.walk_mask;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < A.n_rows; i += (int64_t)gridDim.x * blockDim.x) {
     const uint64_t r = __ldg(A.rows + i);
     double2 acc = make_double2(0.0, 0.0);
@@ -424,48 +447,40 @@ __global__ void __launch_bounds__(256, 2) k_spin_rows(const SpinArgs A) {
         const double2 k = s_k[N + __ffsll((long long)m) - 1];
         c.x += k.x; c.y += k.y;
       }
-      add(c, pm_target<LOOK, TK, CE>(A.src, r, bad, bad_state));
+      add(c, A.src.at<LOOK, TK, CE>(r, bad, bad_state));
     } else {
       if constexpr (WALK & SPIN_SET)
         for (uint64_t m = r & mask; m; m &= m - 1) {
           const int k = __ffsll((long long)m) - 1;
-          add(string_sign(s_k[k], k), pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+          add(string_sign(s_k[k], k), A.src.at<LOOK, TK, CE>(r ^ (1ull << k), bad, bad_state));
         }
       if constexpr (WALK & SPIN_CLEAR)
         for (uint64_t m = ~r & mask; m; m &= m - 1) {
           const int k = __ffsll((long long)m) - 1;
-          add(string_sign(s_k[N + k], k), pm_target<LOOK, TK, CE>(A.src, r ^ (1ull << k), bad, bad_state));
+          add(string_sign(s_k[N + k], k), A.src.at<LOOK, TK, CE>(r ^ (1ull << k), bad, bad_state));
         }
     }
     const double s = A.src_scale / (A.row_norms ? __ldg(A.row_norms + i) : A.row_norm);
     if constexpr (CE) reinterpret_cast<double2 *>(A.y)[i] = make_double2(acc.x * s, acc.y * s);
     else A.y[i] = acc.x * s;
   }
-  if (bad && atomicAdd(A.src.status, bad) == 0) A.src.status[1] = bad_state;
+  report_bad(A.src.status, bad, bad_state);
 }
 
 constexpr int kSpinThreads = 256;
 
-// f(k_spin_rows<LOOK, TK, WALK, CE, JW>); TK (the square-torus orbit minimum) only for the orbit look-ups, JW only for
-// PM_NONE with the set-bit or clear-bit walk
+// f(k_spin_rows<LOOK, TK, WALK, CE, JW>); JW only for LOOK_NONE with the set-bit or clear-bit walk
 template <typename F>
 void with_spin_kernel(int look, int tk, int walk, bool ce, bool jw, F &&f) {
-  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
+  with_lookup("k_spin_rows", look, tk, ce, [&](auto lk, auto t, auto e) {
     with_choice<SPIN_SELF, SPIN_CLEAR, SPIN_SET, SPIN_BOTH>(walk, [&](auto wk) {
-      with_bool(ce, [&](auto e) {
-        with_choice<6, 4, 0>(tk, [&](auto t) {
-          if constexpr (lk() == PM_NONE && t() == 0 && (wk() == SPIN_SET || wk() == SPIN_CLEAR)) {
-            with_bool(jw, [&](auto j) { f(k_spin_rows<lk(), t(), wk(), e(), j()>); });
-          } else if (jw) {
-            throw std::logic_error("k_spin_rows has Jordan-Wigner builds only for the set-bit and clear-bit walks "
-                                   "without symmetries");
-          } else if constexpr (lk() >= PM_GROUP || t() == 0) {
-            f(k_spin_rows<lk(), t(), wk(), e(), false>);
-          } else {
-            throw std::logic_error("k_spin_rows has no square-torus build without a group");
-          }
-        });
-      });
+      if constexpr (lk() == LOOK_NONE && (wk() == SPIN_SET || wk() == SPIN_CLEAR))
+        with_bool(jw, [&](auto j) { f(k_spin_rows<lk(), t(), wk(), e(), j()>); });
+      else if (jw)
+        throw std::logic_error("k_spin_rows has Jordan-Wigner builds only for the set-bit and clear-bit walks "
+                               "without symmetries");
+      else
+        f(k_spin_rows<lk(), t(), wk(), e(), false>);
     });
   });
 }
@@ -476,7 +491,7 @@ void with_spin_kernel(int look, int tk, int walk, bool ce, bool jw, F &&f) {
 // chunk, row-major with `ld` columns (zeros past the chunk's last column), and k_rdm_gram adds Ψ Ψᴴ on the FP64 tensor
 // cores.
 struct RdmArgs {
-  PmArgs src;                  // the look-up of dmv_apply_spin; its rows / classes are unused
+  StateLookup src;             // the basis's look-up
   const uint64_t *embed_a;     // [d]: the states of A's rows, deposited on A's sites
   const uint64_t *binom;       // [64][65]: C(n, k) (B's columns at a fixed weight)
   uint64_t sites_b[64];        // site of bit j of a B configuration, as a one-bit mask
@@ -517,27 +532,19 @@ __global__ void __launch_bounds__(256, 2) k_rdm_fill(const RdmArgs A) {
     const uint64_t b = live ? rdm_column_state(A, (uint64_t)(A.col0 + c)) : 0;
     for (int a = a0; a < a1; ++a) {
       double2 v = make_double2(0.0, 0.0);
-      if (live) v = pm_target<LOOK, TK, CE>(A.src, __ldg(A.embed_a + a) | b, bad, bad_state);
+      if (live) v = A.src.at<LOOK, TK, CE>(__ldg(A.embed_a + a) | b, bad, bad_state);
       if constexpr (CE) reinterpret_cast<double2 *>(A.psi)[a * A.ld + c] = make_double2(v.x * A.scale, v.y * A.scale);
       else A.psi[a * A.ld + c] = v.x * A.scale;
     }
   }
-  if (bad && atomicAdd(A.src.status, bad) == 0) A.src.status[1] = bad_state;
+  report_bad(A.src.status, bad, bad_state);
 }
 
 constexpr int kRdmThreads = 256;
 
-// f(k_rdm_fill<LOOK, TK, CE>); TK (the square-torus orbit minimum) only for the orbit look-ups
 template <typename F>
 void with_rdm_fill(int look, int tk, bool ce, F &&f) {
-  with_choice<PM_NONE, PM_INVERSION, PM_GROUP, PM_TABLE>(look, [&](auto lk) {
-    with_bool(ce, [&](auto e) {
-      with_choice<6, 4, 0>(tk, [&](auto t) {
-        if constexpr (lk() >= PM_GROUP || t() == 0) f(k_rdm_fill<lk(), t(), e()>);
-        else throw std::logic_error("k_rdm_fill has no square-torus build without a group");
-      });
-    });
-  });
+  with_lookup("k_rdm_fill", look, tk, ce, [&](auto lk, auto t, auto e) { f(k_rdm_fill<lk(), t(), e()>); });
 }
 
 // Block tiles of 32 x 32 of ρ: a CTA per tile on or above the diagonal (I <= J) and per slice of the chunk's columns.
@@ -803,7 +810,7 @@ void pm_finish(int N, const PmClasses &K, const double *sums, double W, const do
 // sums[2 c + {0, 1}] = class sum c of the vector A.x over this rank's rows (classes < count).  The lane-major walk runs
 // once per group of classes whose slots fit in shared memory.  jw: the Jordan-Wigner walk of fermionic bases.
 void pm_sums(SolverRun &run, PmArgs A, int count, int look, int tk, bool cplx, bool jw, double *sums) {
-  const bool pairs = look <= PM_INVERSION;
+  const bool pairs = look <= LOOK_INVERSION;
   const int per_pass = pairs ? count : (int)(kPmSmem / ((size_t)kPmThreads * (cplx ? 16 : 8)));
   for (int c0 = 0; c0 < count; c0 += per_pass) {
     A.c_lo = c0;
@@ -1056,6 +1063,59 @@ int64_t rdm_chunk_cols(int d, uint64_t K) {
   return std::min<int64_t>(by_size, (int64_t)((K + 31) / 32 * 32));
 }
 
+// The look-up of the observables in the basis of `ctx`: on several ranks in its whole-basis twin (the replicated-x form)
+// against the gathered x.  The build follows the product's: k_rows' table where k_rows looks up with it, the square-torus
+// orbit minimum where k_rows takes it.  whose ("" or "source's "): for the refusal on several ranks.
+struct ObservableLookup {
+  dmv_context *ctx, *basis;   // the context searched, and where its states are looked up (ctx or its twin)
+  int elt, look, tk;
+  cudaStream_t st;
+  StateLookup dev{};          // everything but x
+
+  ObservableLookup(dmv_context *c, int elt_, cudaStream_t st_, const char *entry, const char *whose = "")
+      : ctx(c), basis(c), elt(elt_), st(st_) {
+    const bool several = ctx->num_ranks > 1;
+    if (several) {
+      if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
+      if (!ctx->replicated)
+        throw std::runtime_error(std::string(entry) + " on several ranks needs the " + whose + "whole basis on every "
+                                 "rank (the replicated-x form), and it is switched off by the exchange / mode options "
+                                 "or does not fit in device memory");
+      basis = ctx->global;
+    }
+    const bool trivial = ctx->proj != PROJ_GROUP || ctx->orbit.trivial_characters;
+    look = ctx->proj == PROJ_NONE        ? LOOK_NONE
+           : ctx->proj == PROJ_INVERSION ? LOOK_INVERSION
+           : (use_rows(basis) && basis->opt.rows_index != 1) ? LOOK_TABLE
+                                                             : LOOK_GROUP;
+    tk = look >= LOOK_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1, basis->opt.rows_ctas)
+                                       : 0;
+    dev.index = base_params(basis).index;
+    dev.orbit = basis->orbit;
+    dev.norms = basis->d_norms.ptr;
+    dev.pos = several ? ctx->d_pos.ptr : nullptr;
+    dev.site_mask = ctx->site_mask;
+    dev.inversion_character = (double)ctx->spin_inversion;
+    dev.status = ctx->d_status.ptr;
+    if (look == LOOK_TABLE) {   // k_rows' table over `basis`, its values refilled per vector (as every product does)
+      ensure_table(basis, elt, st);
+      dev.table = basis->d_table.ptr;
+      dev.table_slots = basis->table_slots;
+      dev.table_dir = basis->table_dir;
+      dev.dord = basis->dord;
+      dev.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
+    }
+  }
+
+  // the look-up of xv, a vector of this rank's states: gathered from every rank on several, the table refilled from it
+  StateLookup vector(const double *xv) const {
+    StateLookup L = dev;
+    L.x = ctx->num_ranks > 1 ? gather_x(ctx, elt, xv) : xv;
+    if (look == LOOK_TABLE) fill_table(basis, elt, L.x, L.pos, st);
+    return L;
+  }
+};
+
 // The walk of dmv_pm_correlations (spin bases: <σ⁺ᵢσ⁻ⱼ>) and dmv_one_body_density_matrix (fermionic bases: <c†ᵢcⱼ>,
 // with the Jordan-Wigner sign).  A spinful basis fixes number_up, so a pair with one mode in each spin half leaves the
 // basis: such pairs are not walked, and their entries stay exactly 0.  entry / out_name: for the messages.
@@ -1065,30 +1125,15 @@ void pair_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
   if (!pm) throw std::runtime_error(std::string(out_name) + " must not be null");
-  const int N = ctx->n_sites, P = run.P;
+  const int N = ctx->n_sites;
   const bool jw = ctx->particle_type != DMV_SPIN;
   const ZzGroup G = zz_group(N, ctx->has_permutations, ctx->k_group_order, ctx->k_perms.data(), ctx->k_flips.data(),
                              ctx->spin_inversion);
   const PmClasses K = pm_classes(N, G);
   const int count = (int)K.size.size();
   cudaStream_t st = run.st;
-  dmv_context *basis = ctx;   // where the targets are looked up
-  if (P > 1) {
-    if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
-    if (!ctx->replicated)
-      throw std::runtime_error(std::string(entry) + " on several ranks needs the whole basis on every rank (the "
-                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
-                               "fit in device memory");
-    basis = ctx->global;
-  }
-  const bool trivial = ctx->proj != PROJ_GROUP || ctx->orbit.trivial_characters;
-  const int look = ctx->proj == PROJ_NONE        ? PM_NONE
-                   : ctx->proj == PROJ_INVERSION ? PM_INVERSION
-                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
-                                                                     : PM_GROUP;
-  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
-                                                            basis->opt.rows_ctas) : 0;
-  const bool cplx = run.ce || !trivial;
+  const ObservableLookup lookup(ctx, elt, st, entry);
+  const bool cplx = run.ce || (ctx->proj == PROJ_GROUP && !ctx->orbit.trivial_characters);
   std::vector<int16_t> class_of(K.of.begin(), K.of.end());
   std::vector<uint16_t> pairs;
   for (int i = 0; i < N; ++i)
@@ -1099,32 +1144,14 @@ void pair_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x
   d_class_of.upload(class_of, st);
   d_pairs.upload(pairs, st);
   PmArgs A{};
-  A.index = base_params(basis).index;
-  A.orbit = basis->orbit;
-  A.norms = basis->d_norms.ptr;
-  A.pos = P > 1 ? ctx->d_pos.ptr : nullptr;
   A.rows = ctx->d_reps.ptr;
   A.row_norms = ctx->d_norms.ptr;
   A.n_rows = run.n;
-  A.x_row_offset = P > 1 ? (int64_t)ctx->rank * ctx->repl_block : 0;
-  A.site_mask = ctx->site_mask;
-  A.inversion_character = (double)ctx->spin_inversion;
+  A.x_row_offset = run.P > 1 ? (int64_t)ctx->rank * ctx->repl_block : 0;
   A.class_of = d_class_of.ptr;
   A.pairs = d_pairs.ptr;
   A.n_sites = N;
   A.n_pairs = (int)pairs.size();
-  A.status = ctx->d_status.ptr;
-  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
-    cudaStream_t keep = basis->stream;
-    basis->stream = st;
-    ensure_table(basis, elt);
-    basis->stream = keep;
-    A.table = basis->d_table.ptr;
-    A.table_slots = basis->table_slots;
-    A.table_dir = basis->table_dir;
-    A.dord = basis->dord;
-    A.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
-  }
   const size_t gram_size = zz_gram_size(N);
   double *d_gram = run.scalars(gram_size + 2 * (size_t)count), *d_sums = d_gram + gram_size;
   const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
@@ -1132,11 +1159,8 @@ void pair_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x
   for (int v = 0; v < num_vectors; ++v) {
     const double *xv = xin.ptr + (size_t)v * run.words;
     const double W = zz_moments(run, G, xv, run.partials(zz_gram_partials(run.n, N)), d_gram, C.data(), m.data());
-    A.x = P > 1 ? gather_x(ctx, elt, xv) : xv;
-    if (look == PM_TABLE)
-      launch_table_fill(basis->n_states, run.ce, A.x, basis->d_norms.ptr, A.pos, basis->d_slot_of.ptr,
-                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
-    pm_sums(run, A, count, look, tk, cplx, jw, d_sums);
+    A.look = lookup.vector(xv);
+    pm_sums(run, A, count, lookup.look, lookup.tk, cplx, jw, d_sums);
     run.all_reduce(d_sums, 2 * (size_t)count);
     CUDA_CHECK(cudaMemcpyAsync(sums.data(), d_sums, sums.size() * sizeof(double), cudaMemcpyDeviceToHost, st));
     check_status(ctx);   // synchronises
@@ -1146,73 +1170,53 @@ void pair_correlations(dmv_context *ctx, int elt, int num_vectors, const void *x
   CUDA_CHECK(cudaStreamSynchronize(st));
 }
 
+// The entry checks of dmv_apply_spin and dmv_apply_fermion: `require` (spin or fermionic bases) of both contexts, and a
+// target on the source's device with the source's rank and number of ranks.  The run is the source's.
+SolverRun one_site_run(dmv_context *target, dmv_context *source, int elt, const char *entry,
+                       void (*require)(const dmv_context *, const char *)) {
+  if (!target || !source) throw std::runtime_error("target and source must not be null");
+  require(source, entry);
+  require(target, entry);
+  SolverRun run(source, elt, entry, false);
+  require_states(target);
+  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
+  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
+    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  return run;
+}
+
 // The launch half of dmv_apply_spin and dmv_apply_fermion: per vector one k_spin_rows pass over the target's rows of
-// this rank.  walk_mask: the modes the set-bit / clear-bit walks visit; jw: Jordan-Wigner signs (fermionic bases).
-void apply_one_site(SolverRun &run, dmv_context *target, dmv_context *source, int elt, const SpinPlan &S, bool jw,
-                    uint64_t walk_mask, int num_vectors, const void *x, void *y, const char *entry) {
+// this rank, with Jordan-Wigner signs on fermionic bases.  walk_mask: the modes the set-bit / clear-bit walks visit.
+void apply_one_site(SolverRun &run, dmv_context *target, const SpinPlan &S, uint64_t walk_mask, int num_vectors,
+                    const void *x, void *y) {
   if (num_vectors < 1) throw std::runtime_error("num_vectors must be positive");
   if (!x) throw std::runtime_error("x must not be null");
   if (!y) throw std::runtime_error("y must not be null");
-  const int N = source->n_sites, P = run.P;
+  dmv_context *source = run.ctx;
   cudaStream_t st = run.st;
-  dmv_context *basis = source;   // where the source states are looked up
-  if (P > 1) {
-    if (!source->exchange_decided) decide_exchange(source);   // collective: every rank reaches the same decision
-    if (!source->replicated)
-      throw std::runtime_error(std::string(entry) + " on several ranks needs the source's whole basis on every rank (the "
-                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
-                               "fit in device memory");
-    basis = source->global;
-  }
-  const bool trivial = source->proj != PROJ_GROUP || source->orbit.trivial_characters;
-  const int look = source->proj == PROJ_NONE        ? PM_NONE
-                   : source->proj == PROJ_INVERSION ? PM_INVERSION
-                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
-                                                                     : PM_GROUP;
-  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
-                                                            basis->opt.rows_ctas) : 0;
+  const ObservableLookup lookup(source, run.elt, st, run.name, "source's ");
+  const bool jw = source->particle_type != DMV_SPIN;
   DevBuf<double> d_k;
   d_k.upload(S.k, st);
   SpinArgs A{};
-  A.src.index = base_params(basis).index;
-  A.src.orbit = basis->orbit;
-  A.src.norms = basis->d_norms.ptr;
-  A.src.pos = P > 1 ? source->d_pos.ptr : nullptr;
-  A.src.site_mask = walk_mask;
-  A.src.inversion_character = (double)source->spin_inversion;
-  A.src.n_sites = N;
-  A.src.status = source->d_status.ptr;
   A.rows = target->d_reps.ptr;
   A.row_norms = target->proj == PROJ_GROUP ? target->d_norms.ptr : nullptr;
   A.row_norm = target->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
   A.src_scale = source->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
   A.k = d_k.ptr;
   A.c0 = make_double2(S.c0[0], S.c0[1]);
+  A.walk_mask = walk_mask;
   A.diag_mask = S.diag_sites ? source->site_mask : 0;
   A.n_rows = target->n_states;
-  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
-    cudaStream_t keep = basis->stream;
-    basis->stream = st;
-    ensure_table(basis, elt);
-    basis->stream = keep;
-    A.src.table = basis->d_table.ptr;
-    A.src.table_slots = basis->table_slots;
-    A.src.table_dir = basis->table_dir;
-    A.src.dord = basis->dord;
-    A.src.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
-  }
-  const size_t out_words = (size_t)target->n_states * elt;
+  A.n_sites = source->n_sites;
+  const size_t out_words = (size_t)target->n_states * run.elt;
   const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
   OutArg<double> yout(static_cast<double *>(y), (size_t)num_vectors * out_words);
   for (int v = 0; v < num_vectors; ++v) {
-    const double *xv = xin.ptr + (size_t)v * run.words;
-    A.src.x = P > 1 ? gather_x(source, elt, xv) : xv;
+    A.src = lookup.vector(xin.ptr + (size_t)v * run.words);
     A.y = yout.ptr + (size_t)v * out_words;
-    if (look == PM_TABLE)
-      launch_table_fill(basis->n_states, run.ce, A.src.x, basis->d_norms.ptr, A.src.pos, basis->d_slot_of.ptr,
-                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
     if (A.n_rows > 0)
-      with_spin_kernel(look, tk, S.walk, run.ce, jw, [&](auto kernel) {
+      with_spin_kernel(lookup.look, lookup.tk, S.walk, run.ce, jw, [&](auto kernel) {
         const int grid = one_wave(kernel, (A.n_rows + kSpinThreads - 1) / kSpinThreads, 0, kSpinThreads);
         kernel<<<grid, kSpinThreads, 0, st>>>(A);
         check_launch("k_spin_rows");
@@ -1220,7 +1224,7 @@ void apply_one_site(SolverRun &run, dmv_context *target, dmv_context *source, in
   }
   yout.finish(st);
   check_status(source);   // synchronises
-  }
+}
 
 }  // namespace
 
@@ -1279,16 +1283,9 @@ int dmv_one_body_density_matrix(dmv_context *ctx, int elt, int num_vectors, cons
 int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights, int num_vectors,
                    const void *x, void *y) {
   API_BEGIN
-  if (!target || !source) throw std::runtime_error("target and source must not be null");
-  require_spin(source, "dmv_apply_spin");
-  require_spin(target, "dmv_apply_spin");
-  SolverRun run(source, elt, "dmv_apply_spin", false);
-  require_states(target);
-  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
-  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
-    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  SolverRun run = one_site_run(target, source, elt, "dmv_apply_spin", require_spin);
   const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt, kind, weights);
-  apply_one_site(run, target, source, elt, S, false, source->site_mask, num_vectors, x, y, "dmv_apply_spin");
+  apply_one_site(run, target, S, source->site_mask, num_vectors, x, y);
   API_END
 }
 
@@ -1297,24 +1294,17 @@ int dmv_apply_spin(dmv_context *target, dmv_context *source, int elt, int kind, 
 int dmv_apply_fermion(dmv_context *target, dmv_context *source, int elt, int kind, const double *weights,
                       int num_vectors, const void *x, void *y) {
   API_BEGIN
-  if (!target || !source) throw std::runtime_error("target and source must not be null");
-  require_fermion(source, "dmv_apply_fermion");
-  require_fermion(target, "dmv_apply_fermion");
-  SolverRun run(source, elt, "dmv_apply_fermion", false);
-  require_states(target);
-  if (target->device != source->device) throw std::runtime_error("target and source must be on the same device");
-  if (target->rank != source->rank || target->num_ranks != source->num_ranks)
-    throw std::runtime_error("target and source must have the same rank and number of ranks");
+  SolverRun run = one_site_run(target, source, elt, "dmv_apply_fermion", require_fermion);
   const uint64_t walk_mask = fermion_walk(source, target, kind, weights);
   const SpinPlan S = spin_plan(spin_basis(source), spin_basis(target), elt,
                                kind == DMV_FERMION_CREATE ? DMV_SPIN_PLUS : DMV_SPIN_MINUS, weights);
-  apply_one_site(run, target, source, elt, S, true, walk_mask, num_vectors, x, y, "dmv_apply_fermion");
+  apply_one_site(run, target, S, walk_mask, num_vectors, x, y);
   API_END
 }
 
 // ---- reduced density matrices (DESIGN.md section 3, "dmv_reduced_density_matrix"): per vector and block w of ρ_A, the
 // columns of B are cut into chunks (every P-th chunk on each rank); per chunk one k_rdm_fill pass writes its amplitudes
-// through the look-up of dmv_apply_spin, k_rdm_gram adds Ψ Ψᴴ per slice of columns and k_rdm_reduce adds the slices,
+// through the observables' look-up, k_rdm_gram adds Ψ Ψᴴ per slice of columns and k_rdm_reduce adds the slices,
 // in order, to the block.  The blocks are all-reduced over the ranks, mirrored and divided by <x|x>.
 int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const void *x, int n_a,
                                const int32_t *sites_a, double *rho) {
@@ -1356,15 +1346,7 @@ int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const
                                " bytes are free on the device");
   }
   cudaStream_t st = run.st;
-  dmv_context *basis = ctx;   // where the states are looked up
-  if (P > 1) {
-    if (!ctx->exchange_decided) decide_exchange(ctx);   // collective: every rank reaches the same decision
-    if (!ctx->replicated)
-      throw std::runtime_error("dmv_reduced_density_matrix on several ranks needs the whole basis on every rank (the "
-                               "replicated-x form), and it is switched off by the exchange / mode options or does not "
-                               "fit in device memory");
-    basis = ctx->global;
-  }
+  const ObservableLookup lookup(ctx, elt, st, "dmv_reduced_density_matrix");
   // <x|x> of every vector first: a zero vector is refused before anything is written
   const InArg<double> xin(static_cast<const double *>(x), (size_t)num_vectors * run.words, st);
   double *d_norm2 = run.scalars(2 * (size_t)num_vectors), *q_part = run.partials(quad_partials(1));
@@ -1379,36 +1361,10 @@ int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const
     if (!(norm2[2 * v] > 0.0))
       throw std::runtime_error("x is a zero vector: <x|x> = 0 (vector " + std::to_string(v) + ")");
 
-  const bool trivial = ctx->proj != PROJ_GROUP || ctx->orbit.trivial_characters;
-  const int look = ctx->proj == PROJ_NONE        ? PM_NONE
-                   : ctx->proj == PROJ_INVERSION ? PM_INVERSION
-                   : (use_rows(basis) && basis->opt.rows_index != 1) ? PM_TABLE
-                                                                     : PM_GROUP;
-  const int tk = look >= PM_GROUP && trivial ? rows_torus_k(basis->orbit, basis->opt.rows_index == 1,
-                                                            basis->opt.rows_ctas) : 0;
   RdmArgs A{};
-  A.src.index = base_params(basis).index;
-  A.src.orbit = basis->orbit;
-  A.src.norms = basis->d_norms.ptr;
-  A.src.pos = P > 1 ? ctx->d_pos.ptr : nullptr;
-  A.src.site_mask = ctx->site_mask;
-  A.src.inversion_character = (double)ctx->spin_inversion;
-  A.src.n_sites = N;
-  A.src.status = ctx->d_status.ptr;
   A.scale = ctx->proj == PROJ_INVERSION ? std::sqrt(0.5) : 1.0;
   A.n_b = n_b;
   std::copy(site_b.begin(), site_b.end(), A.sites_b);
-  if (look == PM_TABLE) {   // k_rows' table over `basis`, its values refilled from x below (every product refills it)
-    cudaStream_t keep = basis->stream;
-    basis->stream = st;
-    ensure_table(basis, elt);
-    basis->stream = keep;
-    A.src.table = basis->d_table.ptr;
-    A.src.table_slots = basis->table_slots;
-    A.src.table_dir = basis->table_dir;
-    A.src.dord = basis->dord;
-    A.src.dense = basis->dense_order ? basis->d_dense.ptr : nullptr;
-  }
   std::vector<uint64_t> h_binom(64 * 65);
   for (int n = 0; n < 64; ++n)
     for (int k = 0; k <= 64; ++k) h_binom[n * 65 + k] = binom().c[n][k];
@@ -1425,11 +1381,7 @@ int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const
   OutArg<double> out(rho, (size_t)num_vectors * acc_words);
   int64_t amplitudes = 0, flops = 0;
   for (int v = 0; v < num_vectors; ++v) {
-    const double *xv = xin.ptr + (size_t)v * run.words;
-    A.src.x = P > 1 ? gather_x(ctx, elt, xv) : xv;
-    if (look == PM_TABLE)
-      launch_table_fill(basis->n_states, run.ce, A.src.x, basis->d_norms.ptr, A.src.pos, basis->d_slot_of.ptr,
-                        basis->d_reps.ptr, basis->d_table.ptr, basis->dense_order ? basis->d_dense.ptr : nullptr, st);
+    A.src = lookup.vector(xin.ptr + (size_t)v * run.words);
     CUDA_CHECK(cudaMemsetAsync(d_acc.ptr, 0, acc_words * sizeof(double), st));
     size_t off = 0;
     for (size_t bi = 0; bi < L.dims.size(); ++bi) {
@@ -1446,7 +1398,7 @@ int dmv_reduced_density_matrix(dmv_context *ctx, int elt, int num_vectors, const
       for (uint64_t c = P > 1 ? (uint64_t)ctx->rank : 0; c < n_chunks; c += P) {   // every P-th chunk
         A.col0 = (int64_t)(c * ld);
         A.cols = (int64_t)std::min<uint64_t>(ld, K - c * ld);
-        with_rdm_fill(look, tk, run.ce, [&](auto kernel) {
+        with_rdm_fill(lookup.look, lookup.tk, run.ce, [&](auto kernel) {
           const int64_t work = (d + kRdmRowGroup - 1) / kRdmRowGroup * ld;
           kernel<<<one_wave(kernel, (work + kRdmThreads - 1) / kRdmThreads, 0, kRdmThreads), kRdmThreads, 0, st>>>(A);
           check_launch("k_rdm_fill");

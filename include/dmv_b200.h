@@ -428,8 +428,9 @@ int dmv_apply_fermion(dmv_context *target, dmv_context *source, int elt, int kin
  * copy do not fit in free device memory (the message names the bytes).
  * Method: per block, the columns b of B (combinadic order at a fixed weight) are cut into chunks of at most 2^24
  * amplitudes, a function of (N, W, A) alone.  k_rdm_fill writes Ψ[a, c] = ψ(embed_A(a) | embed_B(b_c)) of a chunk through
- * the orbit minimum and look-up of dmv_apply_spin; k_rdm_gram adds Ψ Ψᴴ on the FP64 tensor cores (tiles of 32 x 32 on or
- * above the diagonal, a fixed number of column slices summed in order, chunks added in order).  No floating-point
+ * the orbit minimum and look-up the observables share (dmv_pm_correlations, dmv_apply_spin); k_rdm_gram adds Ψ Ψᴴ on
+ * the FP64 tensor cores (tiles of 32 x 32 on or above the diagonal, a fixed number of column slices summed in order,
+ * chunks added in order).  No floating-point
  * atomics: a repeated call is bit-identical.  Collective when num_ranks > 1 (needs dmv_comm_init and the whole basis on
  * every rank, as dmv_apply_spin): rank r takes chunks r, r + P, ...; the blocks are summed over the ranks and every rank
  * returns the same ρ.  dmv_get_info: "rdm_amplitudes" (amplitudes this rank filled in the last call) and
