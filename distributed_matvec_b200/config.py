@@ -15,7 +15,13 @@ plus the basis' particle type (``ls_hs_basis.particle_type``, reference src/FFI.
 A spinless-fermion basis has ``number_sites`` bits, bit i the occupation of site i; with ``number_particles`` it is the
 fixed-weight basis.  A spinful-fermion basis of N = ``number_sites`` <= 32 sites has 2N bits: bit i is the up occupation
 of site i and bit N + i its down occupation, so a state is ``(down << N) | up``; ``number_particles`` and ``number_up``
-are both required.  Fermionic bases take no symmetries, spin inversion or ``hamming_weight``.
+are both required.  Fermionic bases take no spin inversion or ``hamming_weight``, and no spin ``symmetries`` (one
+entry per bit, no exchange sign); their lattice symmetries are
+
+    basis: {site_symmetries: [{permutation, sector}]}
+
+with permutations of the ``number_sites`` sites.  A spinful permutation acts on both spin halves alike.  The state
+|s> = c†_{a1} ... c†_{ak} |0> (a1 < ... < ak) goes to sign(g, s) |g(s)>, the sign of the exchanges (DESIGN.md §3).
 """
 from __future__ import annotations
 
@@ -26,7 +32,7 @@ import numpy as np
 import yaml
 
 from .expr import FermionModes, TermTable, compile_terms, max_number_off_diag
-from .symmetry import SymmetryGroup, build_group
+from .symmetry import SymmetryGroup, build_group, widen_to_spinful
 
 
 SPIN, SPINLESS_FERMION, SPINFUL_FERMION = "spin-1/2", "spinless-fermion", "spinful-fermion"
@@ -75,8 +81,11 @@ class BasisSpec:
 
     @property
     def group(self) -> SymmetryGroup:
+        """The group with one permutation entry per bit: a spinful site permutation p is widened to p[N + i] = N + p[i]."""
         if self._group is None:
             self._group = build_group(self.number_sites, self.generators, self.spin_inversion)
+            if self.particle_type == SPINFUL_FERMION:
+                self._group = widen_to_spinful(self._group)
         return self._group
 
     def min_state_estimate(self) -> int:
@@ -113,8 +122,9 @@ class BasisSpec:
         return comb(n, w) if w is not None else 1 << n
 
     def number_states(self) -> int | None:
-        """Dimension of a fermionic or symmetry-free basis: C(N, N_up) C(N, N_down) for spinful fermions."""
-        if self.particle_type == SPINFUL_FERMION:
+        """Dimension of a symmetry-free basis: C(N, N_up) C(N, N_down) for spinful fermions.  None for a projected
+        basis: its dimension comes from enumeration."""
+        if self.particle_type == SPINFUL_FERMION and not self.requires_projection():
             return comb(self.number_sites, self.number_up) * comb(self.number_sites, self.hamming_weight - self.number_up)
         if self.requires_projection():
             return None
@@ -139,14 +149,27 @@ class OperatorSpec:
         return self.off_diag.is_real() and self.diag.is_real()
 
 
+def _generators(entries) -> list[dict]:
+    return [{"permutation": [int(v) for v in g["permutation"]], "sector": int(g.get("sector", 0))}
+            for g in (entries or [])]
+
+
 def _fermion_basis_from_dict(d: dict, particle: str) -> BasisSpec:
-    for key in ("symmetries", "spin_inversion", "hamming_weight", "number_spins"):
+    if d.get("symmetries") is not None:
+        raise ValueError(f"{particle} basis: 'symmetries' is not supported: it lists spin permutations, one entry per "
+                         "bit, without the fermionic exchange sign; give permutations of the sites as 'site_symmetries'")
+    for key in ("spin_inversion", "hamming_weight", "number_spins"):
         if d.get(key) is not None:
             raise ValueError(f"{particle} basis: '{key}' is not supported (fermionic bases take number_sites, "
-                             "number_particles and, for spinful fermions, number_up)")
+                             "number_particles, site_symmetries and, for spinful fermions, number_up)")
     if "number_sites" not in d:
         raise ValueError(f"{particle} basis needs number_sites")
     n = int(d["number_sites"])
+    gens = _generators(d.get("site_symmetries"))
+    for g in gens:
+        if sorted(g["permutation"]) != list(range(n)):
+            raise ValueError(f"{particle} basis: site_symmetries need permutations of the {n} sites "
+                             f"(got {g['permutation']})")
     np_, nu = d.get("number_particles"), d.get("number_up")
     if particle == SPINLESS_FERMION:
         if not 0 < n <= 64:
@@ -156,7 +179,7 @@ def _fermion_basis_from_dict(d: dict, particle: str) -> BasisSpec:
         if np_ is not None and not 0 <= int(np_) <= n:
             raise ValueError(f"spinless-fermion basis: number_particles must be between 0 and {n} (got {np_})")
         w = None if np_ is None else int(np_)
-        return BasisSpec(number_sites=n, hamming_weight=w, spin_inversion=0, particle_type=particle,
+        return BasisSpec(number_sites=n, hamming_weight=w, spin_inversion=0, generators=gens, particle_type=particle,
                          number_particles=w)
     if not 0 < n <= 32:
         raise ValueError(f"spinful-fermion basis: number_sites must be between 1 and 32 (got {n})")
@@ -166,7 +189,7 @@ def _fermion_basis_from_dict(d: dict, particle: str) -> BasisSpec:
     if not (0 <= nu <= n and 0 <= np_ - nu <= n):
         raise ValueError(f"spinful-fermion basis: need 0 <= number_up <= {n} and 0 <= number_particles - number_up <= "
                          f"{n} (got number_particles {np_}, number_up {nu})")
-    return BasisSpec(number_sites=n, hamming_weight=np_, spin_inversion=0, particle_type=particle,
+    return BasisSpec(number_sites=n, hamming_weight=np_, spin_inversion=0, generators=gens, particle_type=particle,
                      number_particles=np_, number_up=nu)
 
 
@@ -176,6 +199,8 @@ def basis_from_dict(d: dict) -> BasisSpec:
         raise ValueError(f"unknown particle type {particle!r}: expected one of {', '.join(PARTICLE_TYPES)}")
     if particle != SPIN:
         return _fermion_basis_from_dict(d, particle)
+    if d.get("site_symmetries") is not None:
+        raise ValueError("spin-1/2 basis: 'site_symmetries' is for fermionic bases; spin bases take 'symmetries'")
     n = int(d["number_spins"])
     if not 0 < n <= 64:
         raise ValueError("bases with more than 64 bits are not yet implemented")  # DMV:1099-1100
@@ -185,8 +210,7 @@ def basis_from_dict(d: dict) -> BasisSpec:
         number_sites=n,
         hamming_weight=None if hw is None else int(hw),
         spin_inversion=0 if inv is None else int(inv),
-        generators=[{"permutation": [int(v) for v in g["permutation"]], "sector": int(g.get("sector", 0))}
-                    for g in (d.get("symmetries") or [])],
+        generators=_generators(d.get("symmetries")),
     )
 
 

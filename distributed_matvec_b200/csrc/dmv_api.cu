@@ -1105,6 +1105,9 @@ void require_fermion(const dmv_context *ctx, const char *entry) {
   if (ctx && ctx->particle_type == DMV_SPIN)
     throw std::runtime_error(std::string(entry) + ": not defined on a spin-1/2 basis (it applies fermionic operators "
                              "with Jordan-Wigner strings)");
+  if (ctx && ctx->proj == PROJ_GROUP)
+    throw std::runtime_error(std::string(entry) + ": not defined on a projected " + particle_name(ctx->particle_type) +
+                             " basis (site_symmetries): its state look-up carries no fermionic exchange sign");
 }
 
 // the particle numbers of a fermionic basis, checked before anything is allocated
@@ -1115,8 +1118,25 @@ void check_particles(const dmv_basis_desc *basis, const dmv_particles_desc *pt) 
                              std::to_string(type) + ")");
   if (type == DMV_SPIN) return;
   const std::string what = particle_name(type);
-  if (basis->has_permutations || basis->spin_inversion != 0)
+  if (basis->spin_inversion != 0)
     throw std::runtime_error(what + " basis: permutation symmetries and spin inversion are not supported for fermions");
+  if (basis->has_permutations) {   // lattice symmetries: site permutations, no flip; spinful ones act on both halves alike
+    if (basis->group_order <= 0 || !basis->perms || !basis->flips || !basis->characters)
+      throw std::runtime_error(what + " basis: permutation symmetries need the group tables (group_order, perms, flips "
+                               "and characters)");
+    const int N = bits / 2;
+    for (int64_t g = 0; g < basis->group_order; ++g) {
+      if (basis->flips[g] != 0)
+        throw std::runtime_error(what + " basis: group element " + std::to_string(g) +
+                                 " has a spin flip; fermionic bases take permutations only");
+      const int32_t *p = basis->perms + g * bits;
+      if (type == DMV_SPINFUL_FERMION && bits % 2 == 0)
+        for (int i = 0; i < N; ++i)
+          if (p[i] < 0 || p[i] >= N || p[N + i] != N + p[i])
+            throw std::runtime_error(what + " basis: group element " + std::to_string(g) + " is not one site "
+                                     "permutation acting on both spin halves (need p[N + i] = N + p[i] with p[i] < N)");
+    }
+  }
   if (basis->hamming_weight != pt->number_particles)
     throw std::runtime_error(what + " basis: hamming_weight (" + std::to_string(basis->hamming_weight) +
                              ") must equal number_particles (" + std::to_string(pt->number_particles) + ")");
@@ -1256,9 +1276,9 @@ int dmv_context_create_particles(const dmv_basis_desc *basis, const dmv_particle
     if (basis->group_order <= 0 || !basis->perms || !basis->flips || !basis->characters)
       throw std::runtime_error("basis with permutation symmetries needs the group tables");
     ctx->host_orbit = compile_orbit_program(basis->number_sites, basis->group_order, basis->perms,
-                                            basis->flips, basis->characters);
+                                            basis->flips, basis->characters, ctx->particle_type != DMV_SPIN);
     for (double v : ctx->host_orbit.characters) (void)v;
-    for (size_t e = 0; e < ctx->host_orbit.characters.size(); e += 2)
+    for (size_t e = 0; e < (size_t)ctx->host_orbit.n_q * ctx->host_orbit.n_t * 4; e += 2)   // (not the inversion masks)
       if (ctx->host_orbit.characters[e + 1] != 0.0) cplx = true;
     upload_orbit(ctx.get());
   }

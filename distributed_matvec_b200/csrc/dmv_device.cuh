@@ -91,12 +91,20 @@ struct OrbitProgram {
   const int32_t *benes_delta;  // [n_stages]
   const uint64_t *step_mask;   // [n_t-1][n_left + n_right]  (mask in OUTPUT positions)
   const int32_t *step_shift;   // [n_t-1][n_left + n_right]
-  const double2 *characters;   // [n_q][n_t][2]  character of (t_j . q_i, flip); conj NOT applied
+  const double2 *characters;   // [n_q][n_t][2]  character of (t_j . q_i, flip); conj NOT applied; fermionic programs
+                               // continue with the inversion masks (orbit_sign)
   int64_t group_order;         // n_q * n_t * (has_flip ? 2 : 1)
   // fast paths for chains whose every step is one left + one right masked shift (translations):
   //   step_pack32[j] = {mask_left, mask_right, shift_left, shift_right}   (n_sites <= 32: 32-bit arithmetic)
   //   step_pack64[3j..3j+2] = {mask_left, mask_right, shift_left | shift_right << 32}
   int32_t simple;              // 0: general; 1: packed steps are valid
+  // fermionic bases: characters[n_q * n_t * 2 ..] holds, as uint64, per element e = q * n_t + j and bit i the inversion mask
+  //   M_e[i] = { j < i : image(j) > image(i) },   image(j) = the output bit that takes input bit j,
+  // so U_g|s> = sign(g, s)|g(s)> with sign(g, s) = (-1)^(sum over set bits i of s of popc(s & M_e[i])) (orbit_sign).  A
+  // fermionic program never takes the representative-only forms (canon_mode, tor_mode, simple, orbit_representative): they
+  // give no element, so trivial_characters is 0 there.  (The masks share the characters' buffer, so OrbitProgram keeps
+  // its size and the spin builds their code.)
+  int32_t fermionic;
   const uint4 *step_pack32;    // [n_t - 1] or nullptr
   const uint64_t *step_pack64; // [3 (n_t - 1)]
   // canonical form under the chain subgroup WITHOUT walking it, when that subgroup is the group of block rotations
@@ -1079,7 +1087,25 @@ __device__ __forceinline__ uint64_t orbit_representative(const OrbitProgram &P, 
   return orbit_scan<false, false>(P, s).rep;
 }
 
-// Full-precision stabiliser sum  sum_{g : g(s) = s} Re chi(g)  (only needed with non-trivial characters)
+// The fermionic exchange sign of element arg (an OrbitResult::arg) on the state s it is applied to: +1 or -1.  One load and
+// one popcount per set bit of s; evaluated once per term, for the minimising element only.
+__host__ __device__ __forceinline__ double orbit_sign(const OrbitProgram &P, int32_t arg, uint64_t s) {
+  const uint64_t *M = reinterpret_cast<const uint64_t *>(P.characters + (int64_t)P.n_q * P.n_t * 2) +
+                      (int64_t)(arg >> 1) * P.n_sites;
+  uint32_t parity = 0;
+  for (uint64_t b = s; b; b &= b - 1) {
+#ifdef __CUDA_ARCH__
+    parity += (uint32_t)__popcll(s & __ldg(M + (__ffsll((long long)b) - 1)));
+#else
+    parity += (uint32_t)__builtin_popcountll(s & M[__builtin_ctzll(b)]);
+#endif
+  }
+  return (parity & 1u) ? -1.0 : 1.0;
+}
+
+// Full-precision stabiliser sum  sum_{g : g(s) = s} Re chi(g)  (only needed with non-trivial characters); FS (fermionic
+// bases): sum_{g : g(s) = s} Re chi(g) sign(g, s), which vanishes on the orbits that are not basis states
+template <bool FS = false>
 __host__ __device__ inline double orbit_stabiliser_sum(const OrbitProgram &P, uint64_t s) {
   double acc = 0.0;
   const int n_pairs = P.n_left + P.n_right;
@@ -1097,7 +1123,8 @@ __host__ __device__ inline double orbit_stabiliser_sum(const OrbitProgram &P, ui
         cur = nxt;
       }
       const int64_t e = ((int64_t)q * P.n_t + j) * 2;
-      if (cur == s) acc += P.trivial_characters ? 1.0 : P.characters[e].x;
+      if (FS && cur == s) acc += P.characters[e].x * orbit_sign(P, (int32_t)e, s);
+      else if (cur == s) acc += P.trivial_characters ? 1.0 : P.characters[e].x;
       if (P.has_flip && (cur ^ P.site_mask) == s) acc += P.trivial_characters ? 1.0 : P.characters[e + 1].x;
     }
   }

@@ -9,6 +9,7 @@
 #include "dmv_host.h"
 
 #include <algorithm>
+#include <cstring>
 #include <map>
 #include <random>
 #include <set>
@@ -127,7 +128,7 @@ struct Candidate {
 }  // namespace
 
 HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const int32_t *perms,
-                                       const uint8_t *flips, const double *characters) {
+                                       const uint8_t *flips, const double *characters, bool fermionic) {
   HostOrbitProgram H;
   H.n_sites = n_sites;
   H.site_mask = (n_sites == 64) ? ~0ull : ((1ull << n_sites) - 1);
@@ -158,7 +159,8 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
   H.has_flip = any_flip ? 1 : 0;
   bool trivial = true;
   for (auto &kv : chi) trivial &= (kv.second.first == 1.0 && kv.second.second == 0.0);
-  H.trivial_characters = trivial ? 1 : 0;
+  // a fermionic state picks up the exchange sign of the element that maps it, so every scan needs the element
+  H.trivial_characters = trivial && !fermionic ? 1 : 0;
 
   Perm ident(n_sites);
   for (int i = 0; i < n_sites; ++i) ident[i] = i;
@@ -309,7 +311,7 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
   }
   (void)n_pairs;
   // packed steps for the translation-like fast paths (exactly one left and one right shift per step)
-  if (H.n_left == 1 && H.n_right == 1) {
+  if (H.n_left == 1 && H.n_right == 1 && !fermionic) {
     H.simple = 1;
     for (size_t j = 0; j < best.steps.size(); ++j) {
       const uint64_t ml = H.step_mask[2 * j], mr = H.step_mask[2 * j + 1];
@@ -510,6 +512,21 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
       }
     }
   H.group_order = group_order;
+  if (fermionic) {   // inversion masks of every element, in the order of `characters`, behind them (OrbitProgram::fermionic)
+    H.fermionic = 1;
+    std::vector<uint64_t> masks((size_t)H.n_q * H.n_t * n_sites, 0);
+    for (int q = 0; q < H.n_q; ++q)
+      for (int j = 0; j < H.n_t; ++j) {
+        const Perm image = inverse(compose(best.chain[j], best.transversal[q]));   // input bit b goes to output image[b]
+        uint64_t *M = masks.data() + ((size_t)q * H.n_t + j) * n_sites;
+        for (int i = 0; i < n_sites; ++i)
+          for (int b = 0; b < i; ++b)
+            if (image[b] > image[i]) M[i] |= 1ull << b;
+      }
+    const size_t n_chars = H.characters.size();
+    H.characters.resize(n_chars + masks.size());
+    std::memcpy(H.characters.data() + n_chars, masks.data(), masks.size() * sizeof(uint64_t));
+  }
 
   // self-check against bit-by-bit application on random states
   OrbitProgram P = H.view();
@@ -543,6 +560,13 @@ HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const i
     uint64_t y = apply_naive(g, s);
     if (r.arg & 1) y ^= H.site_mask;
     if (y != r.rep) throw std::runtime_error("orbit program argmin self-check failed");
+    if (fermionic) {   // the sign against the inversions of the images of the occupied modes, counted pair by pair
+      const Perm image = inverse(g);
+      int inv = 0;
+      for (int i = 0; i < n_sites; ++i)
+        for (int b = 0; b < i; ++b) inv += ((s >> i) & (s >> b) & 1ull) && image[b] > image[i];
+      if (orbit_sign(P, r.arg, s) != ((inv & 1) ? -1.0 : 1.0)) throw std::runtime_error("orbit program sign self-check failed");
+    }
   }
   return H;
 }
@@ -617,6 +641,7 @@ OrbitProgram HostOrbitProgram::view() const {
   P.tor_frow = tor_frow.data();
   P.tor_net_mask = tor_net_mask.data();
   P.tor_net_delta = tor_net_delta.data();
+  P.fermionic = fermionic;
   return P;
 }
 

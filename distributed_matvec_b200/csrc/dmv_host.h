@@ -22,7 +22,8 @@ struct HostOrbitProgram {
   std::vector<int32_t> benes_delta;
   std::vector<uint64_t> step_mask;
   std::vector<int32_t> step_shift;
-  std::vector<double> characters;  // interleaved, [n_q][n_t][2][2]
+  std::vector<double> characters;  // interleaved, [n_q][n_t][2][2]; fermionic: then the inversion masks' bits, [n_q][n_t][n_sites]
+  int32_t fermionic = 0;
   std::vector<uint32_t> step_pack32;  // 4 words per step (empty unless simple and n_sites <= 32)
   std::vector<uint64_t> step_pack64;  // 3 words per step (empty unless simple)
   int32_t simple = 0;
@@ -43,8 +44,9 @@ struct HostOrbitProgram {
   OrbitProgram view() const;       // pointers into the host vectors
 };
 
+// fermionic: n_sites counts the modes, and every element carries its inversion masks for the exchange sign
 HostOrbitProgram compile_orbit_program(int n_sites, int64_t group_order, const int32_t *perms,
-                                       const uint8_t *flips, const double *characters);
+                                       const uint8_t *flips, const double *characters, bool fermionic = false);
 // the states every orbit form is self-checked on: patterns with many tied images, then 256 seeded random words
 std::vector<uint64_t> orbit_probe_states(uint64_t site_mask);
 // orbit_min_torus_sq_t(s ^ x, transpose(s) ^ transpose(x)) == orbit_min_torus_sq(s ^ x) for every probe state s and

@@ -401,7 +401,8 @@ __device__ __forceinline__ void diagonal(const Tables<CV> &T, int /*n_diag*/, ui
 // route(): projects beta (inversion / full group) and appends the record to the bucket of its owner when
 // that is another rank.  Returns true when the record is this rank's own (to be searched + accumulated).
 // All 32 lanes must call it (warp collectives); `active` lanes carry a record.
-template <int PROJ, bool CV, bool CE, bool COUNT_ONLY>
+// FS (fermionic bases, PROJ_GROUP): the character of the element carries the exchange sign sign(g, beta) (orbit_sign)
+template <int PROJ, bool CV, bool CE, bool COUNT_ONLY, bool FS = false>
 __device__ __forceinline__ bool route(const KernelParams &p, const OrbitProgram &orbit, bool active,
                                       uint64_t &beta, typename ValT<CV>::type &c, unsigned long long &cur) {
   using V = typename ValT<CV>::type;
@@ -416,9 +417,10 @@ __device__ __forceinline__ bool route(const KernelParams &p, const OrbitProgram 
         beta = orbit_representative(orbit, beta);
       } else {
         const OrbitResult r = orbit_scan<false, false>(orbit, beta);
-        beta = r.rep;
         const double2 chi = __ldg(orbit.characters + r.arg);   // state_info returns conj(chi)
         c = v_mul(c, v_make(chi.x, -chi.y, (V *)nullptr));
+        if (FS) c = v_scale(c, orbit_sign(orbit, r.arg, beta));   // fermionic exchange sign
+        beta = r.rep;
       }
     }
   }
@@ -429,7 +431,7 @@ __device__ __forceinline__ bool route(const KernelParams &p, const OrbitProgram 
     if (active && !COUNT_ONLY) {
       if (PROJ == PROJ_GROUP) {   // norm of the representative: BO:200 `norms[k]`
         const double stab = orbit.trivial_characters ? (double)orbit_scan<true, false>(orbit, beta).stab
-                                                     : orbit_stabiliser_sum(orbit, beta);
+                                                     : orbit_stabiliser_sum<FS>(orbit, beta);
         const double nn = stab / (double)orbit.group_order;
         c = v_scale(c, nn > 1e-12 ? sqrt(nn) : 0.0);
       }
@@ -496,7 +498,7 @@ __device__ __forceinline__ bool route(const KernelParams &p, const OrbitProgram 
 }
 
 // finish(): localProcess (reference DMV:73-127) for one located record
-template <int PROJ, bool CV, bool CE>
+template <int PROJ, bool CV, bool CE, bool FS = false>
 __device__ __forceinline__ void finish(const KernelParams &p, const OrbitProgram &orbit, bool active,
                                        uint64_t beta, typename ValT<CV>::type c, int64_t idx) {
   if (!active) return;
@@ -506,7 +508,7 @@ __device__ __forceinline__ void finish(const KernelParams &p, const OrbitProgram
   } else if (v_nonzero(c)) {
     bool fatal = true;
     if (PROJ == PROJ_GROUP && !orbit.trivial_characters)
-      fatal = orbit_stabiliser_sum(orbit, beta) > 1e-12 * (double)orbit.group_order;  // zero-norm orbit
+      fatal = orbit_stabiliser_sum<FS>(orbit, beta) > 1e-12 * (double)orbit.group_order;  // zero-norm orbit
     if (fatal) {                                                             // DMV:115-118
       if (atomicAdd(p.status, 1ull) == 0) p.status[1] = beta;
     }
@@ -549,7 +551,7 @@ __device__ __forceinline__ void locate2(const StateIndex &ix, bool a0, uint64_t 
 }
 
 // Drain up to 64 queued records of this warp: lane handles entries `lane` and `lane + 32`.
-template <int PROJ, bool CV, bool CE, bool COUNT_ONLY>
+template <int PROJ, bool CV, bool CE, bool COUNT_ONLY, bool FS>
 __device__ __forceinline__ void drain(const KernelParams &p, const OrbitProgram &orbit, const StateIndex &index,
                                       const uint64_t *qb, const typename ValT<CV>::type *qc, unsigned head,
                                       unsigned n, unsigned long long &cur) {
@@ -559,19 +561,19 @@ __device__ __forceinline__ void drain(const KernelParams &p, const OrbitProgram 
   bool a0 = lane < n, a1 = lane + 32 < n;
   uint64_t k0 = a0 ? qb[p0] : 0ull, k1 = a1 ? qb[p1] : 0ull;
   V c0 = a0 ? qc[p0] : v_make(0.0, 0.0, (V *)nullptr), c1 = a1 ? qc[p1] : v_make(0.0, 0.0, (V *)nullptr);
-  a0 = route<PROJ, CV, CE, COUNT_ONLY>(p, orbit, a0, k0, c0, cur);
-  if (n > 32) a1 = route<PROJ, CV, CE, COUNT_ONLY>(p, orbit, a1, k1, c1, cur);   // n is warp-uniform
+  a0 = route<PROJ, CV, CE, COUNT_ONLY, FS>(p, orbit, a0, k0, c0, cur);
+  if (n > 32) a1 = route<PROJ, CV, CE, COUNT_ONLY, FS>(p, orbit, a1, k1, c1, cur);   // n is warp-uniform
   else a1 = false;
   if (COUNT_ONLY) return;
   int64_t i0, i1;
   locate2(index, a0, k0, a1, k1, i0, i1);
-  finish<PROJ, CV, CE>(p, orbit, a0, k0, c0, i0);
-  finish<PROJ, CV, CE>(p, orbit, a1, k1, c1, i1);
+  finish<PROJ, CV, CE, FS>(p, orbit, a0, k0, c0, i0);
+  finish<PROJ, CV, CE, FS>(p, orbit, a1, k1, c1, i1);
 }
 
 // (symmetric bases: the orbit scan wants > 100 registers; three resident CTAs per SM hide its latencies better than
 // two, at the price of a few spills outside the scan)
-template <int PROJ, bool CV, bool CE, bool COUNT_ONLY>
+template <int PROJ, bool CV, bool CE, bool COUNT_ONLY, bool FS>
 __global__ void __launch_bounds__(kThreads, PROJ == PROJ_GROUP ? 3 : 1) k_generate(const KernelParams p) {
   using V = typename ValT<CV>::type;
   extern __shared__ __align__(16) unsigned char smem[];
@@ -655,7 +657,7 @@ __global__ void __launch_bounds__(kThreads, PROJ == PROJ_GROUP ? 3 : 1) k_genera
         count += __popc(m);
         if (count >= 64) {
           __syncwarp();
-          drain<PROJ, CV, CE, COUNT_ONLY>(p, T.orbit, T.index, qb, qc, head, 64, cur);
+          drain<PROJ, CV, CE, COUNT_ONLY, FS>(p, T.orbit, T.index, qb, qc, head, 64, cur);
           head = (head + 64) & (kQueue - 1);
           count -= 64;
           __syncwarp();
@@ -665,7 +667,7 @@ __global__ void __launch_bounds__(kThreads, PROJ == PROJ_GROUP ? 3 : 1) k_genera
   }
   if (count > 0) {
     __syncwarp();
-    drain<PROJ, CV, CE, COUNT_ONLY>(p, T.orbit, T.index, qb, qc, head, count, cur);
+    drain<PROJ, CV, CE, COUNT_ONLY, FS>(p, T.orbit, T.index, qb, qc, head, count, cur);
   }
   if (COUNT_ONLY && p.num_ranks <= 32 && (int)lane < p.num_ranks)
     p.warp_counts[gw * p.num_ranks + lane] = cur;
@@ -695,7 +697,7 @@ __device__ __forceinline__ void v_add(double2 &a, double2 b) { a.x += b.x; a.y +
 __device__ __forceinline__ void smem_add(double *p, double v) { atomicAdd(p, v); }
 __device__ __forceinline__ void smem_add(double2 *p, double2 v) { atomicAdd(&p->x, v.x); atomicAdd(&p->y, v.y); }
 
-template <int PROJ, bool CV, bool CE>
+template <int PROJ, bool CV, bool CE, bool FS>
 __global__ void __launch_bounds__(kThreads) k_pull(const KernelParams p) {
   using V = typename ValT<CV>::type;
   using E = typename ValT<CE>::type;
@@ -736,6 +738,7 @@ __global__ void __launch_bounds__(kThreads) k_pull(const KernelParams p) {
         r = orbit_scan<false, false>(orbit, raw);
         const double2 chi = __ldg(orbit.characters + r.arg);   // chi(g), not conjugated (see header)
         h = v_mul(h, v_make(chi.x, chi.y, (V *)nullptr));
+        if (FS) h = v_scale(h, orbit_sign(orbit, r.arg, raw));   // fermionic exchange sign
       }
       const int64_t idx = locate(index, r.rep);
       if (idx >= 0) {
@@ -746,7 +749,7 @@ __global__ void __launch_bounds__(kThreads) k_pull(const KernelParams p) {
       } else if (v_nonzero(h)) {
         bool fatal = true;
         if (!orbit.trivial_characters)
-          fatal = orbit_stabiliser_sum(orbit, r.rep) > 1e-12 * (double)orbit.group_order;
+          fatal = orbit_stabiliser_sum<FS>(orbit, r.rep) > 1e-12 * (double)orbit.group_order;
         if (fatal && atomicAdd(p.status, 1ull) == 0) p.status[1] = r.rep;
       }
     }
@@ -1804,7 +1807,7 @@ __global__ void k_mph_slots(const uint64_t *__restrict__ keys, int64_t n, Perfec
 
 // localProcess for records that arrived from other ranks: already projected and hashed by the sender.
 // Two records per thread with their searches advanced in lock step (see locate2).
-template <int PROJ, bool CV, bool CE>
+template <int PROJ, bool CV, bool CE, bool FS>
 __global__ void __launch_bounds__(kThreads) k_accumulate(const KernelParams p, int64_t count,
                                                          const uint64_t *__restrict__ betas,
                                                          const double *__restrict__ coeffs) {
@@ -1819,8 +1822,8 @@ __global__ void __launch_bounds__(kThreads) k_accumulate(const KernelParams p, i
     const V c1 = a1 ? __ldg(reinterpret_cast<const V *>(coeffs) + k1) : v_make(0.0, 0.0, (V *)nullptr);
     int64_t i0, i1;
     locate2(p.index, true, b0, a1, b1, i0, i1);
-    finish<PROJ, CV, CE>(p, p.orbit, true, b0, c0, i0);
-    finish<PROJ, CV, CE>(p, p.orbit, a1, b1, c1, i1);
+    finish<PROJ, CV, CE, FS>(p, p.orbit, true, b0, c0, i0);
+    finish<PROJ, CV, CE, FS>(p, p.orbit, a1, b1, c1, i1);
   }
 }
 
@@ -1907,7 +1910,7 @@ __global__ void k_locale_idx(int64_t count, const uint64_t *__restrict__ states,
 }
 
 // ls_hs_state_info (reference src/FFI.chpl:181-184): representative, conj(character), norm
-template <int PROJ>
+template <int PROJ, bool FS>
 __global__ void k_state_info(const OrbitProgram P, uint64_t site_mask, double inv_char, int64_t count,
                              const uint64_t *__restrict__ alphas, uint64_t *betas, double2 *characters,
                              double *norms) {
@@ -1930,7 +1933,8 @@ __global__ void k_state_info(const OrbitProgram P, uint64_t site_mask, double in
     double stab = (double)r.stab;
     if (!P.trivial_characters) {
       chi = P.characters[r.arg];
-      stab = orbit_stabiliser_sum(P, a);
+      if (FS) { const double sg = orbit_sign(P, r.arg, a); chi.x *= sg; chi.y *= sg; }
+      stab = orbit_stabiliser_sum<FS>(P, a);
     }
     characters[k] = make_double2(chi.x, -chi.y);
     const double nn = stab / (double)P.group_order;
@@ -1938,13 +1942,14 @@ __global__ void k_state_info(const OrbitProgram P, uint64_t site_mask, double in
   }
 }
 
+template <bool FS>
 __global__ void k_compute_norms(const OrbitProgram P, int64_t count, const uint64_t *__restrict__ reps,
                                 double *norms) {
   const int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= count) return;
   double stab;
   if (P.trivial_characters) stab = (double)orbit_scan<true, false>(P, reps[k]).stab;
-  else stab = orbit_stabiliser_sum(P, reps[k]);
+  else stab = orbit_stabiliser_sum<FS>(P, reps[k]);
   const double nn = stab / (double)P.group_order;
   norms[k] = nn > 1e-12 ? sqrt(nn) : 0.0;
 }
@@ -1959,7 +1964,7 @@ __device__ __forceinline__ uint64_t next_state_fixed_hamming(uint64_t v) {
 // this rank, is the minimum of its orbit and has non-zero norm (reference
 // src/StatesEnumeration.chpl:158-224).  Pass 0 counts, pass 1 writes at chunk_offset[c].
 // half_mask != 0 (spinful fermions): only candidates with popcount(v & half_mask) == half_weight are kept.
-template <int PROJ, bool WRITE>
+template <int PROJ, bool WRITE, bool FS>
 __global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed_hamming, uint64_t half_mask,
                             int half_weight, int rank, int num_ranks, int64_t n_chunks,
                             const uint64_t *__restrict__ chunk_first,
@@ -1983,7 +1988,7 @@ __global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed
         const OrbitResult r = orbit_scan<true, true>(P, v);
         keep = (r.rep == v);
         if (keep) {
-          const double stab = P.trivial_characters ? (double)r.stab : orbit_stabiliser_sum(P, v);
+          const double stab = P.trivial_characters ? (double)r.stab : orbit_stabiliser_sum<FS>(P, v);
           const double nn = stab / (double)P.group_order;
           norm = nn > 1e-12 ? sqrt(nn) : 0.0;
           keep = norm > 0.0;
@@ -2000,15 +2005,17 @@ __global__ void k_enumerate(const OrbitProgram P, uint64_t site_mask, bool fixed
   if (!WRITE) chunk_count[c] = n;
 }
 
-// f(PROJ, CV, CE) as integral constants for the value kinds k_generate, k_pull and k_accumulate are built for: real
-// values and vectors, complex values with real or complex vectors
+// f(PROJ, CV, CE, FS) as integral constants for the value kinds k_generate, k_pull and k_accumulate are built for: real
+// values and vectors, complex values with real or complex vectors; FS (the fermionic exchange sign) with PROJ_GROUP only
 template <typename F>
-void with_values(Projection proj, bool complex_values, bool complex_elements, F &&f) {
+void with_values(Projection proj, bool complex_values, bool complex_elements, const OrbitProgram &orbit, F &&f) {
   if (complex_elements && !complex_values) throw std::runtime_error("complex vectors need complex values");
   with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
     with_bool(complex_values, [&](auto cv) {
       with_bool(complex_elements, [&](auto ce) {
-        if constexpr (cv() || !ce()) f(pj, cv, ce);
+        with_bool(pj() == PROJ_GROUP && orbit.fermionic != 0, [&](auto fs) {
+          if constexpr ((cv() || !ce()) && (pj() == PROJ_GROUP || !fs())) f(pj, cv, ce, fs);
+        });
       });
     });
   });
@@ -2202,9 +2209,9 @@ void launch_mph_slots(const uint64_t *keys, int64_t n, PerfectHash mph, const vo
 void launch_generate(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements, bool count_only,
                      cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
+  with_values(proj, complex_values, complex_elements, p.orbit, [&](auto pj, auto cv, auto ce, auto fs) {
     with_bool(count_only, [&](auto co) {
-      auto kernel = k_generate<pj(), cv(), ce(), co()>;
+      auto kernel = k_generate<pj(), cv(), ce(), co(), fs()>;
       const SmemLayout L = smem_layout(p, pj(), sizeof(typename ValT<cv()>::type));
       if (L.total > 40 * 1024)   // let several CTAs with large tables share the SM
         CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -2220,8 +2227,8 @@ void launch_generate(const KernelParams &p, Projection proj, bool complex_values
 
 void launch_pull(const KernelParams &p, Projection proj, bool complex_values, bool complex_elements, cudaStream_t stream) {
   if (p.row_end <= p.row_begin) return;
-  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
-    auto kernel = k_pull<pj(), cv(), ce()>;
+  with_values(proj, complex_values, complex_elements, p.orbit, [&](auto pj, auto cv, auto ce, auto fs) {
+    auto kernel = k_pull<pj(), cv(), ce(), fs()>;
     const SmemLayout L = smem_layout(p, pj(), sizeof(typename ValT<cv()>::type));
     const int grid = one_wave(kernel, ((p.row_end - p.row_begin + 31) / 32 + kWarps - 1) / kWarps, L.total);
     kernel<<<grid, kThreads, L.total, stream>>>(p);
@@ -2233,8 +2240,8 @@ void launch_accumulate(const KernelParams &p, Projection proj, bool complex_valu
                        const uint64_t *betas, const double *coeffs, cudaStream_t stream) {
   if (count <= 0) return;
   const int blocks = capped_grid(((count + 1) / 2 + kThreads - 1) / kThreads, (int64_t)sm_count() * 8);
-  with_values(proj, complex_values, complex_elements, [&](auto pj, auto cv, auto ce) {
-    k_accumulate<pj(), cv(), ce()><<<blocks, kThreads, 0, stream>>>(p, count, betas, coeffs);
+  with_values(proj, complex_values, complex_elements, p.orbit, [&](auto pj, auto cv, auto ce, auto fs) {
+    k_accumulate<pj(), cv(), ce(), fs()><<<blocks, kThreads, 0, stream>>>(p, count, betas, coeffs);
     check_launch("k_accumulate");
   });
 }
@@ -2295,7 +2302,10 @@ void launch_state_info(const OrbitProgram &P, Projection proj, uint64_t site_mas
   const unsigned blocks = (unsigned)((count + 127) / 128);
   double2 *ch = reinterpret_cast<double2 *>(characters);
   with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
-    k_state_info<pj()><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms);
+    with_bool(pj() == PROJ_GROUP && P.fermionic != 0, [&](auto fs) {
+      if constexpr (pj() == PROJ_GROUP || !fs())
+        k_state_info<pj(), fs()><<<blocks, 128, 0, stream>>>(P, site_mask, inv_char, count, alphas, betas, ch, norms);
+    });
   });
   check_launch("k_state_info");
 }
@@ -2303,7 +2313,9 @@ void launch_state_info(const OrbitProgram &P, Projection proj, uint64_t site_mas
 void launch_compute_norms(const OrbitProgram &P, int64_t count, const uint64_t *reps, double *norms,
                           cudaStream_t stream) {
   if (count <= 0) return;
-  k_compute_norms<<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(P, count, reps, norms);
+  with_bool(P.fermionic != 0, [&](auto fs) {
+    k_compute_norms<fs()><<<(unsigned)((count + 127) / 128), 128, 0, stream>>>(P, count, reps, norms);
+  });
   check_launch("k_compute_norms");
 }
 
@@ -2317,10 +2329,12 @@ void launch_enumerate(const OrbitProgram &P, Projection proj, uint64_t site_mask
   const unsigned blocks = (unsigned)((n_chunks + 127) / 128);
   with_choice<PROJ_NONE, PROJ_INVERSION, PROJ_GROUP>(proj, [&](auto pj) {
     with_bool(write_pass, [&](auto write) {
-      k_enumerate<pj(), write()><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, half_mask, half_weight, rank,
-                                                             num_ranks, n_chunks,
-                                                             chunk_first, chunk_last, chunk_count, chunk_offset, out,
-                                                             out_norms);
+      with_bool(pj() == PROJ_GROUP && P.fermionic != 0, [&](auto fs) {
+        if constexpr (pj() == PROJ_GROUP || !fs())
+          k_enumerate<pj(), write(), fs()><<<blocks, 128, 0, stream>>>(P, site_mask, fixed_hamming, half_mask, half_weight,
+                                                                       rank, num_ranks, n_chunks, chunk_first, chunk_last,
+                                                                       chunk_count, chunk_offset, out, out_norms);
+      });
     });
   });
   check_launch("k_enumerate");

@@ -250,6 +250,40 @@ def benes_masks(perm: np.ndarray, width: int = 64) -> list[tuple[int, int]]:
     return stages
 
 
+def widen_to_spinful(group: SymmetryGroup) -> SymmetryGroup:
+    """The group of site permutations p of a spinful-fermion basis as bit permutations: p[N + i] = N + p[i]."""
+    n = group.number_sites
+    return SymmetryGroup(number_sites=2 * n, perms=np.concatenate([group.perms, group.perms + n], axis=1).astype(np.int32),
+                         flips=group.flips, characters=group.characters, spin_inversion=group.spin_inversion,
+                         has_permutations=group.has_permutations)
+
+
+def inversion_masks(perm: np.ndarray) -> np.ndarray:
+    """Fermionic exchange sign of a bit permutation (result bit i = input bit perm[i]): bit j goes to image(j), the i
+    with perm[i] = j, and M[i] = { j < i : image(j) > image(i) }.  sign(g, s) = (-1)^(sum over set bits i of s of
+    popc(s & M[i])), the parity of the inversions of the images of the occupied modes.  -> uint64 [len(perm)]"""
+    n = len(perm)
+    image = np.empty(n, dtype=np.int64)
+    image[np.asarray(perm, dtype=np.int64)] = np.arange(n)
+    masks = np.zeros(n, dtype=np.uint64)
+    for i in range(n):
+        for j in range(i):
+            if image[j] > image[i]:
+                masks[i] |= np.uint64(1) << np.uint64(j)
+    return masks
+
+
+def fermion_signs(perm: np.ndarray, states: np.ndarray) -> np.ndarray:
+    """sign(g, s) in {+1, -1} for an array of uint64 states, from inversion_masks (host mirror of the device's)."""
+    states = np.asarray(states, dtype=np.uint64)
+    parity = np.zeros(states.shape, dtype=np.uint64)
+    one = np.uint64(1)
+    for i, m in enumerate(inversion_masks(perm)):
+        occupied = (states >> np.uint64(i)) & one
+        parity ^= occupied & (np.bitwise_count(states & m).astype(np.uint64) & one)
+    return np.where(parity == 0, 1, -1).astype(np.int8)
+
+
 def apply_permutation_numpy(perm: np.ndarray, states: np.ndarray) -> np.ndarray:
     """(g.s)[i] = s[perm[i]] for an array of uint64 states (host helper for tests)."""
     out = np.zeros_like(states)

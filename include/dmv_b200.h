@@ -75,12 +75,22 @@ int dmv_context_create(const dmv_basis_desc *basis, const dmv_operator_desc *op,
  *   DMV_SPINFUL_FERMION    N = number_sites / 2 sites: bit i = up occupation of site i, bit N + i = down occupation, so a
  *                          state is (down << N) | up; number_particles and number_up are both fixed, and the basis is
  *                          every state with number_up up and number_particles - number_up down particles
- * For fermions basis->hamming_weight must equal number_particles (the weight over all bits).  Refused before anything
- * is allocated: permutations or spin inversion with fermions; an odd bit count for spinful fermions; number_up outside
- * 0..N or number_particles - number_up outside 0..N; a spinless number_particles outside -1..number_sites.
+ * For fermions basis->hamming_weight must equal number_particles (the weight over all bits).
+ * Lattice symmetries (has_permutations): perms are permutations of the bits (output bit i takes input bit perms[i]),
+ * every flip is 0, and on a spinful basis each element is one site permutation p acting on both halves,
+ * perms[N + i] = N + p[i].  The element g acts as U_g c†_{perms[i]} U_g^-1 = c†_i, so a state |s> = c†_{a1} ... c†_{ak}|0>
+ * (a1 < ... < ak) goes to sign(g, s)|g(s)>, sign(g, s) = (-1)^(inversions of the images of a1 .. ak), and the character
+ * of an orbit element is chi(g) sign(g, s) everywhere: representatives, norms (orbits whose signed stabiliser sum
+ * vanishes are not basis states), dmv_state_info and the products (push and queued pull; k_rows does not take them).
+ * Refused before anything is allocated: spin inversion with fermions; permutations without the group tables, with a
+ * non-zero flip, or (spinful) not acting on both halves as one site permutation; an odd bit count for spinful fermions;
+ * number_up outside 0..N or number_particles - number_up outside 0..N; a spinless number_particles outside
+ * -1..number_sites.
  * On a fermionic context dmv_pm_correlations, dmv_apply_spin and dmv_reduced_density_matrix refuse (they assume spin
- * operators without strings); dmv_zz_correlations gives <(2n_a - 1)(2n_b - 1)> over the bits; dmv_one_body_density_matrix
- * and dmv_apply_fermion (below) are the single-particle observables, and refuse a spin context.
+ * operators without strings); dmv_zz_correlations gives <(2n_a - 1)(2n_b - 1)> over the bits (with permutations, averaged
+ * over the bit permutations of the group); dmv_one_body_density_matrix and dmv_apply_fermion (below) are the
+ * single-particle observables, and refuse a spin context and a fermionic context with permutations (their look-ups carry
+ * no exchange sign).
  * Info "particle_type" answers the constant below. */
 enum { DMV_SPIN = 0, DMV_SPINLESS_FERMION = 1, DMV_SPINFUL_FERMION = 2 };
 typedef struct {

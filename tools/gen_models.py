@@ -14,6 +14,9 @@ Usage:  python tools/gen_models.py REFERENCE_DATA_DIR [data]
 --fermions writes the fermionic models, which the reference's data directory does not have: hubbard_chain_8 (periodic
 chain of 8 sites) and hubbard_square_4x4 (4 x 4 torus), H = -t sum_<ij>,s (c+_is c_js + h.c.) + U sum_i n_i,up n_i,down
 with t = 1, U = 4 at half filling; and spinless_ring_28, H = -t sum_i (c+_i c_i+1 + h.c.) with t = 1 at 14 particles.
+Each also in one symmetry sector (site_symmetries): spinless_ring_28_symm (translations, momentum 0),
+hubbard_chain_8_symm (translations and the reflection i -> 7 - i, both sector 0) and hubbard_square_4x4_symm (the two
+torus translations, momentum (0, 0)).
 """
 import glob
 import os
@@ -86,10 +89,37 @@ def spinless_ring(n_sites, number_particles, t=1.0, name="spinless fermions on a
                 {"expression": f"-{t} × c†₀ c₁ - {t} × c†₁ c₀", "sites": _Flow(_Flow(b) for b in _bonds_ring(n_sites))}]}}
 
 
+def ring_translation(n):
+    return [(i + 1) % n for i in range(n)]
+
+
+def ring_reflection(n):
+    return [n - 1 - i for i in range(n)]
+
+
+def torus_translations(lx, ly):
+    """x -> x + 1 and y -> y + 1 on the sites i = x + lx y of _bonds_torus"""
+    return ([(x + 1) % lx + lx * y for y in range(ly) for x in range(lx)],
+            [x + lx * ((y + 1) % ly) for y in range(ly) for x in range(lx)])
+
+
+def with_site_symmetries(conf, permutations, sectors=None):
+    """conf with basis.site_symmetries = the permutations, in the given sectors (default 0)"""
+    sectors = [0] * len(permutations) if sectors is None else sectors
+    out = {"basis": dict(conf["basis"]), "hamiltonian": conf["hamiltonian"]}
+    out["basis"]["site_symmetries"] = [{"permutation": _Flow(p), "sector": int(k)} for p, k in zip(permutations, sectors)]
+    return out
+
+
 def fermion_models() -> dict:
     return {"hubbard_chain_8": hubbard(8, _bonds_ring(8)),
             "hubbard_square_4x4": hubbard(16, _bonds_torus(4, 4)),
-            "spinless_ring_28": spinless_ring(28, 14)}
+            "spinless_ring_28": spinless_ring(28, 14),
+            "spinless_ring_28_symm": with_site_symmetries(spinless_ring(28, 14), [ring_translation(28)]),
+            "hubbard_chain_8_symm": with_site_symmetries(hubbard(8, _bonds_ring(8)),
+                                                         [ring_translation(8), ring_reflection(8)]),
+            "hubbard_square_4x4_symm": with_site_symmetries(hubbard(16, _bonds_torus(4, 4)),
+                                                            list(torus_translations(4, 4)))}
 
 
 def write_fermion_models(dst):
